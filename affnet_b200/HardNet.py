@@ -1,4 +1,4 @@
-"""HardNet with the reference's interface (HardNet.py:61-101), executed by the sm_100a CUDA library:
+"""HardNet with the reference's interface (HardNet.py:61-101), executed by the sm_90a CUDA library:
 [n,1,32,32] -> L2-normalised [n,128].  `features.*` names match HardNet++.pth."""
 import torch
 import torch.nn as nn

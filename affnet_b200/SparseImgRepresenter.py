@@ -1,5 +1,5 @@
 """ScaleSpaceAffinePatchExtractor with the reference's interface (SparseImgRepresenter.py:14-209), executed by
-the sm_100a CUDA library: Gaussian pyramid -> fused Hessian/NMS/soft-argmax detection -> device-side selection ->
+the sm_90a CUDA library: Gaussian pyramid -> fused Hessian/NMS/soft-argmax detection -> device-side selection ->
 affine patch sampling -> AffNet -> shape filter -> (OriNet) -> denormalised LAFs.
 
 Differences from the reference that a caller can observe: nothing is printed; inputs must be CUDA tensors (there

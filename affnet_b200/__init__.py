@@ -1,4 +1,4 @@
-"""affnet_b200: B200-native (sm_100a) HesAffNet + HardNet detect-and-describe hot path.
+"""affnet_b200: H100-native (sm_90a) HesAffNet + HardNet detect-and-describe hot path.
 
 Drop-in mirror of the reference's Python entry points (ducha-aiki/affnet):
     from affnet_b200.SparseImgRepresenter import ScaleSpaceAffinePatchExtractor

@@ -1,6 +1,6 @@
-"""ctypes binding of the C ABI in include/affnet_b200.h (libaffnet_b200.so, sm_100a).
+"""ctypes binding of the C ABI in include/affnet_b200.h (libaffnet_b200.so, sm_90a).
 
-There is NO CPU / PyTorch fallback: if the shared library is missing or no sm_100 device is usable, every
+There is NO CPU / PyTorch fallback: if the shared library is missing or no sm_90 device is usable, every
 entry point raises.  PyTorch is used only to own device memory and streams.
 """
 import ctypes as C
@@ -107,7 +107,7 @@ _lib = None
 
 
 def build(verbose=False):
-    """Compile the CUDA sources for sm_100a into affnet_b200/lib (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA sources for sm_90a into affnet_b200/lib (nvcc cross-compiles without a GPU)."""
     r = subprocess.run(["bash", os.path.join(HERE, "csrc", "build.sh")], capture_output=True, text=True)
     if r.returncode != 0:
         raise AffnetB200Error("building libaffnet_b200.so failed:\n" + r.stdout + r.stderr)

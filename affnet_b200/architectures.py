@@ -1,5 +1,5 @@
 """AffNetFast / OriNetFast with the reference's interface (architectures.py:204-252, 33-82), executed by the
-sm_100a CUDA library.  Same constructor arguments, same `features.*` parameter names (checkpoints load
+sm_90a CUDA library.  Same constructor arguments, same `features.*` parameter names (checkpoints load
 unchanged), same outputs: AffNetFast -> rectified [n,2,2]; OriNetFast -> rotation [n,2,2] or angle [n]."""
 import torch
 import torch.nn as nn

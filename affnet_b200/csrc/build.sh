@@ -1,11 +1,11 @@
 #!/bin/bash
-# Builds affnet_b200/lib/libaffnet_b200.so for sm_100a (nvcc cross-compiles without a GPU).
+# Builds affnet_b200/lib/libaffnet_b200.so for sm_90a (H100; nvcc cross-compiles without a GPU).
 set -e
 HERE="$(cd "$(dirname "$0")" && pwd)"
 OUT="$HERE/../lib"
 mkdir -p "$OUT" "$HERE/obj"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS="${AG_EXTRA_FLAGS:-} -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xptxas -v"
+FLAGS="${AG_EXTRA_FLAGS:-} -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xptxas -v"
 pids=()
 for f in "$HERE"/*.cu; do
   o="$HERE/obj/$(basename "${f%.cu}").o"
@@ -19,17 +19,5 @@ done
 fail=0
 for p in "${pids[@]}"; do wait $p || fail=1; done
 if [ $fail = 1 ]; then echo "build failed" >&2; rm -f "$HERE"/obj/*.o.failed; for l in "$HERE"/obj/*.o.log; do grep -l "error" "$l" >/dev/null 2>&1 && rm -f "${l%.log}"; done; exit 1; fi
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o "$OUT/libaffnet_b200.so" "$HERE"/obj/*.o -lcudart
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -o "$OUT/libaffnet_b200.so" "$HERE"/obj/*.o -lcudart
 echo "built $OUT/libaffnet_b200.so"
-if [ "${AG_ROLE_PROF:-0}" = "1" ]; then mkdir -p "$HERE/obj_prof";   # developer build with the warp-role cycle counters of tc_first.cuh (scripts/role_prof.sh)
-  $NVCC $FLAGS -DAG_ROLE_PROF -c "$HERE/nets_tc.cu" -o "$HERE/obj_prof/nets_tc.o" > "$HERE/obj_prof/nets_tc.log" 2>&1 || { cat "$HERE/obj_prof/nets_tc.log"; exit 1; }
-  objs=$(ls "$HERE"/obj/*.o | grep -v nets_tc.o)
-  $NVCC -gencode arch=compute_100a,code=sm_100a -shared -o "$OUT/libaffnet_b200_prof.so" $objs "$HERE/obj_prof/nets_tc.o" -lcudart
-  echo "built $OUT/libaffnet_b200_prof.so"
-fi
-if [ "${AG_XPROF:-0}" = "1" ]; then mkdir -p "$HERE/obj_prof";   # developer build with the warp-role cycle counters of the second-generation engine (scripts/role_prof_x.py)
-  $NVCC $FLAGS -DAG_ROLE_PROF -c "$HERE/nets_tcx.cu" -o "$HERE/obj_prof/nets_tcx.o" > "$HERE/obj_prof/nets_tcx.log" 2>&1 || { cat "$HERE/obj_prof/nets_tcx.log"; exit 1; }
-  objs=$(ls "$HERE"/obj/*.o | grep -v nets_tcx.o)
-  $NVCC -gencode arch=compute_100a,code=sm_100a -shared -o "$OUT/libaffnet_b200_xprof.so" $objs "$HERE/obj_prof/nets_tcx.o" -lcudart
-  echo "built $OUT/libaffnet_b200_xprof.so"
-fi

@@ -1,4 +1,4 @@
-// Shared helpers for the affnet_b200 CUDA library (sm_100a only).
+// Shared helpers for the affnet_b200 CUDA library (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -71,7 +71,7 @@ __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? l
 
 // Block-wide bitonic sort (descending) of n = 2^k 64-bit keys in shared memory, optionally with an int payload.  Every thread owns whole
 // compare-exchange PAIRS (pair p -> elements i = p with a 0 bit inserted at log2(j), i | j), so no thread idles on the "ixj > i" half:
-// half the loop trips of the textbook form (select_kernel: 163 -> ~95 us for 4096 keys on 1024 threads).
+// half the loop trips of the textbook form.
 template <bool HAS_IDX>
 __device__ __forceinline__ void bitonic_sort_desc(unsigned long long* key, int* idx, int n) {
     for (int k2 = 2; k2 <= n; k2 <<= 1)

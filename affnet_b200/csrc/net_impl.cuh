@@ -8,9 +8,9 @@
 #include "common.cuh"
 
 #define AG_ENGINE_SIMT 0  /* exact fp32 direct convolution */
-#define AG_ENGINE_TC 1    /* tcgen05: fp16 operands, fp32 accumulate in TMEM, heads as tensor-core GEMMs; AffNet / OriNet with fp16 residual planes of weights and activations (fp32-grade), HardNet plain fp16 */
-#define AG_ENGINE_TC_EXACT 2 /* tcgen05 trunk with fp16 residual planes of weights AND activations, heads as fp32 FMA chains */
-#define AG_ENGINE_TC2 4      /* second-generation tcgen05 engine (tcx_*.cuh): kernel-row taps stacked along N, same numerics contract as engine 1 plus
+#define AG_ENGINE_TC 1    /* wgmma: fp16 operands, fp32 accumulate, heads as tensor-core GEMMs; AffNet / OriNet with fp16 residual planes of weights and activations (fp32-grade), HardNet plain fp16 */
+#define AG_ENGINE_TC_EXACT 2 /* tensor-core trunk with fp16 residual planes of weights AND activations, heads as fp32 FMA chains */
+#define AG_ENGINE_TC2 4      /* second-generation tensor-core engine (tcx_*.cuh): kernel-row taps stacked along N, same numerics contract as engine 1 plus
                                 HardNet weight residuals in layers 2-3 */
 #define AG_ENGINE_TC2_BF16 5 /* HardNet only: engine 4 with bf16 operands (BASELINE.json configs[4]); descriptors ~4e-3 of the fp32 reference */
 #define AG_ENGINE_TC_FAST 3  /* AffNet only: weight residuals but single fp16 activations (A error 2e-4: too coarse for the 1e-3 LAF contract once OriNet amplifies it, kept for A/B timing) */

@@ -1,17 +1,16 @@
 // Tensor-core engine of AffNet / OriNet / HardNet (replaces the conv stacks and heads of architectures.py:207-235 / 36-82 and
 // HardNet.py:67-101; BatchNorm folded, ReLU fused).  Per net:
-//   tc_first2_kernel    sampler + input_norm + conv1 + conv2 (tc_first.cuh), patches and layer-1 activations stay on the SM
-//   tc_conv_kernel      conv3 .. conv6 as shifted-window implicit GEMMs (tc_conv.cuh)
-//   tc_conv_pair_kernel HardNet conv5 / conv6 on CTA pairs, cta_group::2 (tc_pair.cuh)
+//   tc_conv_kernel<first>  sampler + input_norm + conv1 (fp32, CUDA cores) + conv2 (tensor cores); patches and layer-1
+//                          activations stay on the SM
+//   tc_conv_kernel         conv3 .. conv6 as shifted-window implicit GEMMs (tc_conv.cuh); HardNet's 128-channel layers as two
+//                          CTAs per patch, each computing half of the output channels
 //   tc_head_kernel / tc_headx_kernel   the 8x8 heads as GEMMs over 128-patch tiles (tc_head.cuh)
-// Numerics: fp16 operands with fp16 residual planes where a net needs them, fp32 accumulation in TMEM (DESIGN.md section 4).
+// Numerics: fp16 operands with fp16 residual planes where a net needs them, fp32 accumulation (DESIGN.md section 4).
 #include <vector>
 
 #include "net_impl.cuh"
 #include "tc_conv.cuh"
-#include "tc_first.cuh"
 #include "tc_head.cuh"
-#include "tc_pair.cuh"
 #include <stdlib.h>
 #include <string.h>
 
@@ -24,7 +23,7 @@ static int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_num_sms <= 0) g_num_sms = 148;
+        if (g_num_sms <= 0) g_num_sms = 132;
     }
     return g_num_sms;
 }
@@ -40,8 +39,7 @@ static int launch_tc(const __half* in, void* out, const __half* w, const float* 
         if (rc != AG_OK) return rc;
     }
     ConvArgs a;
-    a.in = in; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.prof_id = 0; a.n = n; a.group = group; a.count = count;
-    a.prof_id = (H == 32) ? (FIRST ? 0 : 2) : (H == 16 ? (STRIDE == 1 ? 3 : 4) : 5);
+    a.in = in; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.n = n; a.group = group; a.count = count;
     int gx = num_sms() / NSPLIT;
     if (gx > n) gx = n;
     if (gx < 1) gx = 1;
@@ -50,55 +48,6 @@ static int launch_tc(const __half* in, void* out, const __half* w, const float* 
     kern<<<dim3(gx, NSPLIT), Cfg::THREADS, Cfg::SMEM, st>>>(a, fs);
     AG_CHECK_LAUNCH(FIRST ? "tc_conv_kernel<first>" : "tc_conv_kernel");
     return AG_OK;
-}
-
-template <int C1, int COUT, int SA, int SW, int OSA>
-static int launch_first2(void* out, const __half* w, const float* b, float inv_scale, int n, int group, const int* count, cudaStream_t st, const FirstSrc& src) {
-    using Cfg = FirstCfg<C1, COUT, SA, SW, OSA>;
-    auto kern = tc_first2_kernel<C1, COUT, SA, SW, OSA>;
-    static SmemAttrOnce attr_once;
-    {
-        int rc = attr_once.ensure(kern, Cfg::SMEM, "tc_first2 smem attr");
-        if (rc != AG_OK) return rc;
-    }
-    ConvArgs a;
-    a.in = nullptr; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.prof_id = 0; a.n = n; a.group = group; a.count = count;
-    int gx = num_sms();
-    if (gx > n) gx = n;
-    if (gx < 1) gx = 1;
-    kern<<<gx, 448, Cfg::SMEM, st>>>(a, src);
-    AG_CHECK_LAUNCH("tc_first2_kernel");
-    return AG_OK;
-}
-
-// cta_group::2 launch: clusters of two CTAs, one patch per CTA (tc_pair.cuh)
-template <int CIN, int COUT, int H, int STRIDE, int STAGES, int OUT>
-static int launch_pair(const __half* in, void* out, const __half* w, const float* b, float inv_scale, int n, int group, const int* count, cudaStream_t st) {
-    using Cfg = PairCfg<CIN, COUT, H, STRIDE, STAGES, OUT>;
-    auto kern = tc_conv_pair_kernel<CIN, COUT, H, STRIDE, STAGES, OUT>;
-    static SmemAttrOnce attr_once;
-    {
-        int rc = attr_once.ensure(kern, Cfg::SMEM, "tc_conv_pair smem attr");
-        if (rc != AG_OK) return rc;
-    }
-    ConvArgs a;
-    a.in = in; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.prof_id = 0; a.n = n; a.group = group; a.count = count;
-    int pairs = num_sms() / 2;
-    if (pairs > (n + 1) / 2) pairs = (n + 1) / 2;
-    if (pairs < 1) pairs = 1;
-    kern<<<2 * pairs, 224, Cfg::SMEM, st>>>(a);
-    AG_CHECK_LAUNCH("tc_conv_pair_kernel");
-    return AG_OK;
-}
-
-static bool no_pair() {
-    static const bool v = getenv("AG_NO_PAIR") != nullptr;   // A/B switch: wide HardNet layers as two independent COUT halves
-    return v;
-}
-
-static bool first_simt() {
-    static const bool v = getenv("AG_FIRST_SIMT") != nullptr;   // A/B switch: layer 1 on CUDA cores inside the layer-2 kernel
-    return v;
 }
 
 }  // namespace tc
@@ -141,18 +90,11 @@ int tc_hardnet_forward(const ag_net* net, const tc::FirstSrc& src0, int n, int g
     FirstSrc src = src0;
     src.w1 = net->d_w1; src.b1 = net->d_b[0]; src.w1_inv = net->w_inv_scale[0]; src.w1_scale = 1.0f / net->w_inv_scale[0];
     int rc;
-    if (first_simt()) rc = launch_tc<32, 32, 32, 1, 1, 2, PHASE, 0, 0, 0, 1>(nullptr, B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, &src);
-    else rc = launch_first2<32, 32, 0, 0, 0>(B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, src);
-    if (rc) return rc;
+    if ((rc = launch_tc<32, 32, 32, 1, 1, 2, PHASE, 0, 0, 0, 1>(nullptr, B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, &src))) return rc;
     if ((rc = launch_tc<32, 64, 32, 2, 1, 2, PLAIN>(B, A, net->d_wh[2], net->d_b[2], net->w_inv_scale[2], n, group, count, st))) return rc;
     if ((rc = launch_tc<64, 64, 16, 1, 1, 2, PHASE>(A, B, net->d_wh[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
-    if (no_pair()) {
-        if ((rc = launch_tc<64, 128, 16, 2, 2, 2, PLAIN>(B, A, net->d_wh[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
-        if ((rc = launch_tc<128, 128, 8, 1, 2, 2, HEADL>(A, headbuf, net->d_wh[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st))) return rc;
-    } else {   // two SMs per MMA: every patch is read and multiplied once, each SM holds half of the weights
-        if ((rc = launch_pair<64, 128, 16, 2, 3, PLAIN>(B, A, net->d_wh[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
-        if ((rc = launch_pair<128, 128, 8, 1, 2, HEADL>(A, headbuf, net->d_wh[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st))) return rc;
-    }
+    if ((rc = launch_tc<64, 128, 16, 2, 2, 2, PLAIN>(B, A, net->d_wh[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
+    if ((rc = launch_tc<128, 128, 8, 1, 2, 2, HEADL>(A, headbuf, net->d_wh[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st))) return rc;
     return tc_hardnet_head(net, headbuf, n, group, count, out, st);
 }
 
@@ -165,8 +107,8 @@ int tc_hardnet_head(const ag_net* net, const void* headbuf, int n, int group, co
         if (rc == AG_OK) rc = once1.ensure(tc_head_kernel<1>, HEAD_SMEM, "tc_head smem attr");
         if (rc != AG_OK) return rc;
     }
-    if (bf16) tc_head_kernel<1><<<(n + 127) / 128, 192, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh_bf, net->d_head_b, out, n, group, count);
-    else tc_head_kernel<0><<<(n + 127) / 128, 192, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh, net->d_head_b, out, n, group, count);
+    if (bf16) tc_head_kernel<1><<<(n + 127) / 128, 288, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh_bf, net->d_head_b, out, n, group, count);
+    else tc_head_kernel<0><<<(n + 127) / 128, 288, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh, net->d_head_b, out, n, group, count);
     AG_CHECK_LAUNCH("tc_head_kernel");
     return AG_OK;
 }
@@ -180,8 +122,7 @@ int tc_trunk_affnet(const ag_net* net, const tc::FirstSrc& src0, int n, int grou
     FirstSrc src = src0;
     src.w1 = net->d_w1; src.b1 = net->d_b[0]; src.w1_inv = net->w_inv_scale[0]; src.w1_scale = 1.0f / net->w_inv_scale[0];
     int rc;
-    if (first_simt()) rc = launch_tc<16, 16, 32, 1, 1, 2, PHASE, 0, 1, 0, 1>(nullptr, B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, &src);
-    else rc = launch_first2<16, 16, 0, 1, 0>(B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, src);
+    rc = launch_tc<16, 16, 32, 1, 1, 2, PHASE, 0, 1, 0, 1>(nullptr, B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, &src);
     if (rc) return rc;
     if ((rc = launch_tc<16, 32, 32, 2, 1, 4, PLAIN, 0, 1, 0>(B, A, net->d_wh[2], net->d_b[2], net->w_inv_scale[2], n, group, count, st))) return rc;
     if ((rc = launch_tc<32, 32, 16, 1, 1, 6, PHASE, 0, 1, 0>(A, B, net->d_wh[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
@@ -200,8 +141,7 @@ int tc_trunk_orinet(const ag_net* net, const tc::FirstSrc& src0, int n, int grou
     FirstSrc src = src0;
     src.w1 = net->d_w1; src.b1 = net->d_b[0]; src.w1_inv = net->w_inv_scale[0]; src.w1_scale = 1.0f / net->w_inv_scale[0];
     int rc;
-    if (first_simt()) rc = launch_tc<16, 16, 32, 1, 1, 2, PHASE, 1, 1, 1, 1>(nullptr, B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, &src);
-    else rc = launch_first2<16, 16, 1, 1, 1>(B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, src);
+    rc = launch_tc<16, 16, 32, 1, 1, 2, PHASE, 1, 1, 1, 1>(nullptr, B, net->d_wh[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, &src);
     if (rc) return rc;
     if ((rc = launch_tc<16, 32, 32, 2, 1, 2, PLAIN, 1, 1, 1>(B, A, net->d_wh[2], net->d_b[2], net->w_inv_scale[2], n, group, count, st))) return rc;
     if ((rc = launch_tc<32, 32, 16, 1, 1, 3, PHASE, 1, 1, 1>(A, B, net->d_wh[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
@@ -221,8 +161,8 @@ int tc_headx_forward(const ag_net* net, const void* feat, int n, int group, cons
         if (rc != AG_OK) return rc;
     }
     const int tiles = (n + 127) / 128;
-    if (net->kind == AG_NET_AFFNET) tc_headx_kernel<0><<<tiles, 192, HX_SMEM, st>>>((const __half*)feat, net->d_headh, net->d_head_b, net->head_inv_scale, out, nullptr, raw, n, group, count);
-    else tc_headx_kernel<1><<<tiles, 192, HX_SMEM, st>>>((const __half*)feat, net->d_headh, net->d_head_b, net->head_inv_scale, out, angle, raw, n, group, count);
+    if (net->kind == AG_NET_AFFNET) tc_headx_kernel<0><<<tiles, 288, HX_SMEM, st>>>((const __half*)feat, net->d_headh, net->d_head_b, net->head_inv_scale, out, nullptr, raw, n, group, count);
+    else tc_headx_kernel<1><<<tiles, 288, HX_SMEM, st>>>((const __half*)feat, net->d_headh, net->d_head_b, net->head_inv_scale, out, angle, raw, n, group, count);
     AG_CHECK_LAUNCH("tc_headx_kernel");
     return AG_OK;
 }
@@ -234,12 +174,3 @@ int tc_nsplit(int kind, int layer) { return (kind == AG_NET_HARDNET && layer >= 
 int tc_split_w(int kind) { return kind == AG_NET_HARDNET ? 0 : 1; }
 
 }  // namespace ag
-
-#ifdef AG_ROLE_PROF
-// developer-only: per-CTA role cycle counters of the last tc_first2_kernel launch (tc_first.cuh)
-extern "C" int ag_debug_role_prof(unsigned long long* out) {
-    if (cudaMemcpyFromSymbol(out, ag::tc::g_role_prof, sizeof(unsigned long long) * 8 * 160 * 20) != cudaSuccess) return 1;
-    void* p = nullptr;
-    return (cudaGetSymbolAddress(&p, ag::tc::g_role_prof) == cudaSuccess && cudaMemset(p, 0, sizeof(unsigned long long) * 8 * 160 * 20) == cudaSuccess) ? 0 : 1;
-}
-#endif

@@ -4,8 +4,8 @@
 // tc_head.cuh (same head-operand layout).  Per net:  tcx_first_kernel (sampler + input_norm + conv1 + conv2)  ->  tcx_conv_kernel x4.
 // Numerics: AffNet / OriNet with fp16 residual planes of weights and activations in every layer (three MMAs per K step, fp32-grade);
 // HardNet fp16 activations, weights with their fp16 residual in layers 2 and 3 (emulation on the 2000 graf patches: plain fp16 weights give a
-// descriptor error of 1.1e-3, dominated by the weight rounding of the early layers; measured on the GPU with the residuals of layers 2-3:
-// <= 4.9e-4 end to end over every parity configuration; adding layer 4's residual buys 0.5e-4 for 0.29 ms per step, layer 3's is free: HBM bound).
+// descriptor error of 1.1e-3, dominated by the weight rounding of the early layers; with the residuals of layers 2-3 the parity tests hold
+// the descriptors to 6e-4; adding layer 4's residual buys about 0.5e-4).
 #include <stdlib.h>
 #include <string.h>
 
@@ -26,7 +26,7 @@ static int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
@@ -41,16 +41,15 @@ static int ensure_smem_attr(const void* func, int bytes, bool* configured, const
     return rc;
 }
 
-template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int EW, int BF = 0, int MC = 0>
+template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int BF = 0, int MC = 0>
 static int launch_conv(const void* in, void* out, const __half* w, const float* b, float inv_scale, int n, int group, const int* count, cudaStream_t st) {
-    constexpr int prof_id = (H == 32) ? 2 : (H == 16 ? (STRIDE == 1 ? 3 : 4) : 5);
-    using Cfg = XCfg<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA, EW>;
-    auto kern = tcx_conv_kernel<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA, EW, BF, MC>;
+    using Cfg = XCfg<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA>;
+    auto kern = tcx_conv_kernel<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA, BF, MC>;
     static bool configured[64] = {};   // per device (the attribute is per device)
     int rc = ensure_smem_attr((const void*)kern, (int)Cfg::SMEM, configured, "tcx_conv smem attr");
     if (rc != AG_OK) return rc;
     XArgs a;
-    a.in = (const __half*)in; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.n = n; a.group = group; a.count = count; a.prof_id = prof_id;
+    a.in = (const __half*)in; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.n = n; a.group = group; a.count = count;
     const int units = Cfg::In::PAIR ? (n + 1) / 2 : n;
     int gx = num_sms() / NSPLIT;
     if (gx > units) gx = units;
@@ -79,7 +78,7 @@ static int launch_first(void* out, const __half* w, const float* b, float inv_sc
     int rc = ensure_smem_attr((const void*)kern, (int)Cfg::SMEM, configured, "tcx_first smem attr");
     if (rc != AG_OK) return rc;
     XArgs a;
-    a.in = nullptr; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.n = n; a.group = group; a.count = count; a.prof_id = 0;
+    a.in = nullptr; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.n = n; a.group = group; a.count = count;
     int gx = num_sms();
     if (gx > n) gx = n;
     if (gx < 1) gx = 1;
@@ -167,7 +166,7 @@ int tcx_nsplit(int kind, int layer) { return (kind == AG_NET_HARDNET && layer >=
 #define AG_HARD_SW3 1   // HardNet layer 3 / layer 4 weight residuals (A/B switches for the accuracy / time trade, see DESIGN.md)
 #endif
 #ifndef AG_HARD_SW4
-#define AG_HARD_SW4 0   // measured r02: without it the worst descriptor error over all parity configurations is 4.9e-4 (with: 4.4e-4) and layer 4 is 0.29 ms per step faster
+#define AG_HARD_SW4 0   // worst descriptor error over the parity configurations about 4.9e-4 without it, 4.4e-4 with it
 #endif
 int tcx_split_w(int kind, int layer) { return kind == AG_NET_HARDNET ? (layer == 1 ? AG_HARD_SW2 : layer == 2 ? AG_HARD_SW3 : layer == 3 ? AG_HARD_SW4 : 0) : 1; }
 int tcx_stride(int layer) { return (layer == 2 || layer == 4) ? 2 : 1; }
@@ -178,26 +177,17 @@ size_t tcx_act_bytes(int n) { return (size_t)(n + 1) * 65536; }
 // ---- trunks -------------------------------------------------------------------------------------------------------------------------
 // AffNet / OriNet (same shapes, own weights): features as fp16 hi + lo planes in the head-GEMM layout.  upto: stop after conv layer
 // `upto` (2..6; for the debug decode), 6 = whole trunk.
-// epilogue warps of AffNet / OriNet layers 3 and 4 (4 | 8)
-// cluster-multicast input of HardNet's channel-split layers: layer 5 0.38 -> 0.35 ms, layer 6 unchanged (kept off)
+// cluster-multicast input of HardNet's channel-split layers (the two CTAs of a patch read its input once from L2)
 #ifndef AG_HARD_MC5
 #define AG_HARD_MC5 1
 #endif
 #ifndef AG_HARD_MC6
 #define AG_HARD_MC6 0
 #endif
-#ifndef AG_HARD_EW4
-#define AG_HARD_EW4 16   // HardNet layer 4 (N = 192, two accumulator buffers): 16 epilogue warps = 2 tile sets x 2 column halves, 0.56 -> 0.49 ms
-#endif
-#ifndef AG_AFF_EW6
-#define AG_AFF_EW6 8
-#endif
-// Residual planes of layer 2's output (the largest activation, read by the HBM-bound layer 3) as bytes (1) or fp16 (0).  Measured
-// (tests/test_gpu_tcx.py, bench A/B): with byte planes AffNet's A stays at 4.5e-6 of the oracle and layer 3 goes from 0.80 to 0.69 ms per
-// step (the same in front of layer 5 made that layer slower, 0.37 -> 0.41 ms: not wired).  OFF by default: the application test with the
-// hand-crafted orientation (test_graf_1_to_6_application_counts[hcori]) then has one keypoint of 2996 whose frame differs from the
-// oracle's by more than its near-tie accounting allows (a pixel on a histogram-bin boundary, DESIGN.md section 8; the accounting would
-// have to cover that case before the switch can be on).  OriNet's angle error grows from
+// Residual planes of layer 2's output (the largest activation, read by the HBM-bound layer 3) as bytes (1) or fp16 (0).  With byte
+// planes AffNet's A stays at 4.5e-6 of the oracle and layer 3 reads less.  OFF by default: the application test with the hand-crafted
+// orientation (test_graf_1_to_6_application_counts[hcori]) then has one keypoint of 2996 whose frame differs from the oracle's by more
+// than its near-tie accounting allows (a pixel on a histogram-bin boundary, DESIGN.md section 8).  OriNet's angle error grows from
 // 3e-5 to 1.2e-4 rad with byte planes (its atan2 amplifies): off for OriNet as well.
 #ifndef AG_AFF_LO8
 #define AG_AFF_LO8 0
@@ -206,12 +196,6 @@ size_t tcx_act_bytes(int n) { return (size_t)(n + 1) * 65536; }
 #define AG_ORI_LO8 0
 #endif
 static inline int tcx_lox(const ag_net* net) { return ((net->kind == AG_NET_AFFNET) ? AG_AFF_LO8 : AG_ORI_LO8) ? 2 : 1; }
-#ifndef AG_AFF_EW3
-#define AG_AFF_EW3 4
-#endif
-#ifndef AG_AFF_EW4
-#define AG_AFF_EW4 8   // layer 4 waited for its 4-warp epilogue 23 % of the time: 0.72 -> 0.61 ms (AffNet), 0.48 -> 0.41 (OriNet); layer 3 is HBM bound (no change)
-#endif
 template <int LOX>
 static int trunk_affori_t(const ag_net* net, const tc::FirstSrc& src0, int n, int group, const int* count, void* bufA, void* bufB, void* feat,
                           cudaStream_t st, int upto) {
@@ -221,13 +205,13 @@ static int trunk_affori_t(const ag_net* net, const tc::FirstSrc& src0, int n, in
     int rc;
     if ((rc = launch_first<16, 16, 1, 1, LOX>(bufB, net->d_wx[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, src))) return rc;
     if (upto <= 2) return AG_OK;
-    if ((rc = launch_conv<16, 32, 32, 2, 1, 3, L_S1_16, LOX, 1, 1, AG_AFF_EW3>(bufB, bufA, net->d_wx[2], net->d_b[2], net->w_inv_scale[2], n, group, count, st))) return rc;
+    if ((rc = launch_conv<16, 32, 32, 2, 1, 3, L_S1_16, LOX, 1, 1>(bufB, bufA, net->d_wx[2], net->d_b[2], net->w_inv_scale[2], n, group, count, st))) return rc;
     if (upto <= 3) return AG_OK;
-    if ((rc = launch_conv<32, 32, 16, 1, 1, 4, L_S2_8P, 1, 1, 1, AG_AFF_EW4>(bufA, bufB, net->d_wx[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
+    if ((rc = launch_conv<32, 32, 16, 1, 1, 4, L_S2_8P, 1, 1, 1>(bufA, bufB, net->d_wx[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
     if (upto <= 4) return AG_OK;
-    if ((rc = launch_conv<32, 64, 16, 2, 1, 2, L_S1_8P, 1, 1, 1, 8>(bufB, bufA, net->d_wx[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
+    if ((rc = launch_conv<32, 64, 16, 2, 1, 2, L_S1_8P, 1, 1, 1>(bufB, bufA, net->d_wx[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
     if (upto <= 5) return AG_OK;
-    return launch_conv<64, 64, 8, 1, 1, 2, L_HEAD, 1, 1, 1, AG_AFF_EW6>(bufA, feat, net->d_wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
+    return launch_conv<64, 64, 8, 1, 1, 2, L_HEAD, 1, 1, 1>(bufA, feat, net->d_wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
 }
 int tcx_trunk_affori(const ag_net* net, const tc::FirstSrc& src0, int n, int group, const int* count, void* bufA, void* bufB, void* feat,
                      cudaStream_t st, int upto) {
@@ -245,13 +229,13 @@ static int trunk_hardnet_t(const ag_net* net, const tc::FirstSrc& src0, int n, i
     int rc;
     if ((rc = launch_first<32, 32, 0, AG_HARD_SW2, 0, BF>(bufB, wx[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, src))) return rc;
     if (upto <= 2) return AG_OK;
-    if ((rc = launch_conv<32, 64, 32, 2, 1, 2, L_S1_16, 0, AG_HARD_SW3, 0, 8, BF>(bufB, bufA, wx[2], net->d_b[2], net->w_inv_scale[2], n, group, count, st))) return rc;
+    if ((rc = launch_conv<32, 64, 32, 2, 1, 2, L_S1_16, 0, AG_HARD_SW3, 0, BF>(bufB, bufA, wx[2], net->d_b[2], net->w_inv_scale[2], n, group, count, st))) return rc;
     if (upto <= 3) return AG_OK;
-    if ((rc = launch_conv<64, 64, 16, 1, 1, 2, L_S2_8P, 0, AG_HARD_SW4, 0, AG_HARD_EW4, BF>(bufA, bufB, wx[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
+    if ((rc = launch_conv<64, 64, 16, 1, 1, 2, L_S2_8P, 0, AG_HARD_SW4, 0, BF>(bufA, bufB, wx[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
     if (upto <= 4) return AG_OK;
-    if ((rc = launch_conv<64, 128, 16, 2, 2, 2, L_S1_8P, 0, 0, 0, 8, BF, AG_HARD_MC5>(bufB, bufA, wx[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
+    if ((rc = launch_conv<64, 128, 16, 2, 2, 2, L_S1_8P, 0, 0, 0, BF, AG_HARD_MC5>(bufB, bufA, wx[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
     if (upto <= 5) return AG_OK;
-    return launch_conv<128, 128, 8, 1, 2, 2, L_HEAD, 0, 0, 0, 8, BF, AG_HARD_MC6>(bufA, headbuf, wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
+    return launch_conv<128, 128, 8, 1, 2, 2, L_HEAD, 0, 0, 0, BF, AG_HARD_MC6>(bufA, headbuf, wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
 }
 
 int tcx_trunk_hardnet(const ag_net* net, const tc::FirstSrc& src0, int n, int group, const int* count, void* bufA, void* bufB, void* headbuf,
@@ -294,12 +278,3 @@ int ag_debug_tcx_layer(const ag_net_t* net, const float* d_patches, int n, int u
 }
 
 }  // extern "C"
-
-#ifdef AG_ROLE_PROF
-// developer-only: per-CTA role cycle counters of the last second-generation launches (tcx_conv.cuh)
-extern "C" int ag_debug_role_prof_x(unsigned long long* out) {
-    if (cudaMemcpyFromSymbol(out, ag::tcx::g_xprof, sizeof(unsigned long long) * 8 * 160 * 20) != cudaSuccess) return 1;
-    void* p = nullptr;
-    return (cudaGetSymbolAddress(&p, ag::tcx::g_xprof) == cudaSuccess && cudaMemset(p, 0, sizeof(unsigned long long) * 8 * 160 * 20) == cudaSuccess) ? 0 : 1;
-}
-#endif

@@ -2,7 +2,7 @@
 // num_Baum_iters=1) + extract_patches_from_pyr (:181-188) + HardNet.forward for B images of one size, as a
 // fixed sequence of kernel launches on one stream with fixed-capacity buffers and device-side counters
 // (no host synchronisation, CUDA-graph capturable).  The reference processes one image at a time with
-// several .item()/nonzero host round trips (SURVEY.md §3); this is the B200-native replacement.
+// several .item()/nonzero host round trips (SURVEY.md §3); this is the on-device replacement.
 #include "common.cuh"
 
 struct ag_pipeline {

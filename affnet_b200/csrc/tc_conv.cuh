@@ -1,37 +1,24 @@
-// Tensor-core (tcgen05) 3x3 convolution engine for the AffNet / OriNet / HardNet trunks (sm_100a).
+// Tensor-core (wgmma) 3x3 convolution engine for the AffNet / OriNet / HardNet trunks (sm_90a).
 //
-// Formulation: shifted-window implicit GEMM.  The fp16 activations of one patch live in the UMMA canonical
-// no-swizzle K-major layout  [C/8][NPIX][8]  (8 channels = one 16-byte core-matrix row, pixel slots contiguous),
-// over a zero-padded pixel plane.  For tap (dy,dx) the A operand of the M=128 tile starting at output row m0 is
-// the SAME buffer with its descriptor start address advanced by (m0 + off(dy,dx)) * 16 bytes - no im2col copy.
-// Stride-2 layers read a phase-split plane (4 parity planes) so that they are shifted-window GEMMs too.
-//   D[128 x N] (fp32, TMEM) += A[128 x 16] (smem desc) * W[N x 16]^T (smem desc)      9 * C/16 MMAs per tile
+// Formulation: shifted-window implicit GEMM.  The fp16 activations of one patch live in the canonical no-swizzle K-major layout
+// [C/8][NPIX][8]  (8 channels = one 16-byte core-matrix row, pixel slots contiguous), over a zero-padded pixel plane.  For tap
+// (dy,dx) the A operand of the M=64 block starting at output row m0 is the SAME buffer with its descriptor start address advanced
+// by (m0 + off(dy,dx)) * 16 bytes - no im2col copy.  Stride-2 layers read a phase-split plane (4 parity planes) so that they are
+// shifted-window GEMMs too.
+//   D[64 x N] (fp32, registers) += A[64 x 16] (smem desc) * W[N x 16]^T (smem desc)      9 * C/16 MMAs per block
 // One persistent CTA keeps the layer's (BatchNorm-folded) weights resident in shared memory and loops over patches:
-//   warp 0   : producer  - one cp.async.bulk per patch (global -> smem stage), mbarrier complete_tx
-//   warp 1   : MMA issuer (single thread) + TMEM allocator
-//   warps 2-5: epilogue  - tcgen05.ld 32x32b, bias + ReLU, fp16 pack, 16-byte stores straight into the NEXT layer's
-//              canonical layout (or fp32 NCHW for the last trunk layer), plus the zero border of that layout.
+//   warps 0-7: two consumer warpgroups - warpgroup g takes the M=64 blocks g, g+2, ... of a patch: wgmma, then bias + ReLU,
+//              fp16 pack, stores straight into the NEXT layer's canonical layout (or fp32 NCHW for the last trunk layer), plus the
+//              zero border of that layout
+//   warp 8   : loader - one cp.async.bulk per channel group and patch (global -> smem stage), mbarrier complete_tx
 #pragma once
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace ag {
 namespace tc {
-
-// Developer-only role profiler (build with -DAG_ROLE_PROF, scripts/role_prof.sh): cycles every warp role spends in its loop and
-// waiting on each of its barriers, per CTA.  Compiled out of the product library.
-#ifdef AG_ROLE_PROF
-__device__ unsigned long long g_role_prof[8][160][20];   // [kernel slot: 0 tc_first2, l = conv layer l+1][CTA][role*5 + k]
-#define RP_DECL unsigned long long rp_t0 = clock64(), rp_w[4] = {0, 0, 0, 0}
-#define RP_WAIT(i, stmt) do { const unsigned long long rp_t = clock64(); stmt; rp_w[i] += clock64() - rp_t; } while (0)
-#define RP_STORE(slot, role) do { if (lane == 0 && (warp == 0 || warp == 1 || warp == 2 || warp == 6 || warp == 10)) { unsigned long long* d_ = g_role_prof[slot][blockIdx.x] + (role) * 5; \
-    d_[0] = clock64() - rp_t0; d_[1] = rp_w[0]; d_[2] = rp_w[1]; d_[3] = rp_w[2]; d_[4] = rp_w[3]; } } while (0)
-#else
-#define RP_DECL
-#define RP_WAIT(i, stmt) stmt
-#define RP_STORE(slot, role)
-#endif
 
 enum LayoutKind { PLAIN = 0, PHASE = 1, FINAL = 2, HEADL = 3 };  // HEADL: fp16 [patch/128][pixel*C/8 + c/8][patch%128][8], the A operand of the 8x8-head GEMM
 
@@ -41,16 +28,10 @@ struct InLay {
     static constexpr int HOUT = H / STRIDE;
     static constexpr int PITCH = (STRIDE == 1) ? H + 2 : H / 2 + 1;          // row pitch of the output-row index space
     static constexpr int ROWS = (HOUT - 1) * PITCH + HOUT;                    // output rows m = y*PITCH + x
-    static constexpr int TILES = (ROWS + 127) / 128;
-    // The last tile of a multi-tile plane is issued as an M = 64 MMA when it holds at most 64 live rows: half the A-operand read,
-    // which is what bounds these MMAs.  TMEM then keeps row i of that tile in lane (i % 16) + 32 * (i / 16).
-#ifndef AG_TAIL64
-#define AG_TAIL64 1
-#endif
-    static constexpr bool TAIL64 = AG_TAIL64 && TILES > 1 && (ROWS - 128 * (TILES - 1)) <= 64;
+    static constexpr int BLOCKS = (ROWS + 63) / 64;                           // M = 64 blocks of output rows
     static constexpr int PLANE = (STRIDE == 1) ? 0 : ((PITCH * PITCH + 7) / 8) * 8;   // parity-plane stride (slots)
     static constexpr int MAXOFF = (STRIDE == 1) ? 2 * PITCH + 2 : 3 * PLANE + PITCH + 1;
-    static constexpr int NPIX = ((128 * TILES + MAXOFF + 1 + 7) / 8) * 8;     // slots per channel group incl. slack
+    static constexpr int NPIX = ((64 * BLOCKS + MAXOFF + 1 + 7) / 8) * 8;     // slots per channel group incl. slack
     // slots that hold data (padded plane / four parity planes); the slack behind them only feeds accumulator rows that are never
     // stored, so loaders copy just this prefix of every channel group and leave whatever is in shared memory behind it
     static constexpr int USED = (STRIDE == 1) ? (H + 2) * (H + 2) : 3 * PLANE + PITCH * PITCH;
@@ -65,18 +46,11 @@ struct InLay {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// no-swizzle K-major UMMA shared-memory descriptor (cute::UMMA::SmemDescriptor, version 1)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
-}
-
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
-// AG_MBAR_HINT_NS > 0: try_wait carries a suspend-time hint, so a waiting warp sleeps in hardware until the phase completes (or the hint
-// expires) instead of re-issuing try_wait + branch every ~40 clk (ncu source view without the hint: the polling loops were 7.6 % of
-// tcx_first_kernel's and 16 % of a tcx_conv_kernel's issued instructions; step time -0.5 .. 1 %)
+// try_wait carries a suspend-time hint, so a waiting warp sleeps in hardware until the phase completes (or the hint expires)
+// instead of re-issuing try_wait + branch
 #ifndef AG_MBAR_HINT_NS
 #define AG_MBAR_HINT_NS 200000
 #endif
@@ -104,54 +78,15 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                  "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d), "l"(adesc),
-                 "l"(bdesc), "r"(idesc), "r"(accumulate)
-                 : "memory");
-}
-// Descriptor-lo form: the hi word of every no-swizzle descriptor here is the constant 0x4008 (SBO = 128 B, version 1), so the
-// issuer only does one integer add per operand.  ACC is a compile-time accumulate flag.
-constexpr uint32_t DESC_HI = 0x4008u;
-constexpr uint32_t M64_FIX = (uint32_t)((128 - 64) >> 4) << 24;   // subtract from an M = 128 instruction descriptor to get M = 64
+// named barrier of `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+
+// Shared-memory matrix descriptor of the no-swizzle K-major layout: core matrices of 8 rows x 16 bytes, rows 16 bytes apart, 8-row
+// groups SBO = 128 bytes apart (hi word), the two 16-byte K halves of a K = 16 step LBO bytes apart.  The lo word (start address and LBO
+// in 16-byte units) is what the issuing loops compute; the hi word is the constant SBO.
+constexpr uint32_t DESC_HI = 0x0008u;
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr, uint32_t lbo_bytes) { return ((saddr >> 4) & 0x3FFFu) | ((lbo_bytes >> 4) << 16); }
-template <int ACC>
-__device__ __forceinline__ void umma_f16_lo(uint32_t tmem_d, uint32_t alo, uint32_t blo, uint32_t idesc) {
-    asm volatile(
-        "{\n .reg .pred p;\n .reg .b64 da, db;\n setp.ne.u32 p, %4, 0;\n mov.b64 da, {%1, %5};\n mov.b64 db, {%2, %5};\n"
-        " tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n}\n" ::"r"(tmem_d),
-        "r"(alo), "r"(blo), "r"(idesc), "n"(ACC), "r"(DESC_HI)
-        : "memory");
-}
-__device__ __forceinline__ uint32_t elect_one() {
-    uint32_t pred = 0;
-    asm volatile("{\n .reg .pred P;\n elect.sync _|P, 0xffffffff;\n selp.u32 %0, 1, 0, P;\n}\n" : "=r"(pred));
-    return pred;
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-          "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ uint64_t desc64(uint32_t lo) { return ((uint64_t)DESC_HI << 32) | lo; }
 
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
@@ -183,7 +118,6 @@ struct ConvArgs {
     void* out;            // next layer's canonical fp16 buffer, or fp32 [n][COUT][HOUT][HOUT]
     const __half* wpk;    // [NSPLIT][9][CIN/8][hi rows | lo rows][8]: (1+SW)*COUT/NSPLIT rows per K chunk
     const float* bias;    // [COUT]
-    int prof_id;          // developer role profiler: slot of g_role_prof this launch reports to
     float inv_scale;      // wpk holds the weights times a power of two (fp16 residuals stay normal); accumulators are multiplied by its inverse
     int n, group;
     const int* count;
@@ -194,6 +128,8 @@ struct ConvArgs {
 // Split precision (fp32-grade results from fp16 tensor cores): SA = the input carries hi and lo fp16 planes
 // (x = hi + lo, channel groups [0,KC) hi then [KC,2KC) lo), SW = the weights carry hi and lo copies, OSA = write the
 // output as hi/lo planes.  D = A_hi W_hi (+ A_lo W_hi if SA) (+ A_hi W_lo if SW); the lo*lo term (2^-22) is dropped.
+// FIRST = 1: layer 1 (sampler + input_norm + conv3x3(1 -> CIN) + ReLU, fp32 on CUDA cores) runs in eight producer warps and
+// fills the stages of this layer.
 template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA = 0, int SW = 0, int OSA = 0, int FIRST = 0>
 struct ConvCfg {
     using In = InLay<H, STRIDE>;
@@ -201,15 +137,12 @@ struct ConvCfg {
     static constexpr int KC = CIN / 8;                  // 16-byte channel groups
     static constexpr int NT = COUT / NSPLIT;            // MMA N
     // With split weights the B operand stacks W_hi and W_lo along N (rows [0,NT) hi, [NT,2NT) lo of every K chunk): ONE MMA of
-    // N = 2*NT yields A*W_hi and A*W_lo side by side in TMEM and the epilogue adds the two halves.  The MMA is bound by the
-    // shared-memory read of its A operand (4 KB per 128x16 tile), so halving the MMA count halves the time.
-    static constexpr int ACCW = NT * (1 + SW);                      // accumulator width in TMEM columns
-    static constexpr int NACC = (512 / ACCW) < 8 ? (512 / ACCW) : 8;  // accumulator buffers: the issuer runs up to NACC tiles ahead
-    static constexpr int TMEM_COLS = (NACC * ACCW <= 32) ? 32 : (NACC * ACCW <= 64) ? 64 : (NACC * ACCW <= 128) ? 128 : (NACC * ACCW <= 256) ? 256 : 512;
+    // N = 2*NT yields A*W_hi and A*W_lo side by side and the epilogue adds the two halves.
+    static constexpr int ACCW = NT * (1 + SW);                      // accumulator width (columns)
     static constexpr uint32_t IN_BYTES = (uint32_t)KC * (1 + SA) * In::NPIX * 16;     // one patch
     static constexpr uint32_t W_HALF = 9u * KC * NT * 16;
     static constexpr uint32_t W_BYTES = W_HALF * (1 + SW);
-    static constexpr int THREADS = FIRST ? 448 : 192;   // FIRST adds 8 producer warps (sampler + input_norm + conv1)
+    static constexpr int THREADS = FIRST ? 544 : 288;   // 2 consumer warpgroups + loader (+ 8 producer warps for FIRST)
     static constexpr size_t FIRST_BYTES = FIRST ? (size_t)(2 * 34 * 36 + 9 * CIN + CIN + 64) * 4 : 0;
     static constexpr size_t SMEM = 1024 + (size_t)W_BYTES + (size_t)STAGES * IN_BYTES + FIRST_BYTES;
     // output buffer geometry
@@ -219,23 +152,20 @@ struct ConvCfg {
     static constexpr size_t OUT_BYTES = (OUT == FINAL) ? (size_t)COUT * HOUT * HOUT * 4
                                         : (OUT == HEADL) ? (size_t)COUT * HOUT * HOUT * 2
                                                          : (size_t)(COUT / 8) * (1 + OSA) * OUT_NPIX * 16;
-    static_assert(CIN % 16 == 0 && NT % 16 == 0 && NT <= 128 && ACCW <= 256, "UMMA shape / bias staging");
-    static_assert(2 * STAGES + 2 * NACC + 1 <= 60, "barrier area");
+    static_assert(CIN % 16 == 0 && NT % 16 == 0 && NT <= 128 && ACCW <= 256, "wgmma shape / bias staging");
+    static_assert(2 * STAGES + 1 <= 60, "barrier area");
     static_assert(SMEM <= 232448, "shared memory budget");
 };
 
 template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int FIRST>
-__global__ void __launch_bounds__(FIRST ? 448 : 192, 1) tc_conv_kernel(const ConvArgs a, const FirstSrc src) {
+__global__ void __launch_bounds__(FIRST ? 544 : 288, 1) tc_conv_kernel(const ConvArgs a, const FirstSrc src) {
     using Cfg = ConvCfg<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA, FIRST>;
     using In = typename Cfg::In;
-    constexpr int KC = Cfg::KC, NT = Cfg::NT, NACC = Cfg::NACC, TILES = In::TILES, HOUT = Cfg::HOUT;
+    constexpr int KC = Cfg::KC, NT = Cfg::NT, ACCW = Cfg::ACCW, BLOCKS = In::BLOCKS, HOUT = Cfg::HOUT;
     extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t* full = reinterpret_cast<uint64_t*>(smem);  // [STAGES]
     uint64_t* empty = full + STAGES;                       // [STAGES]
-    uint64_t* tfull = empty + STAGES;                      // [NACC]
-    uint64_t* tempty = tfull + NACC;                       // [NACC]
-    uint64_t* wbar = tempty + NACC;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wbar + 1);
+    uint64_t* wbar = empty + STAGES;
     float* s_bias = reinterpret_cast<float*>(smem + 512);  // [NT] (NT <= 128)
     unsigned char* sW = smem + 1024;
     unsigned char* sIn = sW + Cfg::W_BYTES;
@@ -245,33 +175,24 @@ __global__ void __launch_bounds__(FIRST ? 448 : 192, 1) tc_conv_kernel(const Con
 
     if (threadIdx.x < NT) s_bias[threadIdx.x] = a.bias[split * NT + threadIdx.x];
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], FIRST ? 256 : 1); mbar_init(&empty[s], 1); }
-        for (int i = 0; i < NACC; i++) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
+        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], FIRST ? 256 : 1); mbar_init(&empty[s], 2); }
         mbar_init(wbar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(Cfg::TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
     auto valid = [&](int pi) -> bool { return a.count == nullptr || (pi % a.group) < a.count[pi / a.group]; };
 
-    if (warp == 0) {
-        // ===== producer =====
+    if (warp == 8) {
+        // ===== loader =====
         if (lane == 0) {
             mbar_expect_tx(wbar, Cfg::W_BYTES);
             bulk_g2s(sW, reinterpret_cast<const unsigned char*>(a.wpk) + (size_t)split * Cfg::W_BYTES, Cfg::W_BYTES, wbar);
             int it = 0;
-            RP_DECL;
             for (int pi = blockIdx.x; pi < a.n && !FIRST; pi += gridDim.x) {
                 if (!valid(pi)) continue;
                 const int s = it % STAGES;
-                RP_WAIT(0, mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1));
+                mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
                 constexpr int G = KC * (1 + SA);
                 mbar_expect_tx(&full[s], (uint32_t)G * In::USED * 16u);
                 const unsigned char* gsrc = reinterpret_cast<const unsigned char*>(a.in) + (size_t)pi * Cfg::IN_BYTES;
@@ -280,67 +201,108 @@ __global__ void __launch_bounds__(FIRST ? 448 : 192, 1) tc_conv_kernel(const Con
                     bulk_g2s(sIn + (size_t)s * Cfg::IN_BYTES + (size_t)g * In::NPIX * 16, gsrc + (size_t)g * In::NPIX * 16, In::USED * 16u, &full[s]);
                 it++;
             }
-            RP_STORE(a.prof_id, 3);
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: the whole warp runs the (uniform) control flow, one elected lane issues =====
-        constexpr uint32_t idesc = (1u << 4) | ((uint32_t)(Cfg::ACCW >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);   // N = NT or 2*NT
-        constexpr uint32_t idesc_hi = (1u << 4) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);       // N = NT (hi rows only)
-        const uint32_t leader = elect_one();
+    } else if (warp < 8) {
+        // ===== consumers: warpgroup wg takes the M = 64 blocks wg, wg + 2, ... of every patch =====
+        const int wg = warp >> 2, wq = warp & 3;
+        const int et = threadIdx.x;   // 0..255
         mbar_wait(wbar, 0);
-        tc_fence_after();
-        const uint32_t w_lo = desc_lo(smem_u32(sW), Cfg::ACCW * 16u);
-        int it = 0, tcnt = 0;
-        RP_DECL;
+        const uint32_t w_lo = desc_lo(smem_u32(sW), ACCW * 16u);
+        int it = 0;
         for (int pi = blockIdx.x; pi < a.n; pi += gridDim.x) {
             if (!valid(pi)) continue;
             const int s = it % STAGES;
-            RP_WAIT(0, mbar_wait(&full[s], (it / STAGES) & 1));
-            tc_fence_after();
+            unsigned char* outp = reinterpret_cast<unsigned char*>(a.out) + (size_t)pi * Cfg::OUT_BYTES;
+            // zero border of the consumer's padded plane (each split its own channel groups)
+            if (OUT == PLAIN || OUT == PHASE) {
+                constexpr int HB = HOUT + 1;  // border cells: 4*HB
+                for (int i = et; i < 4 * HB; i += 256) {
+                    const int side = i / HB, k = i - side * HB;
+                    int Y, X;
+                    if (side == 0) { Y = 0; X = k; } else if (side == 1) { Y = HOUT + 1; X = k + 1; }
+                    else if (side == 2) { Y = k + 1; X = 0; } else { Y = k; X = HOUT + 1; }
+                    const int slot = (OUT == PLAIN) ? Cfg::OutP::slot(Y, X) : Cfg::OutS::slot(Y, X);
+#pragma unroll
+                    for (int g = 0; g < NT / 8; g++) {
+                        const int cg = split * (NT / 8) + g;
+                        *reinterpret_cast<uint4*>(outp + ((size_t)cg * Cfg::OUT_NPIX + slot) * 16) = make_uint4(0, 0, 0, 0);
+                        if (OSA) *reinterpret_cast<uint4*>(outp + ((size_t)(COUT / 8 + cg) * Cfg::OUT_NPIX + slot) * 16) = make_uint4(0, 0, 0, 0);
+                    }
+                }
+            }
+            mbar_wait(&full[s], (it / STAGES) & 1);
             const uint32_t in_lo = desc_lo(smem_u32(sIn + (size_t)s * Cfg::IN_BYTES), In::NPIX * 16u);
 #pragma unroll 1
-            for (int t = 0; t < TILES; t++, tcnt++) {
-                const int ab = tcnt % NACC;
-                RP_WAIT(1, mbar_wait(&tempty[ab], ((tcnt / NACC) & 1) ^ 1));
-                tc_fence_after();
-                if (leader) {
-                    const uint32_t d_tmem = tmem + (uint32_t)(ab * Cfg::ACCW);
-                    const uint32_t a_t = in_lo + (uint32_t)(t * 128);  // 16-byte units
-                    const uint32_t mfix = (In::TAIL64 && t == TILES - 1) ? M64_FIX : 0u;   // M = 128 -> 64 in the instruction descriptor
+            for (int b = wg; b < BLOCKS; b += 2) {
+                float d[ACCW / 2];
+                const uint32_t a_t = in_lo + (uint32_t)(b * 64);  // 16-byte units
+                wgmma_fence();
 #pragma unroll
-                    for (int tap = 0; tap < 9; tap++) {
+                for (int tap = 0; tap < 9; tap++) {
 #pragma unroll
-                        for (int j = 0; j < KC / 2; j++) {
-                            const uint32_t alo = a_t + (uint32_t)(In::tap_off(tap / 3, tap % 3) + 2 * j * In::NPIX);
-                            const uint32_t blo = w_lo + (uint32_t)((tap * KC + 2 * j) * Cfg::ACCW);
-                            if (tap == 0 && j == 0) umma_f16_lo<0>(d_tmem, alo, blo, idesc - mfix);               // A_hi * [W_hi ; W_lo]
-                            else umma_f16_lo<1>(d_tmem, alo, blo, idesc - mfix);
-                            if (SA) umma_f16_lo<1>(d_tmem, alo + (uint32_t)(KC * In::NPIX), blo, idesc_hi - mfix);   // A_lo * W_hi -> hi columns
+                    for (int j = 0; j < KC / 2; j++) {
+                        const uint32_t alo = a_t + (uint32_t)(In::tap_off(tap / 3, tap % 3) + 2 * j * In::NPIX);
+                        const uint32_t blo = w_lo + (uint32_t)((tap * KC + 2 * j) * ACCW);
+                        Wgmma<ACCW, 0>::mma(d, desc64(alo), desc64(blo), (tap | j) != 0);                           // A_hi * [W_hi ; W_lo]
+                        if (SA) Wgmma<NT, 0>::mma(d, desc64(alo + (uint32_t)(KC * In::NPIX)), desc64(blo), 1);     // A_lo * W_hi -> hi columns
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_reg_fence<ACCW / 2>(d);
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const int m = b * 64 + wq * 16 + (lane >> 2) + 8 * h;
+                    const int y = m / In::PITCH, x = m - y * In::PITCH;
+                    if (y >= HOUT || x >= HOUT) continue;
+#pragma unroll
+                    for (int j = 0; j < NT / 8; j++) {
+                        const int c = j * 8 + 2 * (lane & 3);    // this thread's channel pair of the block
+                        const int ch = split * NT + c;
+                        float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+                        if (SW) { v0 += d[4 * (j + NT / 8) + 2 * h]; v1 += d[4 * (j + NT / 8) + 2 * h + 1]; }
+                        v0 = fmaxf(fmaf(v0, a.inv_scale, s_bias[c]), 0.f);
+                        v1 = fmaxf(fmaf(v1, a.inv_scale, s_bias[c + 1]), 0.f);
+                        const uint32_t hi = pack_h2(v0, v1);
+                        const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                        const uint32_t lo = pack_h2(v0 - hf.x, v1 - hf.y);   // residual plane: lo = fp16(v - fp16(v))
+                        if (OUT == FINAL) {
+                            float* o = reinterpret_cast<float*>(outp);
+                            o[(size_t)ch * HOUT * HOUT + y * HOUT + x] = v0;
+                            o[(size_t)(ch + 1) * HOUT * HOUT + y * HOUT + x] = v1;
+                        } else if (OUT == HEADL) {
+                            const size_t kch = (size_t)(y * HOUT + x) * (COUT / 8) + ch / 8;
+                            unsigned char* hb = reinterpret_cast<unsigned char*>(a.out);
+                            const size_t off = (((size_t)(pi >> 7) * (HOUT * HOUT * COUT / 8) + kch) * 128 + (pi & 127)) * 16 + (ch & 7) * 2;
+                            *reinterpret_cast<uint32_t*>(hb + off) = hi;
+                            if (OSA) *reinterpret_cast<uint32_t*>(hb + (size_t)((a.n + 127) >> 7) * (HOUT * HOUT * COUT / 8) * 128 * 16 + off) = lo;   // behind the hi plane of all tiles
+                        } else {
+                            const int slot = (OUT == PLAIN) ? Cfg::OutP::slot(y + 1, x + 1) : Cfg::OutS::slot(y + 1, x + 1);
+                            *reinterpret_cast<uint32_t*>(outp + ((size_t)(ch / 8) * Cfg::OUT_NPIX + slot) * 16 + (ch & 7) * 2) = hi;
+                            if (OSA) *reinterpret_cast<uint32_t*>(outp + ((size_t)(COUT / 8 + ch / 8) * Cfg::OUT_NPIX + slot) * 16 + (ch & 7) * 2) = lo;
                         }
                     }
-                    umma_commit(&tfull[ab]);
                 }
-                __syncwarp();
             }
-            if (leader) umma_commit(&empty[s]);  // all MMAs reading this stage have completed when this arrives
-            __syncwarp();
+            bar_sync(3 + wg, 128);   // every warp of the warpgroup has finished its MMAs on this stage
+            if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[s]);
             it++;
         }
-        RP_STORE(a.prof_id, 0);
-    } else if (FIRST && warp >= 6) {
-        // ===== fused first layer: sampler (or patch load) -> input_norm -> conv3x3(1 -> CIN) + ReLU -> fp16 stage =====
+    } else if (FIRST) {
+        // ===== fused first layer (warps 9-16): sampler (or patch load) -> input_norm -> conv3x3(1 -> CIN) + ReLU -> fp16 stage =====
         static_assert(!FIRST || (H == 32 && STRIDE == 1), "the first conv layer feeds a stride-1 32x32 layer");
         float* s_patch = reinterpret_cast<float*>(sIn + (size_t)STAGES * Cfg::IN_BYTES);  // [2][34][36]
         float* s_w1 = s_patch + 2 * 34 * 36;                                               // [9][CIN]
         float* s_b1 = s_w1 + 9 * CIN;                                                      // [CIN]
         float* s_red = s_b1 + CIN;                                                         // [8][2] (+pad)
-        const int pt = threadIdx.x - 192;  // 0..255
+        const int pt = threadIdx.x - 288;  // 0..255
+        const int pw = warp - 9;
         for (int i = pt; i < 9 * CIN; i += 256) s_w1[i] = src.w1[i];
         if (pt < CIN) s_b1[pt] = src.b1[pt];
         for (int i = pt; i < 2 * 34 * 36; i += 256) s_patch[i] = 0.f;
         // the zero border / slack of the stages is written once: conv1 only ever writes interior slots
         for (int i = pt; i < (int)(STAGES * Cfg::IN_BYTES / 16); i += 256) reinterpret_cast<uint4*>(sIn)[i] = make_uint4(0, 0, 0, 0);
-        asm volatile("bar.sync 1, 256;" ::: "memory");
+        bar_sync(1, 256);
         // raw bilinear taps of the NEXT patch are requested before the conv of the current one so that their latency hides
         // behind compute (software prefetch): 16 values + the two fractional weights per pixel.
         float tp[4][4], fx[4], fy[4];
@@ -380,8 +342,8 @@ __global__ void __launch_bounds__(FIRST ? 448 : 192, 1) tc_conv_kernel(const Con
             // 2. input_norm statistics over the 256 producer threads
             float sm = (v4[0] + v4[1]) + (v4[2] + v4[3]);
             for (int o = 16; o > 0; o >>= 1) sm += __shfl_xor_sync(0xffffffffu, sm, o);
-            if (lane == 0) s_red[(warp - 6) * 2 + (it & 1) * 16] = sm;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
+            if (lane == 0) s_red[pw * 2 + (it & 1) * 16] = sm;
+            bar_sync(1, 256);
             sm = 0.f;
 #pragma unroll
             for (int i = 0; i < 8; i++) sm += s_red[i * 2 + (it & 1) * 16];
@@ -390,10 +352,10 @@ __global__ void __launch_bounds__(FIRST ? 448 : 192, 1) tc_conv_kernel(const Con
 #pragma unroll
             for (int k = 0; k < 4; k++) { const float d = v4[k] - mean; q = fmaf(d, d, q); }
             for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-            if (lane == 0) s_red[(warp - 6) * 2 + 1 + (it & 1) * 16] = q;
+            if (lane == 0) s_red[pw * 2 + 1 + (it & 1) * 16] = q;
 #pragma unroll
             for (int k = 0; k < 4; k++) { const int p = pt + k * 256; sp[((p >> 5) + 1) * 36 + (p & 31) + 1] = v4[k] - mean; }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
+            bar_sync(1, 256);
             q = 0.f;
 #pragma unroll
             for (int i = 0; i < 8; i++) q += s_red[i * 2 + 1 + (it & 1) * 16];
@@ -447,126 +409,6 @@ __global__ void __launch_bounds__(FIRST ? 448 : 192, 1) tc_conv_kernel(const Con
             it++;
             pi = pn;
         }
-    } else if (warp >= 2 && warp < 6) {
-        // ===== epilogue (warps 2..5 -> TMEM lane quadrant warp%4) =====
-        const int q = warp & 3;
-        const int et = (warp - 2) * 32 + lane;  // 0..127
-        int tcnt = 0;
-        RP_DECL;
-        for (int pi = blockIdx.x; pi < a.n; pi += gridDim.x) {
-            if (!valid(pi)) continue;
-            unsigned char* outp = reinterpret_cast<unsigned char*>(a.out) + (size_t)pi * Cfg::OUT_BYTES;
-            // zero border of the consumer's padded plane (only by the split that owns channel group range start)
-            if (OUT == PLAIN || OUT == PHASE) {
-                constexpr int HB = HOUT + 1;  // border cells: 4*HB
-                for (int i = et; i < 4 * HB; i += 128) {
-                    const int side = i / HB, k = i - side * HB;
-                    int Y, X;
-                    if (side == 0) { Y = 0; X = k; } else if (side == 1) { Y = HOUT + 1; X = k + 1; }
-                    else if (side == 2) { Y = k + 1; X = 0; } else { Y = k; X = HOUT + 1; }
-                    const int slot = (OUT == PLAIN) ? Cfg::OutP::slot(Y, X) : Cfg::OutS::slot(Y, X);
-#pragma unroll
-                    for (int g = 0; g < NT / 8; g++) {
-                        const int cg = split * (NT / 8) + g;
-                        *reinterpret_cast<uint4*>(outp + ((size_t)cg * Cfg::OUT_NPIX + slot) * 16) = make_uint4(0, 0, 0, 0);
-                        if (OSA) *reinterpret_cast<uint4*>(outp + ((size_t)(COUT / 8 + cg) * Cfg::OUT_NPIX + slot) * 16) = make_uint4(0, 0, 0, 0);
-                    }
-                }
-            }
-#pragma unroll 1
-            for (int t = 0; t < TILES; t++, tcnt++) {
-                const int ab = tcnt % NACC;
-                RP_WAIT(0, mbar_wait(&tfull[ab], (tcnt / NACC) & 1));
-                tc_fence_after();
-                const bool t64 = In::TAIL64 && t == TILES - 1;
-                const int m = t * 128 + (t64 ? q * 16 : q * 32) + lane;
-                const int y = m / In::PITCH, x = m - y * In::PITCH;
-                const bool ok = (y < HOUT) && (x < HOUT) && !(t64 && lane >= 16);
-                const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(ab * Cfg::ACCW);
-#pragma unroll
-                for (int c0 = 0; c0 < NT; c0 += 32) {
-                    uint32_t r[32];
-                    if (NT - c0 >= 32) {
-                        tmem_ld32(taddr + c0, r);
-                        if (SW) {   // add the A*W_lo half
-                            uint32_t r2[32];
-                            tmem_ld32(taddr + NT + c0, r2);
-                            tmem_ld_wait();
-#pragma unroll
-                            for (int i = 0; i < 32; i++) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r2[i]));
-                        }
-                    } else {
-                        uint32_t r16[16];
-                        tmem_ld16(taddr + c0, r16);
-#pragma unroll
-                        for (int i = 0; i < 16; i++) { r[i] = r16[i]; r[16 + i] = 0; }
-                        if (SW) {
-                            tmem_ld16(taddr + NT + c0, r16);
-                            tmem_ld_wait();
-#pragma unroll
-                            for (int i = 0; i < 16; i++) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r16[i]));
-                        }
-                    }
-                    tmem_ld_wait();
-                    if (c0 + 32 >= NT) {  // last column chunk read: release the accumulator buffer
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&tempty[ab]);
-                    }
-                    if (ok) {
-                        constexpr int NC = (NT < 32) ? NT : 32;
-#pragma unroll
-                        for (int g = 0; g < NC / 8; g++) {
-                            const int ch = split * NT + c0 + g * 8;
-                            float v[8];
-                            const float4 b0 = *reinterpret_cast<const float4*>(s_bias + c0 + g * 8), b1 = *reinterpret_cast<const float4*>(s_bias + c0 + g * 8 + 4);
-                            v[0] = fmaxf(fmaf(__uint_as_float(r[g * 8 + 0]), a.inv_scale, b0.x), 0.f); v[1] = fmaxf(fmaf(__uint_as_float(r[g * 8 + 1]), a.inv_scale, b0.y), 0.f);
-                            v[2] = fmaxf(fmaf(__uint_as_float(r[g * 8 + 2]), a.inv_scale, b0.z), 0.f); v[3] = fmaxf(fmaf(__uint_as_float(r[g * 8 + 3]), a.inv_scale, b0.w), 0.f);
-                            v[4] = fmaxf(fmaf(__uint_as_float(r[g * 8 + 4]), a.inv_scale, b1.x), 0.f); v[5] = fmaxf(fmaf(__uint_as_float(r[g * 8 + 5]), a.inv_scale, b1.y), 0.f);
-                            v[6] = fmaxf(fmaf(__uint_as_float(r[g * 8 + 6]), a.inv_scale, b1.z), 0.f); v[7] = fmaxf(fmaf(__uint_as_float(r[g * 8 + 7]), a.inv_scale, b1.w), 0.f);
-                            if (OUT == FINAL) {
-                                float* o = reinterpret_cast<float*>(outp);
-#pragma unroll
-                                for (int e = 0; e < 8; e++) o[(size_t)(ch + e) * HOUT * HOUT + y * HOUT + x] = v[e];
-                            } else if (OUT == HEADL) {
-                                uint4 pk;
-                                pk.x = pack_h2(v[0], v[1]); pk.y = pack_h2(v[2], v[3]); pk.z = pack_h2(v[4], v[5]); pk.w = pack_h2(v[6], v[7]);
-                                const size_t kch = (size_t)(y * HOUT + x) * (COUT / 8) + ch / 8;
-                                unsigned char* hb = reinterpret_cast<unsigned char*>(a.out);
-                                const size_t off = (((size_t)(pi >> 7) * (HOUT * HOUT * COUT / 8) + kch) * 128 + (pi & 127)) * 16;
-                                *reinterpret_cast<uint4*>(hb + off) = pk;
-                                if (OSA) {   // residual plane behind the hi plane of all ceil(n/128) tiles
-                                    float l[8];
-#pragma unroll
-                                    for (int e = 0; e < 8; e++) l[e] = v[e] - __half2float(__float2half_rn(v[e]));
-                                    pk.x = pack_h2(l[0], l[1]); pk.y = pack_h2(l[2], l[3]); pk.z = pack_h2(l[4], l[5]); pk.w = pack_h2(l[6], l[7]);
-                                    *reinterpret_cast<uint4*>(hb + (size_t)((a.n + 127) >> 7) * (HOUT * HOUT * COUT / 8) * 128 * 16 + off) = pk;
-                                }
-                            } else {
-                                const int slot = (OUT == PLAIN) ? Cfg::OutP::slot(y + 1, x + 1) : Cfg::OutS::slot(y + 1, x + 1);
-                                uint4 pk;
-                                pk.x = pack_h2(v[0], v[1]); pk.y = pack_h2(v[2], v[3]); pk.z = pack_h2(v[4], v[5]); pk.w = pack_h2(v[6], v[7]);
-                                *reinterpret_cast<uint4*>(outp + ((size_t)(ch / 8) * Cfg::OUT_NPIX + slot) * 16) = pk;
-                                if (OSA) {  // residual plane: lo = fp16(v - fp16(v))
-                                    float l[8];
-#pragma unroll
-                                    for (int e = 0; e < 8; e++) l[e] = v[e] - __half2float(__float2half_rn(v[e]));
-                                    pk.x = pack_h2(l[0], l[1]); pk.y = pack_h2(l[2], l[3]); pk.z = pack_h2(l[4], l[5]); pk.w = pack_h2(l[6], l[7]);
-                                    *reinterpret_cast<uint4*>(outp + ((size_t)(COUT / 8 + ch / 8) * Cfg::OUT_NPIX + slot) * 16) = pk;
-                                }
-                            }
-                        }
-                    }
-                }
-            }
-        }
-        RP_STORE(a.prof_id, 1);
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(Cfg::TMEM_COLS));
     }
 }
 

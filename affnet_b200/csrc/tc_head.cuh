@@ -1,8 +1,9 @@
 // HardNet 8x8 head on tensor cores: conv8x8(128->128, no bias) == GEMM [n, 8192] x [8192, 128], then BatchNorm and
 // L2 normalisation (HardNet.py:86-101, 12-19).  A = trunk features in the HEADL layout written by the last conv layer
 // ([patch/128][k/8][patch%128][8] fp16: 128 patches are the M rows of one tile), B = head weights [k/8][cout][8] fp16.
-// One CTA per 128-patch tile streams K in 64-wide stages (A 16 KiB + B 16 KiB per stage, bulk copies, 6-stage ring),
-// accumulates 128x128 fp32 in TMEM, and the epilogue thread of each row does BN + sum of squares + scale in registers.
+// One CTA per 128-patch tile streams K in 64-wide stages (A 16 KiB + B 16 KiB per stage, bulk copies, 6-stage ring); two
+// consumer warpgroups hold the 64 x 128 fp32 accumulators of their half of the tile in registers, and the quad of threads that
+// owns a row does BN + sum of squares + scale.
 #pragma once
 #include "tc_conv.cuh"
 
@@ -14,14 +15,12 @@ constexpr uint32_t HEAD_STAGE_A = (HEAD_KS / 8) * 128 * 16, HEAD_STAGE_B = (HEAD
 constexpr size_t HEAD_SMEM = 1024 + (size_t)HEAD_STAGES * (HEAD_STAGE_A + HEAD_STAGE_B);
 
 template <int BF>
-__global__ void __launch_bounds__(192, 1) tc_head_kernel(const __half* __restrict__ feat, const __half* __restrict__ wh,
+__global__ void __launch_bounds__(288, 1) tc_head_kernel(const __half* __restrict__ feat, const __half* __restrict__ wh,
                                                           const float* __restrict__ bn /*scale[128], shift[128]*/, float* __restrict__ out,
                                                           int n, int group, const int* __restrict__ count) {
     extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t* full = reinterpret_cast<uint64_t*>(smem);
     uint64_t* empty = full + HEAD_STAGES;
-    uint64_t* done = empty + HEAD_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
     unsigned char* sA = smem + 1024;
     unsigned char* sB = sA + (size_t)HEAD_STAGES * HEAD_STAGE_A;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -29,20 +28,12 @@ __global__ void __launch_bounds__(192, 1) tc_head_kernel(const __half* __restric
     constexpr int NK = HEAD_K / HEAD_KS;  // 128 stages
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < HEAD_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(done, 1);
+        for (int s = 0; s < HEAD_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(128));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             const unsigned char* ga = reinterpret_cast<const unsigned char*>(feat) + (size_t)tile * (HEAD_K / 8) * 128 * 16;
             const unsigned char* gb = reinterpret_cast<const unsigned char*>(wh);
@@ -54,69 +45,56 @@ __global__ void __launch_bounds__(192, 1) tc_head_kernel(const __half* __restric
                 bulk_g2s(sB + (size_t)s * HEAD_STAGE_B, gb + (size_t)k * HEAD_STAGE_B, HEAD_STAGE_B, &full[s]);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = (BF ? ((1u << 7) | (1u << 10)) : 0u) | (1u << 4) | ((uint32_t)(HEAD_N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);   // BF: bf16 operands
-            for (int k = 0; k < NK; k++) {
-                const int s = k % HEAD_STAGES;
-                mbar_wait(&full[s], (k / HEAD_STAGES) & 1);
-                tc_fence_after();
-                const uint32_t a0 = smem_u32(sA + (size_t)s * HEAD_STAGE_A), b0 = smem_u32(sB + (size_t)s * HEAD_STAGE_B);
-#pragma unroll
-                for (int j = 0; j < HEAD_KS / 16; j++) {
-                    const uint64_t da = make_desc(a0 + (uint32_t)(2 * j) * 128u * 16u, 128u * 16u, 128u);
-                    const uint64_t db = make_desc(b0 + (uint32_t)(2 * j) * HEAD_N * 16u, HEAD_N * 16u, 128u);
-                    umma_f16(tmem, da, db, idesc, (k | j) != 0);
-                }
-                umma_commit(&empty[s]);
-            }
-            umma_commit(done);
-        }
     } else {
-        const int q = warp & 3;
-        mbar_wait(done, 0);
-        tc_fence_after();
-        const int pi = tile * 128 + q * 32 + lane;
-        const bool ok = pi < n && (count == nullptr || (pi % group) < count[pi / group]);
-        const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16);
-        float ss = 0.f;
-        // pass 1: sum of squares of the BatchNorm-ed row; pass 2: reload, scale, store (keeps registers low)
-#pragma unroll 1
-        for (int c0 = 0; c0 < HEAD_N; c0 += 32) {
-            uint32_t r[32];
-            tmem_ld32(taddr + c0, r);
-            tmem_ld_wait();
+        const int wg = warp >> 2, wq = warp & 3;
+        float d[HEAD_N / 2];
+        // stage k's MMAs are issued before stage k-1's are waited for: the tensor core always has the next stage queued
+        for (int k = 0; k < NK; k++) {
+            const int s = k % HEAD_STAGES;
+            mbar_wait(&full[s], (k / HEAD_STAGES) & 1);
+            const uint32_t a0 = smem_u32(sA + (size_t)s * HEAD_STAGE_A) + wg * 64 * 16, b0 = smem_u32(sB + (size_t)s * HEAD_STAGE_B);
+            wgmma_fence();
 #pragma unroll
-            for (int e = 0; e < 32; e++) {
-                const float v = fmaf(__uint_as_float(r[e]), __ldg(bn + c0 + e), __ldg(bn + 128 + c0 + e));
-                ss = fmaf(v, v, ss);
+            for (int j = 0; j < HEAD_KS / 16; j++)
+                Wgmma<HEAD_N, BF>::mma(d, desc64(desc_lo(a0 + (uint32_t)(2 * j) * 128u * 16u, 128u * 16u)),
+                                       desc64(desc_lo(b0 + (uint32_t)(2 * j) * HEAD_N * 16u, HEAD_N * 16u)), (k | j) != 0);
+            wgmma_commit();
+            if (k > 0) {
+                wgmma_wait<1>();
+                bar_sync(3 + wg, 128);
+                if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[(k - 1) % HEAD_STAGES]);
             }
         }
-        const float inv = 1.0f / sqrtf(ss + 1e-8f);
-#pragma unroll 1
-        for (int c0 = 0; c0 < HEAD_N; c0 += 32) {
-            uint32_t r[32];
-            tmem_ld32(taddr + c0, r);
-            tmem_ld_wait();
-            if (ok) {
-                float4* o = reinterpret_cast<float4*>(out + (size_t)pi * 128 + c0);
+        wgmma_wait<0>();
+        wgmma_reg_fence<HEAD_N / 2>(d);
+        // rows r0 = 16 wq + lane/4 (h = 0) and r0 + 8 (h = 1) of this warpgroup's 64; columns 8 j + 2 (lane % 4) + e
 #pragma unroll
-                for (int e = 0; e < 32; e += 4) {
-                    float4 v;
-                    v.x = fmaf(__uint_as_float(r[e + 0]), __ldg(bn + c0 + e + 0), __ldg(bn + 128 + c0 + e + 0)) * inv;
-                    v.y = fmaf(__uint_as_float(r[e + 1]), __ldg(bn + c0 + e + 1), __ldg(bn + 128 + c0 + e + 1)) * inv;
-                    v.z = fmaf(__uint_as_float(r[e + 2]), __ldg(bn + c0 + e + 2), __ldg(bn + 128 + c0 + e + 2)) * inv;
-                    v.w = fmaf(__uint_as_float(r[e + 3]), __ldg(bn + c0 + e + 3), __ldg(bn + 128 + c0 + e + 3)) * inv;
-                    o[e / 4] = v;
+        for (int h = 0; h < 2; h++) {
+            const int pi = tile * 128 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+            const bool ok = pi < n && (count == nullptr || (pi % group) < count[pi / group]);
+            float ss = 0.f;
+#pragma unroll
+            for (int j = 0; j < HEAD_N / 8; j++) {
+                const int c = j * 8 + 2 * (lane & 3);
+                const float v0 = fmaf(d[4 * j + 2 * h], __ldg(bn + c), __ldg(bn + 128 + c));
+                const float v1 = fmaf(d[4 * j + 2 * h + 1], __ldg(bn + c + 1), __ldg(bn + 128 + c + 1));
+                ss = fmaf(v0, v0, ss);
+                ss = fmaf(v1, v1, ss);
+            }
+            ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+            ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+            const float inv = 1.0f / sqrtf(ss + 1e-8f);
+            if (ok) {
+#pragma unroll
+                for (int j = 0; j < HEAD_N / 8; j++) {
+                    const int c = j * 8 + 2 * (lane & 3);
+                    float2 v;
+                    v.x = fmaf(d[4 * j + 2 * h], __ldg(bn + c), __ldg(bn + 128 + c)) * inv;
+                    v.y = fmaf(d[4 * j + 2 * h + 1], __ldg(bn + c + 1), __ldg(bn + 128 + c + 1)) * inv;
+                    *reinterpret_cast<float2*>(out + (size_t)pi * 128 + c) = v;
                 }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128));
     }
 }
 
@@ -126,23 +104,21 @@ __global__ void __launch_bounds__(192, 1) tc_head_kernel(const __half* __restric
 // weights are stored as [k/8][W_hi rows 0..31 | W_lo rows 32..63][8], and per K step the issuer runs A_hi x [W_hi ; W_lo]
 // (N = 64) and A_lo x W_hi (N = 32); the epilogue adds the two accumulator halves and applies the reference's post-processing
 // (architectures.py:57-59,76-82,228-230; LAF.py:276-291).  One CTA per 128-patch tile, K streamed in 64-wide stages.
-// The tensor core adds into its fp32 accumulator with truncation, and the error grows with the length of the running sum (measured:
-// one accumulator over all 512 MMAs costs 2.3e-4 rad of OriNet angle against 2.6e-5 with an fp32 FMA chain).  The K stages
-// therefore rotate over HX_G = 8 accumulator column groups (all 512 TMEM columns) and the epilogue adds the groups in fp32.
-constexpr int HX_K = 4096, HX_NP = 32, HX_KS = 64, HX_STAGES = 5, HX_G = 8;
+// The tensor core adds into its fp32 accumulator with truncation, and the error grows with the length of the running sum (one
+// accumulator over all 512 MMAs costs about 2e-4 rad of OriNet angle against 2.6e-5 with an fp32 FMA chain).  Every K stage therefore
+// starts a fresh accumulator, and the stage sums are added in fp32 registers.
+constexpr int HX_K = 4096, HX_NP = 32, HX_KS = 64, HX_STAGES = 5;
 constexpr uint32_t HX_STAGE_A = (HX_KS / 8) * 128 * 16, HX_STAGE_B = (HX_KS / 8) * (2 * HX_NP) * 16;
 constexpr size_t HX_SMEM = 1024 + (size_t)HX_STAGES * (2 * HX_STAGE_A + HX_STAGE_B);
 constexpr size_t HX_PLANE_TILE = (size_t)(HX_K / 8) * 128 * 16;   // bytes of one 128-patch tile in one plane
 
 template <int KIND /* 0 AffNet, 1 OriNet */>
-__global__ void __launch_bounds__(192, 1) tc_headx_kernel(const __half* __restrict__ feat, const __half* __restrict__ wh, const float* __restrict__ bias,
+__global__ void __launch_bounds__(288, 1) tc_headx_kernel(const __half* __restrict__ feat, const __half* __restrict__ wh, const float* __restrict__ bias,
                                                            const float inv_scale, float* __restrict__ out, float* __restrict__ angle_out, float* __restrict__ raw_out, int n, int group,
                                                            const int* __restrict__ count) {
     extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t* full = reinterpret_cast<uint64_t*>(smem);
     uint64_t* empty = full + HX_STAGES;
-    uint64_t* done = empty + HX_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
     unsigned char* sA = smem + 1024;                                    // [stage][hi | lo]
     unsigned char* sB = sA + (size_t)HX_STAGES * 2 * HX_STAGE_A;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -158,20 +134,12 @@ __global__ void __launch_bounds__(192, 1) tc_headx_kernel(const __half* __restri
         if (!__syncthreads_or(live)) return;
     }
     if (threadIdx.x == 0) {
-        for (int s = 0; s < HX_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(done, 1);
+        for (int s = 0; s < HX_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(HX_G * 2 * HX_NP));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             const unsigned char* ga = reinterpret_cast<const unsigned char*>(feat) + (size_t)tile * HX_PLANE_TILE;
             const unsigned char* gl = ga + (size_t)tiles * HX_PLANE_TILE;
@@ -185,49 +153,46 @@ __global__ void __launch_bounds__(192, 1) tc_headx_kernel(const __half* __restri
                 bulk_g2s(sB + (size_t)s * HX_STAGE_B, gb + (size_t)k * HX_STAGE_B, HX_STAGE_B, &full[s]);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc_st = (1u << 4) | ((uint32_t)((2 * HX_NP) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            constexpr uint32_t idesc_hi = (1u << 4) | ((uint32_t)(HX_NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            for (int k = 0; k < NK; k++) {
-                const int s = k % HX_STAGES;
-                mbar_wait(&full[s], (k / HX_STAGES) & 1);
-                tc_fence_after();
-                const uint32_t a0 = smem_u32(sA + (size_t)s * 2 * HX_STAGE_A), b0 = smem_u32(sB + (size_t)s * HX_STAGE_B);
-#pragma unroll
-                for (int j = 0; j < HX_KS / 16; j++) {
-                    const uint64_t da = make_desc(a0 + (uint32_t)(2 * j) * 128u * 16u, 128u * 16u, 128u);
-                    const uint64_t dl = make_desc(a0 + HX_STAGE_A + (uint32_t)(2 * j) * 128u * 16u, 128u * 16u, 128u);
-                    const uint64_t db = make_desc(b0 + (uint32_t)(2 * j) * (2 * HX_NP) * 16u, (2 * HX_NP) * 16u, 128u);
-                    const uint32_t d = tmem + (uint32_t)((k % HX_G) * 2 * HX_NP);
-                    umma_f16(d, da, db, idesc_st, (k >= HX_G) || j != 0);   // A_hi x [W_hi ; W_lo]
-                    umma_f16(d, dl, db, idesc_hi, 1);                        // A_lo x W_hi -> hi columns
-                }
-                umma_commit(&empty[s]);
-            }
-            umma_commit(done);
-        }
     } else {
-        const int q = warp & 3;
-        mbar_wait(done, 0);
-        tc_fence_after();
-        const int pi = tile * 128 + q * 32 + lane;
-        const bool ok = pi < n && (count == nullptr || (pi % group) < count[pi / group]);
-        const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16);
-        constexpr int NO = KIND == 0 ? 3 : 18;
-        float acc[NO];
+        const int wg = warp >> 2, wq = warp & 3;
+        float tot[HX_NP], d[HX_NP];   // fragment of the N = 64 accumulator: columns [0, 32) = A_hi W_hi + A_lo W_hi, [32, 64) = A_hi W_lo
 #pragma unroll
-        for (int o = 0; o < NO; o++) acc[o] = 0.f;
-#pragma unroll 1
-        for (int g = 0; g < HX_G; g++) {
-            uint32_t r[32], r2[32];
-            tmem_ld32(taddr + g * 2 * HX_NP, r);
-            tmem_ld32(taddr + g * 2 * HX_NP + HX_NP, r2);
-            tmem_ld_wait();
+        for (int i = 0; i < HX_NP; i++) tot[i] = 0.f;
+        for (int k = 0; k < NK; k++) {
+            const int s = k % HX_STAGES;
+            mbar_wait(&full[s], (k / HX_STAGES) & 1);
+            const uint32_t a0 = smem_u32(sA + (size_t)s * 2 * HX_STAGE_A) + wg * 64 * 16, b0 = smem_u32(sB + (size_t)s * HX_STAGE_B);
+            wgmma_fence();
 #pragma unroll
-            for (int o = 0; o < NO; o++) acc[o] += __uint_as_float(r[o]) + __uint_as_float(r2[o]);
+            for (int j = 0; j < HX_KS / 16; j++) {
+                const uint64_t da = desc64(desc_lo(a0 + (uint32_t)(2 * j) * 128u * 16u, 128u * 16u));
+                const uint64_t dl = desc64(desc_lo(a0 + HX_STAGE_A + (uint32_t)(2 * j) * 128u * 16u, 128u * 16u));
+                const uint64_t db = desc64(desc_lo(b0 + (uint32_t)(2 * j) * (2 * HX_NP) * 16u, (2 * HX_NP) * 16u));
+                Wgmma<2 * HX_NP, 0>::mma(d, da, db, j != 0);   // A_hi x [W_hi ; W_lo]
+                Wgmma<HX_NP, 0>::mma(d, dl, db, 1);            // A_lo x W_hi -> hi columns
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_reg_fence<HX_NP>(d);
+            bar_sync(3 + wg, 128);
+            if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[s]);
+#pragma unroll
+            for (int i = 0; i < HX_NP; i++) tot[i] += d[i];
         }
-        if (ok) {
+        constexpr int NO = KIND == 0 ? 3 : 18;
+        // the quad of lanes that shares a row gathers the NO head outputs of that row: column o lives in lane 4 (lane / 4) + (o % 8) / 2,
+        // register 4 (o / 8) + 2 h + o % 2, its A_hi W_lo part 16 registers further (column o + 32)
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            float acc[NO];
+#pragma unroll
+            for (int o = 0; o < NO; o++) {
+                const int src_lane = (lane & ~3) | ((o & 7) >> 1), reg = 4 * (o >> 3) + 2 * h + (o & 1);
+                acc[o] = __shfl_sync(0xffffffffu, tot[reg] + tot[reg + 16], src_lane);
+            }
+            const int pi = tile * 128 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+            const bool ok = (lane & 3) == 0 && pi < n && (count == nullptr || (pi % group) < count[pi / group]);
+            if (!ok) continue;
             if (KIND == 0) {
                 const float s0 = acc[0] * inv_scale, s1 = acc[1] * inv_scale, s2 = acc[2 % NO] * inv_scale;
                 const float a00 = 1.0f + tanhf(s0 + bias[0]), a01 = 0.f, a10 = tanhf(s1 + bias[1]), a11 = 1.0f + tanhf(s2 + bias[2]);
@@ -257,12 +222,6 @@ __global__ void __launch_bounds__(192, 1) tc_headx_kernel(const __half* __restri
                 }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(HX_G * 2 * HX_NP));
     }
 }
 

@@ -2,18 +2,18 @@
 //
 //   sampler (LAF.py:313-372) -> input_norm (architectures.py:231-235) -> conv3x3(1 -> C1)+BN+ReLU -> conv3x3(C1 -> COUT)+BN+ReLU
 //
-// 32x32 patches and the layer-1 activations never exist in HBM.  Tiles are 128 consecutive pixels = 4 image rows of 32 (8 tiles per
-// patch, no padded columns).  Layer 1 (K = 9): the sliding-window plane P[y*32 + x] = {4 pixels of padded row y from column x | 4
-// pixels of padded row y+1} makes one M=128, K=16 MMA cover kernel rows 0 and 1, the same plane two rows further (descriptor
+// 32x32 patches and the layer-1 activations never exist in HBM.  M = 64 blocks are 64 consecutive pixels = 2 image rows of 32 (16
+// blocks per patch, no padded columns).  Layer 1 (K = 9): the sliding-window plane P[y*32 + x] = {4 pixels of padded row y from
+// column x | 4 pixels of padded row y+1} makes one K = 16 MMA cover kernel rows 0 and 1, the same plane two rows further (descriptor
 // leading-byte offset) kernel row 2.  Layer 2: for kernel row dy one MMA over the layer-1 stage advanced by dy rows with the three
-// taps of that row stacked along N (N = 3*COUT, or 6*COUT with the weight residual stacked behind when that still fits N = 96);
-// the epilogue shifts the dx = 0 / dx = 2 blocks by one pixel with warp shuffles (a warp = one image row).
+// taps of that row stacked along N (N = 3*COUT); the epilogue shifts the dx = 0 / dx = 2 blocks by one pixel with warp shuffles, and
+// through shared memory where an image row continues in the next warp (a warp holds 16 accumulator rows, half an image row).
 // Split precision: the input and layer-1 weights always carry fp16 residual planes; SA / SW / OSA as in tcx_conv.cuh.
 //
-// Warp roles (21 warps; 25 for 32-channel nets), ordered by the scheduler's priority (the SMSP arbiter prefers the highest warp id,
-// B300_MICROARCH.md): last warp MMA issuer (+ TMEM, weights) | the four below it layer-1 epilogue (TMEM -> bias/ReLU -> fp16 stage in
-// shared memory) | from warp 8 the layer-2 epilogue, NSET sets of four taking tiles in turn (TMEM -> shuffles -> bias/ReLU -> fp16 ->
-// global, stride-2 consumer layout) | 0-7 sampler + input_norm + P planes.
+// Warp roles (16 warps): 0-7 sampler + input_norm + P planes (two halves with their own barriers, so that the producers build one
+// half while the MMAs read the other) | 8-15 two consumer warpgroups: layer 1 of a patch (MMA, then bias/ReLU -> fp16 stage in shared
+// memory), then its layer 2 (MMA, then x shifts -> bias/ReLU -> fp16 -> global, stride-2 consumer layout); warpgroup g takes the
+// blocks g, g + 2, ... of each layer.
 #pragma once
 #include "tcx_conv.cuh"
 
@@ -23,19 +23,12 @@ namespace tcx {
 template <int C1, int COUT, int SA, int SW, int OSA>
 struct XFirstCfg {
     static constexpr int KC = C1 / 8, NT = COUT;
-    static constexpr int TILES = 8;
+    static constexpr int BLOCKS = 16;                          // M = 64 blocks of a patch
     static constexpr int NPIXP = 18 * 32;                      // slots of one HALF P plane: 18 window rows (16 image rows of outputs + 2 rows of look-ahead)
     static constexpr int SX = 1200;                            // floats of one padded fp32 patch buffer: 34*34 + zero tail (windows of row 33 look one row further)
     static constexpr int S1 = (C1 == 16) ? 1 : 0;              // layer 1: x_hi * [w_hi ; w_lo] as one N = 2*C1 MMA
-    static constexpr int ACC1 = 32;                            // layer-1 accumulator columns per tile (2*16 stacked, or 32)
-    static constexpr int NL1 = 4;                              // layer-1 accumulator buffers
-#ifndef AG_FIRST_STACK
-#define AG_FIRST_STACK 0   // measured (r02): stacking [W_hi ; W_lo] along N saves a third of the MMAs but its extra TMEM reads and hi + lo adds make the layer-2 epilogue the
-                           // critical role: 7.2k -> 7.5k clk per patch (AffNet / OriNet), 10.3k -> 12.8k (HardNet, only two accumulator buffers left)
-#endif
-    static constexpr int STACK = (AG_FIRST_STACK && SW && 6 * NT <= 192) ? 1 : 0; // layer 2: [W_hi ; W_lo] stacked along N
-    static constexpr int ACCW = 3 * NT * (1 + STACK);
-    static constexpr int NACC = (512 - NL1 * ACC1) / ACCW < 4 ? (512 - NL1 * ACC1) / ACCW : 4;
+    static constexpr int ACC1 = 32;                            // layer-1 accumulator columns (2*16 stacked, or 32)
+    static constexpr int ACCW = 3 * NT;
     static constexpr int G = KC * (1 + SA);
     static constexpr int SLOT_STAGE = 1024 + 32;               // zero row + 32 data rows; the zero row below is the next stage's / the trailing one
     static constexpr int GS = 2 * SLOT_STAGE + 32;
@@ -44,35 +37,24 @@ struct XFirstCfg {
     static constexpr uint32_t IN_BYTES = (uint32_t)G * GS * 16u;
     static constexpr uint32_t W1_BYTES = 2u * 2u * C1 * 16;    // [K chunk 0|1][hi rows | lo rows][8]
     static constexpr uint32_t P_BYTES = 2u * 2u * NPIXP * 16;   // [half][hi | lo][NPIXP]: the halves are built and consumed alternately
-    static constexpr size_t SMEM = 1024 + (size_t)W_BYTES + IN_BYTES + P_BYTES + W1_BYTES + 2 * SX * 4 + 256;
+    static constexpr uint32_t XCH_BYTES = 2u * 2u * 4u * 2u * NT * 4u;   // [warpgroup][block parity][warp][left | right][NT] row-boundary values
+    static constexpr size_t SMEM = 1024 + (size_t)W_BYTES + IN_BYTES + P_BYTES + W1_BYTES + 2 * SX * 4 + 256 + XCH_BYTES;
     static constexpr size_t HI_OUT_BYTES = (size_t)(COUT / 8) * 1024 * 16;
     static constexpr size_t UNIT_OUT_BYTES = HI_OUT_BYTES + (OSA == 1 ? HI_OUT_BYTES : OSA == 2 ? HI_OUT_BYTES / 2 : 0);   // OSA = 2: byte residual planes
-#ifndef AG_FIRST_NSET16
-#define AG_FIRST_NSET16 2   // three sets measured slower for the 16-channel nets (4.05 -> 4.28 ms per step over the three first kernels)
-#endif
-    static constexpr int NSET = (C1 >= 32) ? 3 : AG_FIRST_NSET16;            // layer-2 epilogue sets of four warps (HardNet's 32-channel epilogue is its critical role: three sets)
-    static constexpr int W_L2 = 8, W_L1 = W_L2 + 4 * NSET, W_MMA = W_L1 + 4;   // first warp of each role (producers: warps 0-7)
-    static constexpr int THREADS = (W_MMA + 1) * 32;
-    static_assert(C1 % 16 == 0 && NT % 16 == 0 && NACC >= 2 && ACCW <= 256, "shape");
+    static constexpr int THREADS = 512;
+    static_assert(C1 % 16 == 0 && NT % 16 == 0 && ACCW <= 256, "shape");
     static_assert(C1 == 16 || C1 == 32, "layer-1 accumulator width");
     static_assert(SMEM <= 232448, "shared memory budget");
 };
 
 template <int C1, int COUT, int SA, int SW, int OSA, int BF = 0>
-__global__ void __launch_bounds__(XFirstCfg<C1, COUT, SA, SW, OSA>::THREADS, 1) tcx_first_kernel(const XArgs a, const FirstSrc src) {
+__global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const FirstSrc src) {
     using Cfg = XFirstCfg<C1, COUT, SA, SW, OSA>;
-    constexpr int KC = Cfg::KC, NT = Cfg::NT, NACC = Cfg::NACC, TILES = Cfg::TILES, NPIXP = Cfg::NPIXP, SX = Cfg::SX, GS = Cfg::GS, NL1 = Cfg::NL1;
+    constexpr int KC = Cfg::KC, NT = Cfg::NT, ACCW = Cfg::ACCW, NPIXP = Cfg::NPIXP, SX = Cfg::SX, GS = Cfg::GS;
     extern __shared__ __align__(1024) unsigned char smem[];
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem);   // [2]   layer-2 stage filled (128 layer-1 epilogue threads)
-    uint64_t* empty = full + 2;                             // [2]   layer-2 MMAs done with the stage
-    uint64_t* tfull = empty + 2;                            // [4]
-    uint64_t* tempty = tfull + 4;                           // [4]
-    uint64_t* wbar = tempty + 4;
+    uint64_t* wbar = reinterpret_cast<uint64_t*>(smem);
     uint64_t* p_full = wbar + 1;                            // [2] half P plane written (256 producer threads)
-    uint64_t* p_empty = p_full + 2;                         // [2] layer-1 MMAs done with the half
-    uint64_t* c1_full = p_empty + 2;                        // [4]
-    uint64_t* c1_empty = c1_full + 4;                       // [4]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(c1_empty + 4);
+    uint64_t* p_empty = p_full + 2;                         // [2] layer-1 MMAs done with the half (2 warpgroups)
     float* s_bias1 = reinterpret_cast<float*>(smem + 384);  // [C1]
     float* s_bias = reinterpret_cast<float*>(smem + 512);   // [NT]
     unsigned char* sW = smem + 1024;
@@ -81,6 +63,7 @@ __global__ void __launch_bounds__(XFirstCfg<C1, COUT, SA, SW, OSA>::THREADS, 1) 
     unsigned char* sW1 = sP + Cfg::P_BYTES;                 // [chunk][hi|lo][C1][8] fp16
     float* s_x = reinterpret_cast<float*>(sW1 + Cfg::W1_BYTES);   // [2][SX]
     float* s_red = s_x + 2 * SX;                            // [2][8][2]
+    float* s_xch = s_red + 64;                              // [2][2][4][2][NT]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     auto valid = [&](int pi) -> bool { return a.count == nullptr || (pi % a.group) < a.count[pi / a.group]; };
@@ -93,10 +76,8 @@ __global__ void __launch_bounds__(XFirstCfg<C1, COUT, SA, SW, OSA>::THREADS, 1) 
     if (threadIdx.x < NT) s_bias[threadIdx.x] = a.bias[threadIdx.x];
     if (threadIdx.x < C1) s_bias1[threadIdx.x] = src.b1[threadIdx.x];
     if (threadIdx.x == 0) {
-        for (int s = 0; s < 2; s++) { mbar_init(&full[s], 128); mbar_init(&empty[s], 1); }
-        for (int i = 0; i < 4; i++) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); mbar_init(&c1_full[i], 1); mbar_init(&c1_empty[i], 4); }
         mbar_init(wbar, 1);
-        for (int hh = 0; hh < 2; hh++) { mbar_init(&p_full[hh], 256); mbar_init(&p_empty[hh], 1); }
+        for (int hh = 0; hh < 2; hh++) { mbar_init(&p_full[hh], 256); mbar_init(&p_empty[hh], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < 2 * 2 * C1 * 8; i += blockDim.x) {   // W1[chunk][hi rows | lo rows][e]: chunk 0 = kernel rows 0 (e 0..2), 1 (e 4..6); chunk 1 = kernel row 2
@@ -112,64 +93,76 @@ __global__ void __launch_bounds__(XFirstCfg<C1, COUT, SA, SW, OSA>::THREADS, 1) 
     }
     for (int i = threadIdx.x; i < (int)((Cfg::IN_BYTES + Cfg::P_BYTES) / 16); i += blockDim.x) reinterpret_cast<uint4*>(sIn)[i] = make_uint4(0, 0, 0, 0);
     for (int i = threadIdx.x; i < 2 * SX; i += blockDim.x) s_x[i] = 0.f;
-    if (warp == Cfg::W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t tmem_l2 = tmem + (uint32_t)(NL1 * Cfg::ACC1);
 
-    if (warp == Cfg::W_MMA) {
-        // ===== MMA issuer: layer 1 runs one patch ahead of layer 2 =====
-        constexpr uint32_t idesc_all = XFmt<BF>::IDESC | (1u << 4) | ((uint32_t)(Cfg::ACCW >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);      // N = 3 NT (or 6 NT stacked)
-        constexpr uint32_t idesc_3 = XFmt<BF>::IDESC | (1u << 4) | ((uint32_t)((3 * NT) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        constexpr uint32_t idesc1 = XFmt<BF>::IDESC | (1u << 4) | ((uint32_t)(C1 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        constexpr uint32_t idesc1_st = XFmt<BF>::IDESC | (1u << 4) | ((uint32_t)((2 * C1) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-        const uint32_t leader = elect_one();
-        if (leader) {
+    if (warp >= 8) {
+        // ===== consumers =====
+        const int wg = (warp - 8) >> 2, wq = warp & 3;
+        if (threadIdx.x == 256) {
             mbar_expect_tx(wbar, Cfg::W_BYTES);
             bulk_g2s(sW, a.wpk, Cfg::W_BYTES, wbar);
         }
-        __syncwarp();
         mbar_wait(wbar, 0);
-        tc_fence_after();
         const uint32_t w_base = smem_u32(sW) >> 4, in_base = smem_u32(sIn) >> 4;
         const uint32_t w1_lo = desc_lo(smem_u32(sW1), 2 * C1 * 16u);       // K chunks are 2*C1 rows apart (hi rows, then lo rows)
         const uint32_t p_lo = desc_lo(smem_u32(sP), 2 * 32 * 16u);          // leading-byte offset = two image rows
         constexpr uint32_t LBO_A = ((uint32_t)GS) << 16;
-        int c1cnt = 0, tcnt = 0;
-        RP_DECL;
-        auto l1_tile = [&](int t) {
-            const int b = c1cnt % NL1;
-            RP_WAIT(1, mbar_wait(&c1_empty[b], ((c1cnt / NL1) & 1) ^ 1));
-            tc_fence_after();
-            if (leader) {
-                const uint32_t d = tmem + (uint32_t)(b * Cfg::ACC1);
-                const uint32_t alo = p_lo + (uint32_t)((t >> 2) * 2 * NPIXP + (t & 3) * 128);   // half t/4, tile t%4 of it
-                if (Cfg::S1) {   // x_hi * [w_hi ; w_lo] in one MMA, then x_lo * w_hi
-                    umma_f16_lo<0>(d, alo, w1_lo, idesc1_st);
-                    umma_f16_lo<1>(d, alo + (uint32_t)NPIXP, w1_lo, idesc1);
-                } else {
-                    umma_f16_lo<0>(d, alo, w1_lo, idesc1);
-                    umma_f16_lo<1>(d, alo + (uint32_t)NPIXP, w1_lo, idesc1);             // x_lo * w_hi
-                    umma_f16_lo<1>(d, alo, w1_lo + (uint32_t)C1, idesc1);                 // x_hi * w_lo (lo rows follow the hi rows)
+        int it = 0, nblk = 0;
+        for (int pi = next_valid(blockIdx.x); pi < a.n; pi = next_valid(pi + gridDim.x), it++) {
+            const int s = it & 1;
+            unsigned char* st = sIn + (size_t)s * Cfg::SLOT_STAGE * 16;
+            // ---- layer 1, half plane by half plane -> fp16 (hi [+lo]) stage of layer 2 ----
+#pragma unroll 1
+            for (int hh = 0; hh < 2; hh++) {
+                mbar_wait(&p_full[hh], it & 1);
+#pragma unroll 1
+                for (int k = 0; k < 4; k++) {
+                    const int b = hh * 8 + wg + 2 * k;
+                    float d1[Cfg::ACC1 / 2];
+                    const uint32_t alo = p_lo + (uint32_t)(hh * 2 * NPIXP + (b & 7) * 64);
+                    wgmma_fence();
+                    if (Cfg::S1) {   // x_hi * [w_hi ; w_lo] in one MMA, then x_lo * w_hi
+                        Wgmma<2 * C1, BF>::mma(d1, desc64(alo), desc64(w1_lo), 0);
+                        Wgmma<C1, BF>::mma(d1, desc64(alo + (uint32_t)NPIXP), desc64(w1_lo), 1);
+                    } else {
+                        Wgmma<C1, BF>::mma(d1, desc64(alo), desc64(w1_lo), 0);
+                        Wgmma<C1, BF>::mma(d1, desc64(alo + (uint32_t)NPIXP), desc64(w1_lo), 1);             // x_lo * w_hi
+                        Wgmma<C1, BF>::mma(d1, desc64(alo), desc64(w1_lo + (uint32_t)C1), 1);                 // x_hi * w_lo (lo rows follow the hi rows)
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_reg_fence<Cfg::ACC1 / 2>(d1);
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const int slot = b * 64 + wq * 16 + (lane >> 2) + 8 * h + 32;      // pixel m sits one (zero) row into the stage
+#pragma unroll
+                        for (int j = 0; j < C1 / 8; j++) {
+                            const int c = j * 8 + 2 * (lane & 3);
+                            float v0 = d1[4 * j + 2 * h], v1 = d1[4 * j + 2 * h + 1];
+                            if (Cfg::S1) { v0 += d1[4 * (j + 2) + 2 * h]; v1 += d1[4 * (j + 2) + 2 * h + 1]; }   // [x*w_hi | x_hi*w_lo] side by side
+                            v0 = fmaxf(fmaf(v0, src.w1_inv, s_bias1[c]), 0.f);
+                            v1 = fmaxf(fmaf(v1, src.w1_inv, s_bias1[c + 1]), 0.f);
+                            uint32_t hi, lo;
+                            split_pack2<SA, BF>(v0, v1, hi, lo);
+                            *reinterpret_cast<uint32_t*>(st + ((size_t)j * GS + slot) * 16 + (c & 7) * 2) = hi;
+                            if (SA) *reinterpret_cast<uint32_t*>(st + ((size_t)(KC + j) * GS + slot) * 16 + (c & 7) * 2) = lo;
+                        }
+                    }
                 }
-                umma_commit(&c1_full[b]);
+                bar_sync(3 + wg, 128);
+                if ((threadIdx.x & 127) == 0) mbar_arrive(&p_empty[hh]);
             }
-            __syncwarp();
-            c1cnt++;
-        };
-        auto l2_tile = [&](uint32_t st_base, int t) {
-            const int ab = tcnt % NACC;
-            RP_WAIT(3, mbar_wait(&tempty[ab], ((tcnt / NACC) & 1) ^ 1));
-            tc_fence_after();
-            if (leader) {
-                const uint32_t d = tmem_l2 + (uint32_t)(ab * Cfg::ACCW);
-                const uint32_t a_t = st_base + (uint32_t)(t * 128);
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
+            bar_sync(2, 256);   // the whole stage is written (both warpgroups)
+            // ---- layer 2 ----
+            unsigned char* outp = reinterpret_cast<unsigned char*>(a.out) + (size_t)pi * Cfg::UNIT_OUT_BYTES;
+            const uint32_t st_base = in_base + (uint32_t)(s * Cfg::SLOT_STAGE);
+#pragma unroll 1
+            for (int b = wg; b < Cfg::BLOCKS; b += 2, nblk++) {
+                float d[ACCW / 2];
+                const uint32_t a_t = st_base + (uint32_t)(b * 64);
+                wgmma_fence();
 #pragma unroll
                 for (int dy = 0; dy < 3; dy++) {
 #pragma unroll
@@ -178,180 +171,70 @@ __global__ void __launch_bounds__(XFirstCfg<C1, COUT, SA, SW, OSA>::THREADS, 1) 
                         const uint32_t alo = ((a_t + (uint32_t)(dy * 32 + (KC + 2 * j) * GS)) & 0x3FFFu) | LBO_A;
                         const uint32_t blk = w_base + (uint32_t)((dy * (KC / 2) + j) * 2 * Cfg::NR);
                         const uint32_t bhi = (blk & 0x3FFFu) | ((uint32_t)Cfg::NR << 16), blo = ((blk + 3 * NT) & 0x3FFFu) | ((uint32_t)Cfg::NR << 16);
-                        if (Cfg::STACK) {   // A_hi * [W_hi ; W_lo] (N = 6 NT), then A_lo * W_hi into the hi columns
-                            if (dy == 0 && j == 0) umma_f16_lo<0>(d, ahi, bhi, idesc_all); else umma_f16_lo<1>(d, ahi, bhi, idesc_all);
-                            if (SA) umma_f16_lo<1>(d, alo, bhi, idesc_3);
-                        } else {
-                            if (dy == 0 && j == 0) umma_f16_lo<0>(d, ahi, bhi, idesc_3); else umma_f16_lo<1>(d, ahi, bhi, idesc_3);
-                            if (SW) umma_f16_lo<1>(d, ahi, blo, idesc_3);
-                            if (SA) umma_f16_lo<1>(d, alo, bhi, idesc_3);
-                        }
+                        Wgmma<3 * NT, BF>::mma(d, desc64(ahi), desc64(bhi), (dy | j) != 0);
+                        if (SW) Wgmma<3 * NT, BF>::mma(d, desc64(ahi), desc64(blo), 1);
+                        if (SA) Wgmma<3 * NT, BF>::mma(d, desc64(alo), desc64(bhi), 1);
                     }
                 }
-                umma_commit(&tfull[ab]);
-            }
-            __syncwarp();
-            tcnt++;
-        };
-        // layer 1 of patch i+1 is issued tile by tile between the layer-2 tiles of patch i: both epilogues are fed at a steady rate and
-        // four layer-1 accumulator buffers are enough
-        // The P plane lives in two halves (tiles 0-3 / 4-7) with their own barriers: while the layer-1 MMAs of one half run the producers
-        // build the other, so the issuer never waits for a whole plane.
-        // (two nested loops over half and tile-in-half: indexing the barriers with t >> 2 under (t & 3) guards was miscompiled by nvcc 12.9 -
-        // the strength-reduced address of &p_empty[t >> 2] came out as base + 2 t)
-        int pi = next_valid(blockIdx.x);
-        if (pi < a.n) {
-#pragma unroll 1
-            for (int hh = 0; hh < 2; hh++) {
-                mbar_wait(&p_full[hh], 0);
-                tc_fence_after();
-#pragma unroll 1
-                for (int j = 0; j < 4; j++) l1_tile(hh * 4 + j);
-                if (leader) umma_commit(&p_empty[hh]);
-                __syncwarp();
-            }
-        }
-        int it = 0;
-        while (pi < a.n) {
-            const int pn = next_valid(pi + gridDim.x);
-            const bool has_next = pn < a.n;
-            const int s = it & 1;
-            RP_WAIT(2, mbar_wait(&full[s], (it >> 1) & 1));
-            tc_fence_after();
-            const uint32_t st_base = in_base + (uint32_t)(s * Cfg::SLOT_STAGE);
-#pragma unroll 1
-            for (int hh = 0; hh < 2; hh++) {
-                if (has_next) { RP_WAIT(0, mbar_wait(&p_full[hh], (it + 1) & 1)); tc_fence_after(); }
-#pragma unroll 1
-                for (int j = 0; j < 4; j++) {
-                    if (has_next) l1_tile(hh * 4 + j);
-                    l2_tile(st_base, hh * 4 + j);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_reg_fence<ACCW / 2>(d);
+                // rows r = 16 wq + lane/4 + 8 h of the block: pixel m = 64 b + r, y = m / 32, x = m % 32.  Warps 2k and 2k+1 share an image
+                // row: the last row of an even warp and the first of the odd one exchange their dx = 0 / dx = 2 values through shared memory.
+                float* xw = s_xch + (size_t)((wg * 2 + (nblk & 1)) * 4) * 2 * NT;
+                if (lane >= 28) {
+#pragma unroll
+                    for (int j = 0; j < NT / 8; j++) {
+                        const int c = j * 8 + 2 * (lane & 3);
+                        xw[(wq * 2 + 0) * NT + c] = d[4 * j + 2]; xw[(wq * 2 + 0) * NT + c + 1] = d[4 * j + 3];   // row 15, dx = 0
+                    }
                 }
-                if (has_next) { if (leader) umma_commit(&p_empty[hh]); __syncwarp(); }
-            }
-            if (leader) umma_commit(&empty[s]);
-            __syncwarp();
-            it++;
-            pi = pn;
-        }
-        XP_STORE(0, 0);
-    } else if (warp >= Cfg::W_L2 && warp < Cfg::W_L1) {
-        // ===== layer-2 epilogue: TMEM -> x shifts -> bias + ReLU -> fp16 -> global (parity planes of the stride-2 consumer) =====
-        const int q = warp & 3, set = (warp - Cfg::W_L2) >> 2;
-        const int r = q * 32 + lane;
-        const int x = lane;
-        const float mask_l = x > 0 ? 1.f : 0.f, mask_r = x < 31 ? 1.f : 0.f;
-        float bias2[NT];
+                if (lane < 4) {
 #pragma unroll
-        for (int i = 0; i < NT; i++) bias2[i] = s_bias[i];
-        int tcnt = 0;
-        RP_DECL;
-        for (int pi = next_valid(blockIdx.x); pi < a.n; pi = next_valid(pi + gridDim.x)) {
-            unsigned char* outp = reinterpret_cast<unsigned char*>(a.out) + (size_t)pi * Cfg::UNIT_OUT_BYTES;
-#pragma unroll 1
-            for (int t = 0; t < TILES; t++, tcnt++) {
-                if ((tcnt % Cfg::NSET) != set) continue;
-                const int ab = tcnt % NACC;
-                RP_WAIT(0, mbar_wait(&tfull[ab], (tcnt / NACC) & 1));
-                tc_fence_after();
-                const int y = t * 4 + q;
-                const uint32_t taddr = tmem_l2 + ((uint32_t)(q * 32) << 16) + (uint32_t)(ab * Cfg::ACCW);
-                unsigned char* obase = outp + (size_t)layout_slot(L_S2_16, y, x, 0) * 16;
-                (void)r;
-#pragma unroll
-                for (int c0 = 0; c0 < NT; c0 += 16) {
-                    uint32_t r0[16], r1[16], r2[16];
-                    if (Cfg::STACK) {   // hi block + A_hi * W_lo block, one tap at a time (registers)
-                        uint32_t l[16];
-                        tmem_ld16(taddr + (uint32_t)c0, r0); tmem_ld16(taddr + (uint32_t)(3 * NT + c0), l);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; i++) r0[i] = __float_as_uint(__uint_as_float(r0[i]) + __uint_as_float(l[i]));
-                        tmem_ld16(taddr + (uint32_t)(NT + c0), r1); tmem_ld16(taddr + (uint32_t)(4 * NT + c0), l);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; i++) r1[i] = __float_as_uint(__uint_as_float(r1[i]) + __uint_as_float(l[i]));
-                        tmem_ld16(taddr + (uint32_t)(2 * NT + c0), r2); tmem_ld16(taddr + (uint32_t)(5 * NT + c0), l);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; i++) r2[i] = __float_as_uint(__uint_as_float(r2[i]) + __uint_as_float(l[i]));
-                    } else {
-                        tmem_ld16(taddr + (uint32_t)c0, r0);
-                        tmem_ld16(taddr + (uint32_t)(NT + c0), r1);
-                        tmem_ld16(taddr + (uint32_t)(2 * NT + c0), r2);
-                        tmem_ld_wait();
+                    for (int j = 0; j < NT / 8; j++) {
+                        const int c = j * 8 + 2 * (lane & 3);
+                        xw[(wq * 2 + 1) * NT + c] = d[4 * (j + 2 * NT / 8)]; xw[(wq * 2 + 1) * NT + c + 1] = d[4 * (j + 2 * NT / 8) + 1];   // row 0, dx = 2
                     }
-                    if (c0 + 16 >= NT) {
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&tempty[ab]);
-                    }
-                    float v[16];
+                }
+                bar_sync(3 + wg, 128);
+                const int y0 = (b * 64 + wq * 16) >> 5;
+                const int x0 = (wq & 1) * 16 + (lane >> 2);             // h = 0; h = 1 is x0 + 8
+                const float ml0 = x0 > 0 ? 1.f : 0.f, mr1 = x0 + 8 < 31 ? 1.f : 0.f;
+                const bool from_prev = (wq & 1) && lane < 4, from_next = !(wq & 1) && lane >= 28;
 #pragma unroll
-                    for (int i = 0; i < 16; i++) {
-                        const float left = __shfl_up_sync(0xffffffffu, __uint_as_float(r0[i]), 1);
-                        const float right = __shfl_down_sync(0xffffffffu, __uint_as_float(r2[i]), 1);
-                        const float acc = fmaf(left, mask_l, fmaf(right, mask_r, __uint_as_float(r1[i])));   // 0/1 masks: zero padding outside the row
-                        v[i] = fmaxf(fmaf(acc, a.inv_scale, bias2[c0 + i]), 0.f);
+                for (int j = 0; j < NT / 8; j++) {
+                    const int c = j * 8 + 2 * (lane & 3);
+                    float v[2][2];
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const float c00 = d[4 * j + e], c01 = d[4 * j + 2 + e];
+                        const float c10 = d[4 * (j + NT / 8) + e], c11 = d[4 * (j + NT / 8) + 2 + e];
+                        const float c20 = d[4 * (j + 2 * NT / 8) + e], c21 = d[4 * (j + 2 * NT / 8) + 2 + e];
+                        float l0, l1, r0, r1;
+                        frag_left(c00, c01, lane, l0, l1);
+                        frag_right(c20, c21, lane, r0, r1);
+                        if (from_prev) l0 = xw[((wq - 1) * 2 + 0) * NT + c + e];
+                        if (from_next) r1 = xw[((wq + 1) * 2 + 1) * NT + c + e];
+                        // 0/1 masks: zero padding outside the row (x = 0 for h = 0 of even warps' first lanes, x = 31 for h = 1 of odd warps' last lanes)
+                        const float acc0 = fmaf(l0, ml0, r0 + c10);
+                        const float acc1 = fmaf(r1, mr1, l1 + c11);
+                        v[0][e] = fmaxf(fmaf(acc0, a.inv_scale, s_bias[c + e]), 0.f);
+                        v[1][e] = fmaxf(fmaf(acc1, a.inv_scale, s_bias[c + e]), 0.f);
                     }
 #pragma unroll
-                    for (int g = 0; g < 2; g++) {
-                        const size_t goff = (size_t)(c0 / 8 + g) * 1024 * 16;
-                        uint4 hi, lo;
-                        split_pack8<OSA, BF>(v + g * 8, hi, lo);
-                        *reinterpret_cast<uint4*>(obase + goff) = hi;
-                        if (OSA == 1) *reinterpret_cast<uint4*>(obase + (size_t)(COUT / 8) * 1024 * 16 + goff) = lo;
-                        if (OSA == 2) *reinterpret_cast<uint2*>(outp + Cfg::HI_OUT_BYTES + ((size_t)(c0 / 8 + g) * 1024 + layout_slot(L_S2_16, y, x, 0)) * 8) = pack_lo8(lo);
+                    for (int h = 0; h < 2; h++) {
+                        const int slot = layout_slot(L_S2_16, y0, x0 + 8 * h, 0);
+                        const size_t goff = (size_t)(c / 8) * 1024 * 16;
+                        uint32_t hi, lo;
+                        split_pack2<OSA, BF>(v[h][0], v[h][1], hi, lo);
+                        *reinterpret_cast<uint32_t*>(outp + goff + (size_t)slot * 16 + (c & 7) * 2) = hi;
+                        if (OSA == 1) *reinterpret_cast<uint32_t*>(outp + (size_t)(COUT / 8) * 1024 * 16 + goff + (size_t)slot * 16 + (c & 7) * 2) = lo;
+                        if (OSA == 2) *reinterpret_cast<uint16_t*>(outp + Cfg::HI_OUT_BYTES + ((size_t)(c / 8) * 1024 + slot) * 8 + (c & 7)) = pack_lo8_2(lo);
                     }
                 }
             }
         }
-        if (warp == Cfg::W_L2) XP_STORE(0, 1);
-    } else if (warp >= Cfg::W_L1 && warp < Cfg::W_MMA) {
-        // ===== layer-1 epilogue: TMEM -> bias + ReLU -> fp16 (hi [+lo]) -> shared-memory stage of layer 2 =====
-        const int q = warp & 3;
-        int it = 0, c1cnt = 0;
-        float bias1[C1];   // registers: a shared-memory read per use would cost the shared-memory pipe 16 wavefronts per tile and warp
-#pragma unroll
-        for (int i = 0; i < C1; i++) bias1[i] = s_bias1[i];
-        RP_DECL;
-        for (int pi = next_valid(blockIdx.x); pi < a.n; pi = next_valid(pi + gridDim.x), it++) {
-            const int s = it & 1;
-            RP_WAIT(0, mbar_wait(&empty[s], ((it >> 1) & 1) ^ 1));
-            unsigned char* st = sIn + (size_t)s * Cfg::SLOT_STAGE * 16;
-#pragma unroll 1
-            for (int t = 0; t < TILES; t++, c1cnt++) {
-                const int b = c1cnt % NL1;
-                RP_WAIT(1, mbar_wait(&c1_full[b], (c1cnt / NL1) & 1));
-                tc_fence_after();
-                const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(b * Cfg::ACC1);
-                uint32_t r[32];
-                tmem_ld32(taddr, r);
-                tmem_ld_wait();
-                if (Cfg::S1) {   // [x*w_hi | x_hi*w_lo] side by side: add the halves
-#pragma unroll
-                    for (int i = 0; i < 16; i++) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r[16 + i]));
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&c1_empty[b]);
-                const int slot = t * 128 + q * 32 + lane + 32;      // pixel m = t*128 + row sits one (zero) row into the stage
-#pragma unroll
-                for (int g = 0; g < C1 / 8; g++) {
-                    float v[8];
-#pragma unroll
-                    for (int e = 0; e < 8; e++) v[e] = fmaxf(fmaf(__uint_as_float(r[g * 8 + e]), src.w1_inv, bias1[g * 8 + e]), 0.f);
-                    uint4 hi, lo;
-                    split_pack8<SA, BF>(v, hi, lo);
-                    *reinterpret_cast<uint4*>(st + ((size_t)g * GS + slot) * 16) = hi;
-                    if (SA) *reinterpret_cast<uint4*>(st + ((size_t)(KC + g) * GS + slot) * 16) = lo;
-                }
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_arrive(&full[s]);
-        }
-        if (warp == Cfg::W_L1) XP_STORE(0, 2);
-    } else if (warp < 8) {
+    } else {
         // ===== producers (8 warps): sampler (or patch load) -> input_norm -> sliding-window planes P_hi / P_lo =====
         const int pw = warp;                                 // 0..7
         const int pt = pw * 32 + lane;                       // 0..255
@@ -381,7 +264,6 @@ __global__ void __launch_bounds__(XFirstCfg<C1, COUT, SA, SW, OSA>::THREADS, 1) 
         int pi = next_valid(blockIdx.x);
         if (pi < a.n) issue_fetch(pi);
         int it = 0;
-        RP_DECL;
         while (pi < a.n) {
             float* sx = s_x + (it & 1) * SX;
             float* red = s_red + (it & 1) * 16;
@@ -409,7 +291,7 @@ __global__ void __launch_bounds__(XFirstCfg<C1, COUT, SA, SW, OSA>::THREADS, 1) 
             // P planes, half by half
 #pragma unroll 1
             for (int hh = 0; hh < 2; hh++) {
-                RP_WAIT(0, mbar_wait(&p_empty[hh], (it & 1) ^ 1));   // layer-1 MMAs of the previous patch have consumed this half
+                mbar_wait(&p_empty[hh], (it & 1) ^ 1);   // layer-1 MMAs of the previous patch have consumed this half
                 unsigned char* ph = sP + (size_t)hh * 2 * NPIXP * 16;
                 // one 16-byte window per thread and step: consecutive lanes read consecutive pixels and write consecutive slots (no bank
                 // conflicts; the shared-memory pipe is this kernel's busiest unit)
@@ -430,13 +312,6 @@ __global__ void __launch_bounds__(XFirstCfg<C1, COUT, SA, SW, OSA>::THREADS, 1) 
             it++;
             pi = pn;
         }
-        if (warp == 0) XP_STORE(0, 3);
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == Cfg::W_MMA) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
     }
 }
 

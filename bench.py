@@ -1,14 +1,15 @@
 #!/usr/bin/env python
 """Benchmark of the HesAffNet + HardNet detect-and-describe hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config 2|3|5] [--batch B] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config 2|3|5] [--batch B] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one pass of the whole path (pyramid -> Hessian/NMS -> top-k -> sample -> AffNet -> filter -> sample
 -> OriNet -> sample -> HardNet) over one batch of B synthetic images per GPU.  Headline workload (--config 2, the default):
 1024x768, K=2000 keypoints, B=16 (BASELINE.json configs[1] tiled B times = configs[3]'s per-GPU shard).  --config 3: 1920x1080, K=4000,
 B=64; --config 5: 3840x2160, K=8000, border=33 (the 5-octave pyramid), B=1.  N>1: one process per GPU (torchrun), B images per rank
 (weak scaling), one NCCL all-gather of descriptors/LAFs/counts per step.  Prints ONE JSON line; with the default config the line
-also carries `extra`: the same metric for B=1, B=64 (configs[3] as written) and configs 3 and 5.
+also carries `extra`: the same metric for B=1, B=64 (configs[3] as written) and configs 3 and 5.  --dump-outputs DIR writes what the
+last timed step returned (LAFs, responses, descriptors, counts) as DIR/<name>.npy, so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -45,25 +46,12 @@ def oracle_module():
     return affnet_oracle
 
 
-def ncu_traffic(batch):
-    """DRAM bytes per step of the tcgen05 kernel family from the committed `ncu --set full` capture (profiles/*_ncu_traffic.json,
-    written by scripts/ncu_summary.py); None when no capture exists for this batch size."""
-    best = None
-    pdir = os.path.join(ROOT, "profiles")
-    for f in sorted(os.listdir(pdir)) if os.path.isdir(pdir) else []:
-        if f.endswith("_ncu_traffic.json"):
-            d = json.load(open(os.path.join(pdir, f)))
-            if d.get("batch") == batch:
-                best = {"dram_bytes_per_step": d["family_bytes_per_step"], "launches": len(d["launches"]), "source": "profiles/" + f}
-    return best
-
-
 def peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(path):
         d = json.load(open(path))
         return dict(hbm=d["hbm_gbs"], tensor=d["bf16_tflops"], tensor_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tensor=1590.0, tensor_sustained=1400.0, src="fallback")
+    return dict(hbm=3350.0, tensor=989.0, tensor_sustained=989.0, src="H100 SXM data sheet (dense fp16/bf16, 700 W)")
 
 
 def make_images(B, seed0, H, W):
@@ -77,7 +65,7 @@ def load_state_dicts():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, gpu_index):
@@ -218,8 +206,33 @@ def emit(real_stdout, line):
     os.write(real_stdout, (json.dumps(line) + "\n").encode())
 
 
-TC_FAMILY = ("tc_first2_kernel", "tc_conv_kernel", "tc_conv_pair_kernel", "tc_head_kernel", "tc_headx_kernel", "tcx_first_kernel", "tcx_conv_kernel")
+TC_FAMILY = ("tc_conv_kernel<first>", "tc_conv_kernel", "tc_head_kernel", "tc_headx_kernel", "tcx_first_kernel", "tcx_conv_kernel")
 STENCIL = ("blur_kernel", "octave_kernel", "pyramid_tail_kernel", "detect_level_kernel", "detect_fused_kernel", "detect_warp_kernel", "detect_rows_kernel", "resolve_kernel")
+
+
+DUMP_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(d, outs):
+    """outs = (lafs [B,K,2,3], responses [B,K], descriptors [B,K,128], counts [B]) of one step -> d/<name>.npy in float32.  Rows beyond an
+    image's count are zero.  When the arrays exceed DUMP_BYTES, a fixed seeded sample of (image, keypoint) rows is written instead, with its
+    flat row indices in keypoint_rows.npy."""
+    os.makedirs(d, exist_ok=True)
+    lafs, resp, desc, cnt = [t.detach().float().cpu().numpy() for t in outs]
+    B, K = resp.shape
+    lafs, resp, desc = lafs.reshape(B * K, 2, 3), resp.reshape(B * K), desc.reshape(B * K, -1)
+    per_row = 4 * (6 + 1 + desc.shape[1])
+    arrays = {"counts": cnt.astype(np.float32)}
+    if B * K * per_row > DUMP_BYTES:
+        n = (DUMP_BYTES - 4 * B) // (per_row + 8)
+        rows = np.sort(np.random.default_rng(0).choice(B * K, size=n, replace=False))
+        lafs, resp, desc = lafs[rows], resp[rows], desc[rows]
+        arrays["keypoint_rows"] = rows.astype(np.float64)
+    else:
+        lafs, resp, desc = lafs.reshape(B, K, 2, 3), resp.reshape(B, K), desc.reshape(B, K, -1)
+    arrays.update(lafs=lafs, responses=resp, descriptors=desc)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), a)
 
 
 class Workload:
@@ -239,6 +252,7 @@ class Workload:
         self.host_imgs = make_images(B, 1234 + rank * B, H, W).pin_memory()
         self.dev_imgs = self.host_imgs.to(dev)
         self.last = [None, None, None, None]
+        self.kept = None      # copies of the last timed step's outputs (keep_last)
         self.step_i = 0
         if use_graph:
             self.pipe.capture()
@@ -258,7 +272,7 @@ class Workload:
     def step_device(self):
         return self._run(self.dev_imgs)
 
-    def timed(self, steps, warmup, sampler=None):
+    def timed(self, steps, warmup, sampler=None, keep_last=False):
         ctx = self.ctx
         dist, dev, flush = ctx["dist"], ctx["dev"], ctx["flush"]
         for _ in range(warmup):
@@ -280,6 +294,8 @@ class Workload:
             evs.append((e0, e1))
         torch.cuda.synchronize()
         t_stop = time.time()
+        if keep_last:
+            self.kept = [t.detach().clone() for t in self.last]
         clocks = None
         if sampler:
             # The sampler runs since before the warm-up; only samples that arrived inside the timed region count.  If the region was
@@ -410,6 +426,7 @@ def _main(real_stdout):
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the extra configurations (B=1, B=64, configs 3 and 5)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
 
@@ -442,13 +459,15 @@ def _main(real_stdout):
     sampler = ClockSampler(local) if rank == 0 else None
     if sampler:
         sampler.start()   # nvidia-smi needs a few hundred ms to deliver its first sample: start it long before the timed region
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # 256 MiB > the 50 MB L2 of an H100
     ctx = {"dev": dev, "dist": dist, "rank": rank, "world": world, "nets": (a, o, h), "flush": flush}
     use_graph = not args.no_graph
     wl = Workload(ctx, H, W, K, border, B, use_graph)
     pipe = wl.pipe
 
-    total_ms, clocks = wl.timed(args.steps, args.warmup, sampler)
+    total_ms, clocks = wl.timed(args.steps, args.warmup, sampler, keep_last=bool(args.dump_outputs))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, wl.kept)
     pipe.check()
     wl.check_exchange()
     n_desc = int(wl.last[3].sum().item())
@@ -470,17 +489,17 @@ def _main(real_stdout):
         step_ms = sum(sum(v) for v in per_kernel.values()) / prof_steps
         agg = sorted(((sum(v) / prof_steps, len(v) // prof_steps, k) for k, v in per_kernel.items()), reverse=True)
         pk = peaks()
-        # dominant kernel family: every tcgen05 kernel of the three CNNs (layers 1+2 fused with the sampler in the "first" kernels, layers 3-6 in
+        # dominant kernel family: every tensor-core kernel of the three CNNs (layers 1+2 fused with the sampler in the "first" kernels, layers 3-6 in
         # the conv kernels, the 8x8 head GEMMs in tc_head_kernel / tc_headx_kernel)
         n_aff, n_ori, n_hard = B * int(1.5 * K), n_desc, n_desc
         tc_flop = n_aff * FLOP_PER_PATCH["affnet"] + n_ori * FLOP_PER_PATCH["orinet"] + n_hard * FLOP_PER_PATCH["hardnet"]
         tc_ms = sum(t for t, n, k in agg if k in TC_FAMILY)
         tc_launches = sum(n for t, n, k in agg if k in TC_FAMILY)
         ach = tc_flop / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else 0.0
-        roof = {"kernel": "tcgen05 kernels (%d launches/step: %s; fp16 operands with fp16 residual planes for AffNet/OriNet and HardNet layers 2-3, fp32 accumulate in TMEM)"
+        roof = {"kernel": "wgmma kernels (%d launches/step: %s; fp16 operands with fp16 residual planes for AffNet/OriNet and HardNet layers 2-3, fp32 accumulate)"
                           % (tc_launches, ", ".join("%s x%d" % (k, n) for t, n, k in agg if k in TC_FAMILY)),
                 "bound": "tensor", "achieved": ach, "peak": pk["tensor_sustained"], "unit": "TFLOP/s", "frac": ach / pk["tensor_sustained"],
-                "traffic": ncu_traffic(B), "peak_source": pk["src"] + " bf16 sustained (kernel timed inside a long step)", "kernel_ms_per_step": tc_ms,
+                "peak_source": pk["src"] + " bf16 sustained (kernel timed inside a long step)", "kernel_ms_per_step": tc_ms,
                 "algorithmic_flop_per_step": tc_flop, "share_of_step": tc_ms / step_ms if step_ms else None,
                 "note": "algorithmic flops = 2*MAC of the reference's fp32 convolutions; the residual-plane products (3 MMAs per K step for AffNet/OriNet, 2 for HardNet "
                         "layers 2-3) and the K=9 first layer padded to K=16 are extra tensor work that is not counted",

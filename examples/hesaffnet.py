@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Counterpart of the reference's examples/hesaffnet/hesaffnet.py on the B200-native path:
+"""Counterpart of the reference's examples/hesaffnet/hesaffnet.py on the H100-native path:
 
     python examples/hesaffnet.py img.png out.txt 2000 [--weights tests/golden/weights.npz | --affnet pretrained/AffNet.pth]
 

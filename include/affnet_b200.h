@@ -1,5 +1,5 @@
 /*
- * affnet_b200 C ABI  --  the drop-in boundary of the B200-native HesAffNet + HardNet hot path.
+ * affnet_b200 C ABI  --  the drop-in boundary of the H100-native HesAffNet + HardNet hot path.
  *
  * The reference (ducha-aiki/affnet) has no FFI: its boundary is the Python module API
  * (SURVEY.md §8b).  The thin Python mirror in `affnet_b200/` keeps those names and calls ONLY the
@@ -30,7 +30,7 @@ extern "C" {
 #define AG_ERR_INVALID -1   /* bad argument */
 #define AG_ERR_CUDA -2      /* a CUDA runtime call failed */
 #define AG_ERR_CAPACITY -3  /* a fixed-capacity buffer is too small */
-#define AG_ERR_NO_DEVICE -4 /* no sm_100 device / kernel image not loadable */
+#define AG_ERR_NO_DEVICE -4 /* no sm_90 device / kernel image not loadable */
 
 #define AG_MAX_OCTAVES 16
 #define AG_MAX_LEVELS 8 /* nlevels + 2 */
@@ -163,14 +163,14 @@ typedef struct ag_net ag_net_t;
 int ag_net_create(int kind, const float* h_blob, size_t n_floats, ag_net_t** out);
 void ag_net_destroy(ag_net_t* net);
 size_t ag_net_blob_floats(int kind);
-/* Compute engine: 0 = exact fp32 SIMT (needs materialised patches); 1 = first-generation tcgen05 engine (round 1; one MMA per tap): fp16
- * operands, fp32 accumulation in TMEM, all six conv layers and the 8x8 heads as MMAs; AffNet and OriNet carry fp16 residual
+/* Compute engine: 0 = exact fp32 SIMT (needs materialised patches); 1 = first-generation tensor-core engine (one MMA per tap): fp16
+ * operands, fp32 accumulation, all six conv layers and the 8x8 heads as MMAs; AffNet and OriNet carry fp16 residual
  * planes of weights AND activations in every layer (fp32-grade: A 1e-5, angle 3e-5 rad - OriNet's atan2 amplifies an error of
  * AffNet's A about 15x, so the 1e-3 LAF contract needs A to 5e-5), HardNet plain fp16 operands (descriptors 6e-4);
  * 2 = as 1 with fp32 FMA-chain heads (A 2e-6, angle 3e-6 rad; AffNet/OriNet only); 3 = AffNet with the weight residual only
  * (A 2e-4; for A/B timing, AffNet only);
- * 4 = second-generation tcgen05 engine, THE DEFAULT for all three nets (same operand precision as 1, plus fp16 residuals of HardNet's
- * layer 2-3 weights: descriptors 4e-4): 128-pixel
+ * 4 = second-generation tensor-core engine, THE DEFAULT for all three nets (same operand precision as 1, plus fp16 residuals of HardNet's
+ * layer 2-3 weights: descriptors 4e-4): 64-pixel
  * row tiles without x padding, the three taps of a kernel row stacked along N of one MMA, x shifts by warp shuffles in the epilogue;
  * 5 = engine 4 with bf16 operands (HardNet only; BASELINE.json configs[4] "bf16 HardNet tensor-core path"; descriptors ~4e-3). */
 int ag_net_set_engine(ag_net_t* net, int engine);

@@ -200,6 +200,16 @@ def make_jit():
         save("jit.npz", patches=P, affnet_raw=aff(P), orinet_raw=ori(P))
 
 
+def make_distance():
+    """Losses.distance_matrix_vector of the reference on two seeded descriptor sets."""
+    import importlib
+    R.ref_modules()
+    LS = importlib.import_module("Losses")
+    g = torch.Generator().manual_seed(5)
+    a, b = torch.randn(50, 128, generator=g), torch.randn(70, 128, generator=g)
+    save("distance_matrix.npz", a_sum=a.double().sum(), b_sum=b.double().sum(), dm=LS.distance_matrix_vector(a, b))
+
+
 def make_match():
     import importlib
     m = R.ref_modules()
@@ -233,8 +243,11 @@ if __name__ == "__main__":
         make_match()
     elif len(sys.argv) > 1 and sys.argv[1] == "jit":
         make_jit()
+    elif len(sys.argv) > 1 and sys.argv[1] == "distance":
+        make_distance()
     else:
         main()
         make_ell()
         make_match()
+        make_distance()
         make_jit()

@@ -233,7 +233,7 @@ def test_level_selection_identical(L):
 
 @pytest.mark.parametrize("engine", ["simt", "tc"])
 def test_nets_vs_oracle(L, nets, engine):
-    """a9/a12/a16.  simt = exact fp32 engine (1e-4); tc = first-generation tcgen05 engine (the default second-generation engine has
+    """a9/a12/a16.  simt = exact fp32 engine (1e-4); tc = first-generation tensor-core engine (the default second-generation engine has
     the same checks in tests/test_gpu_tcx.py): north_star's 1e-3 for descriptors, fp32-grade A matrices and angles."""
     aff, ori, hn = nets
     e = L.ENGINE_SIMT if engine == "simt" else L.ENGINE_TC
