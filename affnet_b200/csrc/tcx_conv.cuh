@@ -179,7 +179,10 @@ struct XCfg {
 };
 
 // Neighbours of an accumulator fragment value along x: v0 / v1 are the values of rows i = lane/4 and i + 8 of this warp's 16 rows.
-// Row i - 1 (left) and i + 1 (right); a neighbour outside the warp's rows is an image-row boundary (callers multiply by their 0/1 masks).
+// Row i - 1 (left) and i + 1 (right); a neighbour outside the image row is garbage that callers must drop by a select, never by
+// multiplying with 0: in the pair layouts it is the other patch of the unit, whose input rows are stale workspace when that patch is
+// skipped (beyond a count, or the tail of an odd n).  NaN * 0 = NaN, and the ReLU's fmaxf(NaN, 0) = 0 then silently zeroes the valid
+// patch's border pixel.
 __device__ __forceinline__ void frag_left(float v0, float v1, int lane, float& l0, float& l1) {
     const float s0 = __shfl_sync(0xffffffffu, v0, (lane + 28) & 31), s1 = __shfl_sync(0xffffffffu, v1, (lane + 28) & 31);
     l0 = s0;
@@ -325,7 +328,7 @@ __global__ void __launch_bounds__(288 + (SA == 2 ? 128 : 0), 1) tcx_conv_kernel(
                 int pis[2];
                 unsigned char* obase[2];
                 unsigned char* obase8[2];     // OSA = 2: byte residual planes behind the hi planes
-                float mask_l[2], mask_r[2];
+                bool has_l[2], has_r[2];      // the left / right neighbour lies inside the image row (else: zero padding)
                 bool ok[2];
                 size_t lo_off = 0;
 #pragma unroll
@@ -336,7 +339,7 @@ __global__ void __launch_bounds__(288 + (SA == 2 ? 128 : 0), 1) tcx_conv_kernel(
                     else { y = r / W; x = r - y * W; pi = u; }
                     pis[h] = pi;
                     ok[h] = pvalid(pi);
-                    mask_l[h] = x > 0 ? 1.f : 0.f; mask_r[h] = x < W - 1 ? 1.f : 0.f;
+                    has_l[h] = x > 0; has_r[h] = x < W - 1;
                     if (OUT == L_HEAD) {
                         obase[h] = reinterpret_cast<unsigned char*>(a.out) + (((size_t)(pi >> 7) * (HOUT * HOUT * COUT / 8) + (size_t)(y * HOUT + x) * (COUT / 8)) * 128 + (pi & 127)) * 16;
                         lo_off = (size_t)((a.n + 127) >> 7) * (HOUT * HOUT * COUT / 8) * 128 * 16;
@@ -361,15 +364,19 @@ __global__ void __launch_bounds__(288 + (SA == 2 ? 128 : 0), 1) tcx_conv_kernel(
                         const float c20 = d[4 * (j + 2 * NT / 8) + e], c21 = d[4 * (j + 2 * NT / 8) + 2 + e];     // block 2
                         float l0, l1;
                         frag_left(c00, c01, lane, l0, l1);
+                        // zero padding by selects: the same roundings as adding the neighbour (fmaf(l, 1, t) == l + t), and a NaN of a
+                        // skipped pair partner stays out of the valid patch
                         float acc0, acc1;
                         if (STRIDE == 1) {
                             float r0, r1;
                             frag_right(c20, c21, lane, r0, r1);
-                            acc0 = fmaf(l0, mask_l[0], fmaf(r0, mask_r[0], c10));
-                            acc1 = fmaf(l1, mask_l[1], fmaf(r1, mask_r[1], c11));
+                            const float t0 = has_r[0] ? r0 + c10 : c10, t1 = has_r[1] ? r1 + c11 : c11;
+                            acc0 = has_l[0] ? l0 + t0 : t0;
+                            acc1 = has_l[1] ? l1 + t1 : t1;
                         } else {
-                            acc0 = fmaf(l0, mask_l[0], c10 + c20);
-                            acc1 = fmaf(l1, mask_l[1], c11 + c21);
+                            const float t0 = c10 + c20, t1 = c11 + c21;
+                            acc0 = has_l[0] ? l0 + t0 : t0;
+                            acc1 = has_l[1] ? l1 + t1 : t1;
                         }
                         v[0][e] = fmaxf(fmaf(acc0, a.inv_scale, s_bias[c + e]), 0.f);
                         v[1][e] = fmaxf(fmaf(acc1, a.inv_scale, s_bias[c + e]), 0.f);

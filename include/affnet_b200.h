@@ -186,7 +186,9 @@ size_t ag_net_workspace_bytes(int kind, int n);
 
 /* d_patches [n,1,32,32] (any scale: per-patch mean/std normalisation is part of forward).
  * Row validity: rows are grouped in groups of `group` rows (group <= 0 => one group of n rows); if d_count is
- * not NULL, only the first d_count[g] rows of group g are computed (device int32 array), else all rows.
+ * not NULL, only the first d_count[g] rows of group g are computed (device int32 array), else all rows.  Rows beyond `d_count` are
+ * not written (d_out / d_angle keep what the caller left there), and every engine gives a valid row the same bits whatever the other
+ * rows hold and whatever the workspace held before the call (tests/test_gpu_rows.py).
  * AffNet -> d_out [n,2,2] rectified A.   OriNet -> d_out [n,2,2] rotation (and/or d_angle [n]; either may be NULL).
  * HardNet -> d_out [n,128] L2-normalised. */
 int ag_affnet_forward(const ag_net_t* net, const float* d_patches, int n, const int* d_count, int group, float* d_out,
@@ -204,7 +206,8 @@ int ag_affnet_forward_raw(const ag_net_t* net, const float* d_patches, int n, fl
 int ag_orinet_forward_raw(const ag_net_t* net, const float* d_patches, int n, float* d_raw, void* d_ws, size_t ws_bytes, void* stream);
 /* Fused sampler + net (tensor-core engine): LAF i of image b is sampled at pyr[oct][lvl] INSIDE the first tensor-core
  * layer (32x32 patches never touch HBM), then the net runs as above.  Layout as ag_extract_patches_pyr: d_lafs
- * [B,cap,2,3] normalised, d_oct/d_lvl [B,cap], d_count [B] or NULL.  d_out: [B*cap,2,2] (AffNet, OriNet) or [B*cap,128]. */
+ * [B,cap,2,3] normalised, d_oct/d_lvl [B,cap], d_count [B] or NULL (rows beyond d_count[b] of image b are not written).
+ * d_out: [B*cap,2,2] (AffNet, OriNet) or [B*cap,128].  The fp32 SIMT engine (0) is refused with AG_ERR_INVALID. */
 int ag_net_forward_pyr(const ag_net_t* net, const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct,
                        const int* d_lvl, const int* d_count, int cap, float* d_out, void* d_ws, size_t ws_bytes, void* stream);
 

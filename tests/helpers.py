@@ -72,6 +72,70 @@ def parity_report(oL, odesc, dL, desc, tag=""):
 
 TOL = 1e-3     # north_star: LAF parameters (relative to the LAF scale) and HardNet descriptors within 1e-3
 
+# ---- direct calls of the net entry points with row counts and a caller-owned workspace -------------------------------------------
+POISON_NAN, POISON_INF = 0xFFFF, 0x7C00    # 16-bit words a workspace is filled with: all-ones bytes (NaN in fp16 and fp32), fp16 +Inf
+SENTINEL = -12345.0                        # output rows a call must not write keep this value
+
+
+def poisoned(nbytes, word, device="cuda"):
+    """A device buffer of `nbytes` (even) bytes whose every 16-bit word is `word`, or uninitialised when word is None."""
+    buf = torch.empty(nbytes, dtype=torch.uint8, device=device)
+    if word is not None:
+        buf.view(torch.int16).fill_(word - 0x10000 if word >= 0x8000 else word)
+    return buf
+
+
+def row_valid(n, group, counts):
+    """Row validity of the C ABI: row i is valid when i % group < counts[i // group] (counts None: every row).  -> bool [n]."""
+    if counts is None:
+        return torch.ones(n, dtype=torch.bool)
+    i = torch.arange(n)
+    return (i % group) < torch.as_tensor(counts, dtype=torch.int64)[i // group]
+
+
+def net_forward_rows(L, net, patches, counts=None, group=0, ws_word=None):
+    """ag_affnet_forward / ag_orinet_forward / ag_hardnet_forward called directly on CUDA patches [n,1,32,32] with the net's current
+    engine: `counts` (list of ints, one per group of `group` rows; None = NULL count array) is uploaded as the device int32 array, the
+    workspace of ag_net_workspace_bytes(kind, n) bytes is owned here and filled with `ws_word` (see poisoned), and the outputs start
+    as SENTINEL.  Returns (out, angle): out [n,2,2] (AffNet, OriNet) or [n,128] (HardNet); angle [n] for OriNet (both outputs are
+    requested), else None."""
+    lib = L.lib()
+    n = patches.size(0)
+    P = patches.to("cuda", torch.float32).contiguous()
+    nbytes = lib.ag_net_workspace_bytes(net.KIND, n)
+    ws = poisoned(nbytes, ws_word)
+    cnt = None if counts is None else torch.tensor(counts, dtype=torch.int32, device="cuda")
+    out = torch.full((n, 128) if net.KIND == L.NET_HARDNET else (n, 2, 2), SENTINEL, device="cuda")
+    angle = torch.full((n,), SENTINEL, device="cuda") if net.KIND == L.NET_ORINET else None
+    if net.KIND == L.NET_AFFNET:
+        rc = lib.ag_affnet_forward(net.handle(), L.ptr(P), n, L.ptr(cnt), group, L.ptr(out), L.ptr(ws), nbytes, L.stream_ptr())
+    elif net.KIND == L.NET_ORINET:
+        rc = lib.ag_orinet_forward(net.handle(), L.ptr(P), n, L.ptr(cnt), group, L.ptr(out), L.ptr(angle), L.ptr(ws), nbytes, L.stream_ptr())
+    else:
+        rc = lib.ag_hardnet_forward(net.handle(), L.ptr(P), n, L.ptr(cnt), group, L.ptr(out), L.ptr(ws), nbytes, L.stream_ptr())
+    L.check(rc)
+    torch.cuda.synchronize()
+    return out, angle
+
+
+def net_forward_pyr(L, net, plan, pyr, lafs, octs, lvls, counts, cap, ws_word=None):
+    """ag_net_forward_pyr over a pyramid (plan, flat buffer) with LAFs [B*cap,2,3] normalised, octave / level indices [B*cap] and the
+    per-image counts (list of B ints; None = NULL), over a workspace filled with `ws_word`, into an output prefilled with SENTINEL.
+    Returns (rc, out): the call's return code is handed back unchecked."""
+    import ctypes as C
+    lib = L.lib()
+    n = plan.B * cap
+    nbytes = lib.ag_net_workspace_bytes(net.KIND, n)
+    ws = poisoned(nbytes, ws_word)
+    cnt = None if counts is None else torch.tensor(counts, dtype=torch.int32, device="cuda")
+    d = lambda t, dt: t.to("cuda", dt).contiguous()  # noqa: E731
+    dl, do, dv = d(lafs, torch.float32), d(octs, torch.int32), d(lvls, torch.int32)
+    out = torch.full((n, 128) if net.KIND == L.NET_HARDNET else (n, 2, 2), SENTINEL, device="cuda")
+    rc = lib.ag_net_forward_pyr(net.handle(), C.byref(plan), L.ptr(pyr), L.ptr(dl), L.ptr(do), L.ptr(dv), L.ptr(cnt), cap, L.ptr(out),
+                                L.ptr(ws), nbytes, L.stream_ptr())
+    torch.cuda.synchronize()
+    return rc, out
+
 
 def synthetic_image(H, W, seed):
     """SURVEY.md §8(d) config 3 input: U[0,255) noise blurred with sigma=2 (separable, replicate border), stretched to 0..255.
