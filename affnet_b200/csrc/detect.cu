@@ -997,7 +997,7 @@ __global__ void __launch_bounds__(SNT) select_kernel(const SelectParams P) {
     int* s_idx = reinterpret_cast<int*>(smem_raw + sizeof(unsigned long long) * P.sort_cap);
     __shared__ int s_hist[256];
     __shared__ unsigned s_accept;  // bit per slot
-    __shared__ int s_misc[4];      // 0: sorted mode, 1: m (number to select), 2: still needed inside the chosen digit / done flag (rank 0), 3: fill counter (rank 0)
+    __shared__ int s_misc[4];      // 0: sorted mode, 1: m (number to select), 2: radix select needed, 3: fill counter (rank 0)
     __shared__ unsigned long long s_prefix;   // rank 0 publishes the radix prefix here
     __shared__ int s_ctl[2];       // rank 0: [0] remaining, [1] done
 
@@ -1028,6 +1028,9 @@ __global__ void __launch_bounds__(SNT) select_kernel(const SelectParams P) {
         if (m > n) m = n;
         s_misc[0] = sorted;
         s_misc[1] = (int)m;
+        // Unsorted mode takes every valid key unless out_cap leaves room for fewer than all of them: then the radix select picks
+        // the m lowest seqs (unsorted keys order by ascending seq), so the sort buffer never receives more keys than it holds.
+        s_misc[2] = sorted || m < total;
         s_misc[3] = 0;
         s_prefix = 0ull;
         s_ctl[0] = (int)m; s_ctl[1] = 0;
@@ -1036,6 +1039,7 @@ __global__ void __launch_bounds__(SNT) select_kernel(const SelectParams P) {
     const unsigned accept = s_accept;
     const bool sorted = s_misc[0] != 0;
     const int m = s_misc[1];
+    const bool radix = s_misc[2] != 0;
 
     auto key_of = [&](int i) -> unsigned long long {
         const uint32_t sq = seq[i];
@@ -1047,8 +1051,8 @@ __global__ void __launch_bounds__(SNT) select_kernel(const SelectParams P) {
     const uint32_t r0_prefix = dsmem_addr(&s_prefix, 0), r0_ctl = dsmem_addr(s_ctl, 0);
     const uint32_t r0_fill = dsmem_addr(&s_misc[3], 0), r0_key = dsmem_addr(s_key, 0), r0_idx = dsmem_addr(s_idx, 0);
 
-    unsigned long long kth = 1ull;   // unsorted mode: every valid key (>= 1) is taken
-    if (m > 0 && sorted) {
+    unsigned long long kth = 1ull;   // unsorted mode with room for all: every valid key (>= 1) is taken
+    if (m > 0 && radix) {
         // radix select of the m-th largest key, 8 bits per pass from the top; candidates are dealt round-robin to the CTAs of the cluster
         unsigned long long prefix = 0ull;
         for (int pass = 7; pass >= 0; pass--) {

@@ -119,6 +119,10 @@ int ag_detect_level_from_responses(const float* d_low, const float* d_cur, const
  * levels with <=1 positive response are dropped; if more than num_features candidates remain the
  * top num_features by (response desc, seq asc) are returned sorted, otherwise all in
  * (octave, level, raster) order.  num_features <= 0 returns everything (capacity permitting).
+ * out_cap bounds the rows written: when it is below the number the rule above selects, the first out_cap rows of that answer
+ * are returned in the same order (the out_cap highest by (response desc, seq asc) when sorted, else the out_cap first in
+ * (octave, level, raster) order), deterministically.  min(num_features, out_cap) (out_cap when num_features <= 0) may not
+ * exceed 16384 (shared-memory sort): larger requests return AG_ERR_CAPACITY and write nothing.
  * a_scale multiplies the A part of the LAF (mrSize; SparseImgRepresenter.py:198).
  * Outputs [B, out_cap(,..)]: resp, LAFs (normalised), octave idx, level idx (= detection level-1); d_count[b] = -1 if the
  * candidate list of image b overflowed ws->cand_cap (the caller should retry with a larger capacity). */

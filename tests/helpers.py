@@ -185,3 +185,119 @@ def orientation_boundary_shares(patches, tol_bins=1e-4, num_bins=36):
     w = (mag.flatten(1) / float(PS * PS)) / top[:, :1]
     share = torch.where(dist < tol_bins, w, torch.zeros_like(w)).amax(dim=1)
     return margin, share
+
+
+# ---- detector stage: pyramids no blur would produce, and the oracle's keypoints in the selection's order ----------------------------
+SEQ_PIX_BITS = 27                           # candidate seq = (level slot << 27) | flat pixel index (include/affnet_b200.h)
+ADV_H = ADV_W = 40                          # adversarial pyramids: plan(40, 40, border 5) has octaves 40x40 and 20x20
+
+
+def _bump_levels(g, n, h, w, lo, span, max_sigma):
+    yy, xx = torch.meshgrid(torch.arange(h).float(), torch.arange(w).float(), indexing="ij")
+    levels = []
+    for _ in range(n):
+        k = int(torch.randint(0, 3, (1,), generator=g))
+        img = torch.full((h, w), 10.0)
+        for _ in range(k):
+            cy, cx = (torch.rand(2, generator=g) * span + lo).tolist()
+            s = float(torch.rand(1, generator=g) * (max_sigma - 1.0) + 1.0)
+            a = float(torch.rand(1, generator=g) * 60 + 1)
+            img += a * torch.exp(-((yy - cy) ** 2 + (xx - cx) ** 2) / (2 * s * s))
+        levels.append(img.view(1, 1, h, w))
+    return levels
+
+
+def adversarial_pyramid(seed, nlevels=3):
+    """A pyramid for plan(B, 40, 40, nlevels, 1.6, 5) that drives the level-drop rule: every level of octave 0 is a constant 10 plus 0-2
+    Gaussian bumps (sigma 1-3, amplitude 1-61, centres in [8, 32)), so levels with 0, 1 or 2 positive maxima, negative masked responses
+    and wrapping uint8 octave maps all occur.  Octave 1 (20x20) is constant or gets its own bumps.  -> pyr[o][l] float32 [1,1,h,w]."""
+    g = torch.Generator().manual_seed(seed)
+    n = nlevels + 2
+    oct0 = _bump_levels(g, n, ADV_H, ADV_W, 8.0, 24.0, 3.0)
+    h1, w1 = (ADV_H + 1) // 2, (ADV_W + 1) // 2
+    if int(torch.randint(0, 2, (1,), generator=g)):
+        oct1 = [torch.full((1, 1, h1, w1), 10.0) for _ in range(n)]
+    else:
+        oct1 = _bump_levels(g, n, h1, w1, 4.0, 12.0, 2.0)
+    return [oct0, oct1]
+
+
+def detector_level_stats(octave, sigmas, mrSize, th=0.0):
+    """Per detection level of one octave, from the oracle's primitives (HandCraftedModules.py:240-263): (n_pos, accepted, has negative
+    masked responses, octave map wrapped).  n_pos <= 1 drops the level; 'wrapped' means some pixel's uint8 map value came out below
+    the float sum it truncates (Q4)."""
+    import affnet_oracle as O
+    h, w = octave[0].size(2), octave[0].size(3)
+    maps = [torch.clamp(O.hessian_response(octave[l], sigmas[l]) - th, min=0) for l in range(len(octave))]
+    om = np.zeros((h, w), np.uint8)
+    b = int(mrSize)
+    out = []
+    for l in range(1, len(octave) - 1):
+        nm = O.nms3d_mask(maps[l - 1], maps[l], maps[l + 1]).clone()
+        if b < w and b < h:
+            nm[:, :, :b, :] = 0; nm[:, :, h - b:, :] = 0; nm[:, :, :, :b] = 0; nm[:, :, :, w - b:] = 0
+        else:
+            nm = nm * 0
+        nm = nm * (1.0 - torch.from_numpy(om.astype(np.float32)).view(1, 1, h, w))
+        n_pos = int((nm > 0).sum())
+        neg = bool((nm < 0).any())
+        r, _, om2, _ = O.nms3d_and_compose(maps[l - 1], maps[l], maps[l + 1], 0, om, sigmas[l - 1:l + 2], mrSize)
+        wrapped = r is not None and bool((om2.astype(np.float64) < np.trunc((om.astype(np.float64) + nm.numpy().reshape(h, w)).clip(0))).any())
+        out.append((n_pos, r is not None, neg, wrapped))
+        om = om2
+    return out
+
+
+class OracleCandidates:
+    """Every keypoint the oracle emits for one image before its global top-k (num_features <= 0: per-level raster order, octave after
+    octave, level after level), with each one's seq; select(nf) applies the selection rule the C ABI documents: the top nf by (response
+    descending, seq ascending) when more than nf remain or a level was trimmed, otherwise all in seq order.  An image without an accepted
+    level has no candidates (the oracle, like the reference, raises from torch.cat there)."""
+
+    def __init__(self, pyr, sigmas, mrSize, th=0.0):
+        import affnet_oracle as O
+        self.pyr, self.sigmas, self.mrSize, self.th = pyr, sigmas, mrSize, th
+        n_det = len(pyr[0]) - 2
+        try:
+            self.resp, self.lafs, self.oct, self.lvl, dump = O.multi_scale_detector(pyr, sigmas, 0, mrSize, th=th, return_levels=True)
+        except ValueError:                  # torch.cat of an empty list: no level of any octave was accepted
+            self.resp, self.lafs, dump = torch.zeros(0), torch.zeros(0, 2, 3), [(o, l, None, None) for o in range(len(pyr)) for l in range(1, n_det + 1)]
+            self.oct = self.lvl = torch.zeros(0)
+        self.accepted = {(o, l - 1): idxs is not None for (o, l, idxs, _) in dump}
+        self.n_pos = [int((r > 0).sum()) for (_, _, idxs, r) in dump if idxs is not None]
+        self.seq = torch.cat([((o * n_det + l - 1) << SEQ_PIX_BITS) + idxs for (o, l, idxs, _) in dump if idxs is not None] or [torch.zeros(0, dtype=torch.int64)])
+        self.total = self.resp.numel()
+
+    def order(self, nf):
+        trimmed = nf > 0 and any(nf < p for p in self.n_pos)
+        if nf > 0 and (self.total > nf or trimmed):
+            return np.lexsort((self.seq.numpy(), -self.resp.double().numpy()))[:nf], True
+        return np.arange(self.total), False
+
+    def select(self, nf):
+        """-> (resp, lafs, oct, lvl, seq, sorted)."""
+        idx, srt = self.order(nf)
+        idx = torch.from_numpy(np.ascontiguousarray(idx)).long()
+        return self.resp[idx], self.lafs[idx], self.oct[idx], self.lvl[idx], self.seq[idx], srt
+
+    def check_against_oracle(self, nf):
+        """select(nf) must be what O.multi_scale_detector(.., nf, ..) returns, up to the order of equal responses: the same values in the
+        same order, and the same keypoint wherever the value is unique among all candidates.  Returns the number of tie groups that
+        straddle the cut (some members selected, some not)."""
+        import affnet_oracle as O
+        r, la, po, lo = self.select(nf)[:4]
+        try:
+            r_o, L_o, p_o, l_o = O.multi_scale_detector(self.pyr, self.sigmas, nf, self.mrSize, th=self.th)
+        except ValueError:
+            r_o = L_o = p_o = l_o = None
+        if self.total == 0:
+            assert r_o is None
+            return 0
+        assert torch.equal(r, r_o), (nf, r.numel(), r_o.numel())
+        vals, counts = torch.unique(self.resp, return_counts=True)
+        multi = vals[counts > 1]
+        uniq = ~torch.isin(r, multi)
+        assert torch.equal(la[uniq], L_o[uniq]) and torch.equal(po[uniq], p_o[uniq]) and torch.equal(lo[uniq], l_o[uniq]), nf
+        sel_vals, sel_counts = torch.unique(r, return_counts=True)
+        all_counts = dict(zip(vals.tolist(), counts.tolist()))
+        return sum(1 for v, c in zip(sel_vals.tolist(), sel_counts.tolist()) if all_counts[v] > c)
