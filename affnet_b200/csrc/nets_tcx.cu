@@ -1,7 +1,8 @@
 // Second-generation tensor-core engine of AffNet / OriNet / HardNet (tcx_first.cuh, tcx_conv.cuh): row tiles without x padding, the
 // three taps of a kernel row stacked along N, x shifts by warp shuffles in the epilogue.  Replaces the conv stacks of
 // architectures.py:207-235 / 36-82 and HardNet.py:67-101 (BatchNorm folded, ReLU fused); the 8x8 heads stay the GEMM kernels of
-// tc_head.cuh (same head-operand layout).  Per net:  tcx_first_kernel (sampler + input_norm + conv1 + conv2)  ->  tcx_conv_kernel x4.
+// tc_head.cuh (same head-operand layout).  Per net:  AffNet / OriNet  tcx_first_kernel (sampler + input_norm + conv1 + conv2 + conv3)
+// ->  tcx_conv_kernel x3;  HardNet  tcx_first_kernel (sampler + input_norm + conv1 + conv2)  ->  tcx_conv_kernel x4.
 // Numerics: AffNet / OriNet with fp16 residual planes of weights and activations in every layer (three MMAs per K step, fp32-grade);
 // HardNet fp16 activations, weights with their fp16 residual in layers 2 and 3 (emulation on the 2000 graf patches: plain fp16 weights give a
 // descriptor error of 1.1e-3, dominated by the weight rounding of the early layers; with the residuals of layers 2-3 the parity tests hold
@@ -70,19 +71,23 @@ static int launch_conv(const void* in, void* out, const __half* w, const float* 
     return AG_OK;
 }
 
-template <int C1, int COUT, int SA, int SW, int OSA, int BF = 0>
-static int launch_first(void* out, const __half* w, const float* b, float inv_scale, int n, int group, const int* count, cudaStream_t st, const FirstSrc& src) {
-    using Cfg = XFirstCfg<C1, COUT, SA, SW, OSA>;
-    auto kern = tcx_first_kernel<C1, COUT, SA, SW, OSA, BF>;
+// L3 = 1: layer 3 as well, with weights w3 / bias b3, into out3 (out is then unused)
+template <int C1, int COUT, int SA, int SW, int OSA, int BF = 0, int L3 = 0>
+static int launch_first(void* out, const __half* w, const float* b, float inv_scale, int n, int group, const int* count, cudaStream_t st, const FirstSrc& src,
+                        void* out3 = nullptr, const __half* w3 = nullptr, const float* b3 = nullptr, float inv_scale3 = 0.f) {
+    using Cfg = XFirstCfg<C1, COUT, SA, SW, OSA, L3>;
+    auto kern = tcx_first_kernel<C1, COUT, SA, SW, OSA, BF, L3>;
     static bool configured[64] = {};
     int rc = ensure_smem_attr((const void*)kern, (int)Cfg::SMEM, configured, "tcx_first smem attr");
     if (rc != AG_OK) return rc;
     XArgs a;
     a.in = nullptr; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.n = n; a.group = group; a.count = count;
+    XArgs a3 = a;
+    a3.out = out3; a3.wpk = w3; a3.bias = b3; a3.inv_scale = inv_scale3;
     int gx = num_sms();
     if (gx > n) gx = n;
     if (gx < 1) gx = 1;
-    kern<<<gx, Cfg::THREADS, Cfg::SMEM, st>>>(a, src);
+    kern<<<gx, Cfg::THREADS, Cfg::SMEM, st>>>(a, src, a3);
     AG_CHECK_LAUNCH("tcx_first_kernel");
     return AG_OK;
 }
@@ -93,17 +98,12 @@ __global__ void tcx_decode_kernel(const __half* __restrict__ buf, int layout, in
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const int x = (int)(i % H), y = (int)((i / H) % H), c = (int)((i / ((size_t)H * H)) % C), pi = (int)(i / ((size_t)H * H * C));
         const int slots = layout_slots(layout);
-        const size_t unit_halfs = (size_t)(C / 8) * slots * 8 * (osa == 1 ? 2 : 1) + (osa == 2 ? (size_t)(C / 8) * slots * 4 : 0);
+        const size_t unit_halfs = (size_t)(C / 8) * slots * 8 * (osa ? 2 : 1);
         const int unit = layout_pair(layout) ? (pi >> 1) : pi;
         const int slot = layout_slot(layout, y, x, pi & 1);
         const __half* ub = buf + (size_t)unit * unit_halfs;
         float v = __half2float(ub[((size_t)(c / 8) * slots + slot) * 8 + (c & 7)]);
-        if (osa == 1) v += __half2float(ub[((size_t)(C / 8 + c / 8) * slots + slot) * 8 + (c & 7)]);
-        if (osa == 2) {   // byte residual planes behind the hi planes
-            const unsigned char* lb = reinterpret_cast<const unsigned char*>(ub) + (size_t)(C / 8) * slots * 16;
-            const unsigned short bits = (unsigned short)(lb[((size_t)(c / 8) * slots + slot) * 8 + (c & 7)] << 8);
-            v += __half2float(__ushort_as_half(bits));
-        }
+        if (osa) v += __half2float(ub[((size_t)(C / 8 + c / 8) * slots + slot) * 8 + (c & 7)]);
         out[i] = v;
     }
 }
@@ -184,39 +184,23 @@ size_t tcx_act_bytes(int n) { return (size_t)(n + 1) * 65536; }
 #ifndef AG_HARD_MC6
 #define AG_HARD_MC6 0
 #endif
-// Residual planes of layer 2's output (the largest activation, read by the HBM-bound layer 3) as bytes (1) or fp16 (0).  With byte
-// planes AffNet's A stays at 4.5e-6 of the oracle and layer 3 reads less.  OFF by default: the application test with the hand-crafted
-// orientation (test_graf_1_to_6_application_counts[hcori]) then has one keypoint of 2996 whose frame differs from the oracle's by more
-// than its near-tie accounting allows (a pixel on a histogram-bin boundary, DESIGN.md section 8).  OriNet's angle error grows from
-// 3e-5 to 1.2e-4 rad with byte planes (its atan2 amplifies): off for OriNet as well.
-#ifndef AG_AFF_LO8
-#define AG_AFF_LO8 0
-#endif
-#ifndef AG_ORI_LO8
-#define AG_ORI_LO8 0
-#endif
-static inline int tcx_lox(const ag_net* net) { return ((net->kind == AG_NET_AFFNET) ? AG_AFF_LO8 : AG_ORI_LO8) ? 2 : 1; }
-template <int LOX>
-static int trunk_affori_t(const ag_net* net, const tc::FirstSrc& src0, int n, int group, const int* count, void* bufA, void* bufB, void* feat,
-                          cudaStream_t st, int upto) {
+// Layers 1-3 run in one kernel (layer 2's 32x32 output stays in shared memory).  upto = 2 runs the layers 1-2 kernel instead, which
+// writes layer 2's output to bufB for the debug decode.
+int tcx_trunk_affori(const ag_net* net, const tc::FirstSrc& src0, int n, int group, const int* count, void* bufA, void* bufB, void* feat,
+                     cudaStream_t st, int upto) {
     using namespace tcx;
     tc::FirstSrc src = src0;
     src.w1 = net->d_w1; src.b1 = net->d_b[0]; src.w1_inv = net->w_inv_scale[0]; src.w1_scale = 1.0f / net->w_inv_scale[0];
     int rc;
-    if ((rc = launch_first<16, 16, 1, 1, LOX>(bufB, net->d_wx[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, src))) return rc;
-    if (upto <= 2) return AG_OK;
-    if ((rc = launch_conv<16, 32, 32, 2, 1, 3, L_S1_16, LOX, 1, 1>(bufB, bufA, net->d_wx[2], net->d_b[2], net->w_inv_scale[2], n, group, count, st))) return rc;
+    if (upto <= 2) return launch_first<16, 16, 1, 1, 1>(bufB, net->d_wx[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, src);
+    if ((rc = launch_first<16, 16, 1, 1, 1, 0, 1>(nullptr, net->d_wx[1], net->d_b[1], net->w_inv_scale[1], n, group, count, st, src,
+                                                   bufA, net->d_wx[2], net->d_b[2], net->w_inv_scale[2]))) return rc;
     if (upto <= 3) return AG_OK;
     if ((rc = launch_conv<32, 32, 16, 1, 1, 4, L_S2_8P, 1, 1, 1>(bufA, bufB, net->d_wx[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
     if (upto <= 4) return AG_OK;
     if ((rc = launch_conv<32, 64, 16, 2, 1, 2, L_S1_8P, 1, 1, 1>(bufB, bufA, net->d_wx[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
     if (upto <= 5) return AG_OK;
     return launch_conv<64, 64, 8, 1, 1, 2, L_HEAD, 1, 1, 1>(bufA, feat, net->d_wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
-}
-int tcx_trunk_affori(const ag_net* net, const tc::FirstSrc& src0, int n, int group, const int* count, void* bufA, void* bufB, void* feat,
-                     cudaStream_t st, int upto) {
-    return tcx_lox(net) == 2 ? trunk_affori_t<2>(net, src0, n, group, count, bufA, bufB, feat, st, upto)
-                             : trunk_affori_t<1>(net, src0, n, group, count, bufA, bufB, feat, st, upto);
 }
 
 template <int BF>
@@ -270,8 +254,7 @@ int ag_debug_tcx_layer(const ag_net_t* net, const float* d_patches, int n, int u
     const int Cb = hard ? 32 : 16;
     const int C = upto == 2 ? Cb : (upto <= 4 ? 2 * Cb : 4 * Cb);
     const void* buf = (upto == 2 || upto == 4) ? base + act : base;
-    // the planes layer 2 writes carry byte residuals when the net uses them (tcx_lox)
-    const int osa = hard ? 0 : (upto == 2 ? tcx_lox(net) : 1);
+    const int osa = hard ? 0 : 1;
     tcx::tcx_decode_kernel<<<296, 256, 0, st>>>((const __half*)buf, lay, C, osa, H, n, d_out);
     AG_CHECK_LAUNCH("tcx_decode_kernel");
     return AG_OK;

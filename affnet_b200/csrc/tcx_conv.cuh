@@ -26,8 +26,8 @@
 //   L_HEAD   the 8x8 head GEMM's A operand (tc_head.cuh): [patch/128][pixel*C/8 + c/8][patch%128][8] (+ a residual plane behind it)
 //
 // Warp roles: 0-7 two consumer warpgroups (warpgroup g takes the M = 64 blocks g, g + 2, ... of a unit: wgmma into registers, then the
-// epilogue from the accumulator fragment) | 8 loader (cp.async.bulk per channel group and plane) | 9-12 converters of byte residual
-// planes (SA = 2 only).
+// epilogue from the accumulator fragment) | 8 loader (cp.async.bulk per channel group and plane).  The MMAs and the epilogue of one
+// block are xconv_block_mma / xconv_block_epilogue, which tcx_first_kernel also runs for layer 3 of AffNet / OriNet.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -96,18 +96,6 @@ __device__ __forceinline__ void split_pack2(float v0, float v1, uint32_t& hi, ui
     } else lo = 0;
 }
 
-// Byte residual planes (SA / OSA = 2): the fp16 residual rounded to its high byte (= e5m2).  Emulation (scripts/emu_residual_bits.py):
-// AffNet's output moves by 5e-6 when the residual of an activation keeps 2 mantissa bits (budget 5e-5), so the planes that cross HBM
-// in front of the bandwidth-bound stride-2 layers are stored at half the size and expanded in shared memory by the consumer.
-__device__ __forceinline__ uint2 pack_lo8(const uint4& lo) {
-    const uint32_t t0 = lo.x + 0x00800080u, t1 = lo.y + 0x00800080u, t2 = lo.z + 0x00800080u, t3 = lo.w + 0x00800080u;   // round the magnitude to 8 bits
-    return make_uint2(__byte_perm(t0, t1, 0x7531), __byte_perm(t2, t3, 0x7531));
-}
-
-__device__ __forceinline__ uint16_t pack_lo8_2(uint32_t lo) {   // pack_lo8 of one pair
-    return (uint16_t)(__byte_perm(lo + 0x00800080u, 0u, 0x0031) & 0xFFFFu);
-}
-
 // slots per channel group and unit of an HBM activation layout, and patches per unit
 __host__ __device__ constexpr int layout_slots(int lay) { return lay == L_S2_16 ? 1024 : lay == L_S1_16 ? 256 : lay == L_S2_8P ? 512 : 128; }
 __host__ __device__ constexpr int layout_pair(int lay) { return (lay == L_S2_8P || lay == L_S1_8P) ? 1 : 0; }
@@ -146,33 +134,31 @@ struct XArgs {
     const int* count;     // valid patches per image (NULL: all)
 };
 
-// SA: input hi/lo planes (2: the lo planes arrive as bytes); SW: weight hi/lo copies; OSA: write hi/lo planes (2: lo as bytes).  OUT: layout of the output buffer.
+// SA: input hi/lo planes; SW: weight hi/lo copies; OSA: write hi/lo planes.  OUT: layout of the output buffer.
 template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA>
 struct XCfg {
     using In = XIn<H, STRIDE>;
+    static constexpr int CO = COUT, STRD = STRIDE, OUTL = OUT, SPLIT_A = SA, SPLIT_W = SW, SPLIT_O = OSA;   // for the block functions below
     static constexpr int KC = CIN / 8, NT = COUT / NSPLIT, HOUT = In::HOUT;
-    static constexpr int HAS_LO = SA ? 1 : 0, LO8 = (SA == 2) ? 1 : 0;      // SA = 2: the residual planes arrive as bytes
-    static constexpr int G = KC * (1 + HAS_LO);                               // channel groups of one unit (in shared memory)
+    static constexpr int G = KC * (1 + SA);                                   // channel groups of one unit (in shared memory)
     static constexpr int GS = STAGES * In::SLOT_STAGE + (STRIDE == 1 ? In::RW : 0);   // slots per channel group in shared memory
     static constexpr int ACCW = 3 * NT;                                        // accumulator columns of one block
     static constexpr int BLOCKS = 2 * In::TILES;                               // M = 64 blocks of one unit
     static constexpr uint32_t W_BYTES = 9u * CIN * NT * 2u * (1 + SW);         // per split
     static constexpr uint32_t IN_BYTES = (uint32_t)G * GS * 16u;               // all stages
     static constexpr uint32_t HI_IN_BYTES = (uint32_t)KC * In::NPLANES * In::DATA * 16u;
-    static constexpr uint32_t UNIT_IN_BYTES = HI_IN_BYTES + (SA == 1 ? HI_IN_BYTES : SA == 2 ? HI_IN_BYTES / 2 : 0u);   // one unit in HBM
-    static constexpr int NCONV = 4;                                            // LO8: converter warps (one alone was the new critical path: 32 dependent steps per unit)
-    static constexpr int THREADS = 288 + 32 * NCONV * LO8;
+    static constexpr uint32_t UNIT_IN_BYTES = HI_IN_BYTES * (1 + SA);        // one unit in HBM
+    static constexpr int THREADS = 288;
     static constexpr size_t SMEM = 1024 + (size_t)W_BYTES + IN_BYTES;
     static constexpr size_t HI_OUT_BYTES = (size_t)(COUT / 8) * layout_slots(OUT) * 16;
-    static constexpr size_t UNIT_OUT_BYTES = (OUT == L_HEAD) ? 0 : HI_OUT_BYTES + (OSA == 1 ? HI_OUT_BYTES : OSA == 2 ? HI_OUT_BYTES / 2 : 0);
+    static constexpr size_t UNIT_OUT_BYTES = (OUT == L_HEAD) ? 0 : HI_OUT_BYTES * (1 + OSA);
     // weight rows per K group of one (dy, k step) block
     static constexpr int NR1 = (1 + SW) * 3 * NT;                              // stride 1: [hi: dx0 dx1 dx2][lo: dx0 dx1 dx2]
     static constexpr int NRO = (1 + SW) * 2 * NT, NRE = (1 + SW) * NT;         // stride 2: odd-x plane [hi: dx0 dx2][lo: ...], even-x plane [hi: dx1][lo: dx1]
     static_assert(CIN % 16 == 0 && NT % 16 == 0 && ACCW <= 256, "wgmma shape");
     static_assert(In::W == 8 || In::W == 16, "a warp's 16 accumulator rows hold whole image rows");
-    static_assert(3 * STAGES + 1 <= 60, "barrier area");
-    static_assert(!LO8 || (STRIDE == 2 && In::DATA % 64 == 0), "byte residual planes: stride-2 consumers");
-    static_assert(OSA != 2 || OUT == L_S2_16 || OUT == L_S2_8P, "byte residual planes are written for stride-2 consumers");
+    static_assert(SA <= 1 && SW <= 1 && OSA <= 1, "split-precision switches are 0 | 1");
+    static_assert(2 * STAGES + 1 <= 60, "barrier area");
     static_assert(SMEM <= 232448, "shared memory budget");
     static_assert(GS < 16384, "leading-byte offset field");
     static_assert(OUT == L_HEAD || layout_pair(OUT) || !In::PAIR, "a pair layer writes pair layouts or the head operand");
@@ -194,22 +180,145 @@ __device__ __forceinline__ void frag_right(float v0, float v1, int lane, float& 
     r1 = t1;
 }
 
+__device__ __forceinline__ bool xpatch_valid(const XArgs& a, int pi) { return pi < a.n && (a.count == nullptr || (pi % a.group) < a.count[pi / a.group]); }
+
+// The MMAs of one M = 64 block of a layer (Cfg: XCfg) into d[ACCW / 2]: a_t = the block's first slot in shared memory, w_base = the
+// layer's packed weights (both in 16-byte units).  The input's channel groups are Cfg::GS slots apart.  Used by tcx_conv_kernel and by
+// the layer-3 stage of tcx_first_kernel.
+template <class Cfg, int BF>
+__device__ __forceinline__ void xconv_block_mma(float* d, uint32_t a_t, uint32_t w_base) {
+    using In = typename Cfg::In;
+    constexpr int KC = Cfg::KC, NT = Cfg::NT, GS = Cfg::GS, RW = In::RW, SA = Cfg::SPLIT_A, SW = Cfg::SPLIT_W;
+    constexpr uint32_t LBO_A = ((uint32_t)GS) << 16;      // (bytes >> 4) << 16
+    wgmma_fence();
+    if (Cfg::STRD == 1) {
+#pragma unroll
+        for (int dy = 0; dy < 3; dy++) {
+#pragma unroll
+            for (int j = 0; j < KC / 2; j++) {
+                const uint32_t ahi = ((a_t + (uint32_t)(dy * RW + 2 * j * GS)) & 0x3FFFu) | LBO_A;
+                const uint32_t alo = ((a_t + (uint32_t)(dy * RW + (KC + 2 * j) * GS)) & 0x3FFFu) | LBO_A;
+                const uint32_t blk = w_base + (uint32_t)((dy * (KC / 2) + j) * 2 * Cfg::NR1);
+                const uint32_t bhi = (blk & 0x3FFFu) | ((uint32_t)Cfg::NR1 << 16), blo = ((blk + 3 * NT) & 0x3FFFu) | ((uint32_t)Cfg::NR1 << 16);
+                Wgmma<3 * NT, BF>::mma(d, desc64(ahi), desc64(bhi), (dy | j) != 0);
+                if (SW) Wgmma<3 * NT, BF>::mma(d, desc64(ahi), desc64(blo), 1);
+                if (SA) Wgmma<3 * NT, BF>::mma(d, desc64(alo), desc64(bhi), 1);
+            }
+        }
+    } else {
+#pragma unroll
+        for (int dy = 0; dy < 3; dy++) {
+            constexpr int PL = In::PLANE;
+            const int py = (dy == 1) ? 0 : 1, ro = (dy == 0) ? 0 : 1;
+#pragma unroll
+            for (int j = 0; j < KC / 2; j++) {
+                const uint32_t blk = w_base + (uint32_t)((dy * (KC / 2) + j) * 2 * (Cfg::NRO + Cfg::NRE));
+                const uint32_t bo_hi = (blk & 0x3FFFu) | ((uint32_t)Cfg::NRO << 16), bo_lo = ((blk + 2 * NT) & 0x3FFFu) | ((uint32_t)Cfg::NRO << 16);
+                const uint32_t be = blk + 2 * Cfg::NRO;
+                const uint32_t be_hi = (be & 0x3FFFu) | ((uint32_t)Cfg::NRE << 16), be_lo = ((be + NT) & 0x3FFFu) | ((uint32_t)Cfg::NRE << 16);
+                // odd-x plane (px = 1): taps dx = 0 and dx = 2 -> columns [0, 2 NT)
+                const uint32_t ao = a_t + (uint32_t)((py * 2 + 1) * PL + ro * RW);
+                const uint32_t ao_hi = ((ao + (uint32_t)(2 * j * GS)) & 0x3FFFu) | LBO_A, ao_lo = ((ao + (uint32_t)((KC + 2 * j) * GS)) & 0x3FFFu) | LBO_A;
+                Wgmma<2 * NT, BF>::mma(d, desc64(ao_hi), desc64(bo_hi), (dy | j) != 0);
+                if (SW) Wgmma<2 * NT, BF>::mma(d, desc64(ao_hi), desc64(bo_lo), 1);
+                if (SA) Wgmma<2 * NT, BF>::mma(d, desc64(ao_lo), desc64(bo_hi), 1);
+                // even-x plane (px = 0): tap dx = 1 -> columns [2 NT, 3 NT) = fragment registers from NT on
+                const uint32_t ae = a_t + (uint32_t)((py * 2 + 0) * PL + ro * RW);
+                const uint32_t ae_hi = ((ae + (uint32_t)(2 * j * GS)) & 0x3FFFu) | LBO_A, ae_lo = ((ae + (uint32_t)((KC + 2 * j) * GS)) & 0x3FFFu) | LBO_A;
+                Wgmma<NT, BF>::mma(d + NT, desc64(ae_hi), desc64(be_hi), (dy | j) != 0);
+                if (SW) Wgmma<NT, BF>::mma(d + NT, desc64(ae_hi), desc64(be_lo), 1);
+                if (SA) Wgmma<NT, BF>::mma(d + NT, desc64(ae_lo), desc64(be_hi), 1);
+            }
+        }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence<Cfg::ACCW / 2>(d);
+}
+
+// Epilogue of one block from the accumulator fragment d (xconv_block_mma) of warp wq of a warpgroup: x shifts, bias, ReLU, fp16 hi [+ lo]
+// into a.out in the layout Cfg::OUTL.  Rows r = 64 b + 16 wq + lane/4 + 8 h of unit u, columns 8 j + 2 (lane % 4) + e of each NT block;
+// output channels from split * NT on.
+template <class Cfg, int BF>
+__device__ __forceinline__ void xconv_block_epilogue(const float* d, const XArgs& a, const float* s_bias, int u, int b, int split, int wq, int lane) {
+    using In = typename Cfg::In;
+    constexpr int NT = Cfg::NT, HOUT = Cfg::HOUT, W = In::W, PAIR = In::PAIR, COUT = Cfg::CO, OUT = Cfg::OUTL, OSA = Cfg::SPLIT_O;
+    unsigned char* obase[2];
+    bool has_l[2], has_r[2];      // the left / right neighbour lies inside the image row (else: zero padding)
+    bool ok[2];
+    size_t lo_off = 0;
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const int r = b * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        int y, x, pi;
+        if (PAIR) { y = r >> 4; x = r & 7; pi = 2 * u + ((r >> 3) & 1); }
+        else { y = r / W; x = r - y * W; pi = u; }
+        ok[h] = xpatch_valid(a, pi);
+        has_l[h] = x > 0; has_r[h] = x < W - 1;
+        if (OUT == L_HEAD) {
+            obase[h] = reinterpret_cast<unsigned char*>(a.out) + (((size_t)(pi >> 7) * (HOUT * HOUT * COUT / 8) + (size_t)(y * HOUT + x) * (COUT / 8)) * 128 + (pi & 127)) * 16;
+            lo_off = (size_t)((a.n + 127) >> 7) * (HOUT * HOUT * COUT / 8) * 128 * 16;
+        } else {
+            const int ou = layout_pair(OUT) ? (pi >> 1) : pi;
+            obase[h] = reinterpret_cast<unsigned char*>(a.out) + (size_t)ou * Cfg::UNIT_OUT_BYTES + (size_t)layout_slot(OUT, y, x, pi & 1) * 16;
+            lo_off = (size_t)(COUT / 8) * layout_slots(OUT) * 16;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < NT / 8; j++) {
+        const int c = j * 8 + 2 * (lane & 3);
+        float v[2][2];
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+            // stride 1: blocks dx0 | dx1 | dx2;  stride 2: odd dx0 | odd dx2 | even dx1
+            const float c00 = d[4 * j + e], c01 = d[4 * j + 2 + e];                                   // block 0, rows h = 0 / 1
+            const float c10 = d[4 * (j + NT / 8) + e], c11 = d[4 * (j + NT / 8) + 2 + e];             // block 1
+            const float c20 = d[4 * (j + 2 * NT / 8) + e], c21 = d[4 * (j + 2 * NT / 8) + 2 + e];     // block 2
+            float l0, l1;
+            frag_left(c00, c01, lane, l0, l1);
+            // zero padding by selects: the same roundings as adding the neighbour (fmaf(l, 1, t) == l + t), and a NaN of a
+            // skipped pair partner stays out of the valid patch
+            float acc0, acc1;
+            if (Cfg::STRD == 1) {
+                float r0, r1;
+                frag_right(c20, c21, lane, r0, r1);
+                const float t0 = has_r[0] ? r0 + c10 : c10, t1 = has_r[1] ? r1 + c11 : c11;
+                acc0 = has_l[0] ? l0 + t0 : t0;
+                acc1 = has_l[1] ? l1 + t1 : t1;
+            } else {
+                const float t0 = c10 + c20, t1 = c11 + c21;
+                acc0 = has_l[0] ? l0 + t0 : t0;
+                acc1 = has_l[1] ? l1 + t1 : t1;
+            }
+            v[0][e] = fmaxf(fmaf(acc0, a.inv_scale, s_bias[c + e]), 0.f);
+            v[1][e] = fmaxf(fmaf(acc1, a.inv_scale, s_bias[c + e]), 0.f);
+        }
+        const int ch = split * NT + c;       // output channel of the pair
+        const size_t goff = ((OUT == L_HEAD) ? (size_t)(ch / 8) * 128 * 16 : (size_t)(ch / 8) * layout_slots(OUT) * 16) + (ch & 7) * 2;
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            if (!ok[h]) continue;
+            uint32_t hi, lo;
+            split_pack2<OSA, BF>(v[h][0], v[h][1], hi, lo);
+            *reinterpret_cast<uint32_t*>(obase[h] + goff) = hi;
+            if (OSA) *reinterpret_cast<uint32_t*>(obase[h] + lo_off + goff) = lo;
+        }
+    }
+}
+
 // MC = 1 (NSPLIT = 2 only): the two CTAs of a unit form a thread-block cluster (1 x 2); each loader fetches half of the unit's planes and
 // multicasts them to both, so the input crosses the L2 -> SM fabric once instead of twice.
 template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int BF = 0, int MC = 0>
-__global__ void __launch_bounds__(288 + (SA == 2 ? 128 : 0), 1) tcx_conv_kernel(const XArgs a) {
+__global__ void __launch_bounds__(288, 1) tcx_conv_kernel(const XArgs a) {
     static_assert(MC == 0 || NSPLIT == 2, "multicast pairs the two channel-split CTAs");
     using Cfg = XCfg<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA>;
     using In = typename Cfg::In;
-    constexpr int KC = Cfg::KC, NT = Cfg::NT, ACCW = Cfg::ACCW, BLOCKS = Cfg::BLOCKS, HOUT = Cfg::HOUT, GS = Cfg::GS, RW = In::RW, W = In::W;
+    constexpr int ACCW = Cfg::ACCW, BLOCKS = Cfg::BLOCKS, GS = Cfg::GS, RW = In::RW;
     constexpr int PAIR = In::PAIR;
     extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t* full = reinterpret_cast<uint64_t*>(smem);  // [STAGES]
     uint64_t* empty = full + STAGES;                       // [STAGES]
     uint64_t* wbar = empty + STAGES;
-    uint64_t* cfull = wbar + 1;                            // [STAGES] byte planes of the stage expanded (LO8)
-    constexpr int LO8 = Cfg::LO8;
-    static_assert(!(BF && (SA == 2 || OSA == 2)), "byte residual planes are fp16");
     float* s_bias = reinterpret_cast<float*>(smem + 512);  // [NT]
     unsigned char* sW = smem + 1024;
     unsigned char* sIn = sW + Cfg::W_BYTES;
@@ -218,10 +327,10 @@ __global__ void __launch_bounds__(288 + (SA == 2 ? 128 : 0), 1) tcx_conv_kernel(
     const int split = blockIdx.y;
     const int n_units = PAIR ? (a.n + 1) >> 1 : a.n;
 
-    if (threadIdx.x < NT) s_bias[threadIdx.x] = a.bias[split * NT + threadIdx.x];
+    if (threadIdx.x < Cfg::NT) s_bias[threadIdx.x] = a.bias[split * Cfg::NT + threadIdx.x];
     if (threadIdx.x == 0) {
         // empty: one arrival per consumer warpgroup (MC: of both CTAs, the stage holds planes multicast by both loaders)
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2 * (1 + MC)); mbar_init(&cfull[s], Cfg::NCONV); }
+        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2 * (1 + MC)); }
         mbar_init(wbar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -231,8 +340,7 @@ __global__ void __launch_bounds__(288 + (SA == 2 ? 128 : 0), 1) tcx_conv_kernel(
     __syncthreads();
     if (MC) cluster_sync();      // the peer's barriers are initialised before anything is multicast into this CTA
 
-    auto pvalid = [&](int pi) -> bool { return pi < a.n && (a.count == nullptr || (pi % a.group) < a.count[pi / a.group]); };
-    auto uvalid = [&](int u) -> bool { return PAIR ? (pvalid(2 * u) || pvalid(2 * u + 1)) : pvalid(u); };
+    auto uvalid = [&](int u) -> bool { return PAIR ? (xpatch_valid(a, 2 * u) || xpatch_valid(a, 2 * u + 1)) : xpatch_valid(a, u); };
 
     if (warp == 8) {
         // ===== loader =====
@@ -252,9 +360,7 @@ __global__ void __launch_bounds__(288 + (SA == 2 ? 128 : 0), 1) tcx_conv_kernel(
                     for (int pl = 0; pl < In::NPLANES; pl++) {
                         unsigned char* dst = sIn + ((size_t)g * GS + (size_t)s * In::SLOT_STAGE + (size_t)pl * In::PLANE + RW) * 16;
                         const unsigned char* srcp = gsrc + ((size_t)g * In::NPLANES + pl) * In::DATA * 16;
-                        if (LO8 && g >= KC) {   // byte plane: into the upper half of the fp16 plane's place, expanded there by the converter warps
-                            bulk_g2s(dst + In::DATA * 8, gsrc + Cfg::HI_IN_BYTES + ((size_t)(g - KC) * In::NPLANES + pl) * In::DATA * 8, In::DATA * 8u, &full[s]);
-                        } else if (MC) { if (((g * In::NPLANES + pl) & 1) == split) bulk_g2s_mc(dst, srcp, In::DATA * 16u, &full[s], (uint16_t)3); }
+                        if (MC) { if (((g * In::NPLANES + pl) & 1) == split) bulk_g2s_mc(dst, srcp, In::DATA * 16u, &full[s], (uint16_t)3); }
                         else bulk_g2s(dst, srcp, In::DATA * 16u, &full[s]);
                     }
                 it++;
@@ -269,168 +375,23 @@ __global__ void __launch_bounds__(288 + (SA == 2 ? 128 : 0), 1) tcx_conv_kernel(
         mbar_wait(wbar, 0);
         const uint32_t w_base = smem_u32(sW) >> 4;           // 16-byte units
         const uint32_t in_base = smem_u32(sIn) >> 4;
-        constexpr uint32_t LBO_A = ((uint32_t)GS) << 16;      // (bytes >> 4) << 16
         int it = 0;
         for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
             if (!uvalid(u)) continue;
             const int s = it % STAGES;
-            mbar_wait(LO8 ? &cfull[s] : &full[s], (it / STAGES) & 1);
+            mbar_wait(&full[s], (it / STAGES) & 1);
             const uint32_t st_base = in_base + (uint32_t)(s * In::SLOT_STAGE);
 #pragma unroll 1
             for (int b = wg; b < BLOCKS; b += 2) {
                 float d[ACCW / 2];
-                const uint32_t a_t = st_base + (uint32_t)(b * 64);
-                wgmma_fence();
-                if (STRIDE == 1) {
-#pragma unroll
-                    for (int dy = 0; dy < 3; dy++) {
-#pragma unroll
-                        for (int j = 0; j < KC / 2; j++) {
-                            const uint32_t ahi = ((a_t + (uint32_t)(dy * RW + 2 * j * GS)) & 0x3FFFu) | LBO_A;
-                            const uint32_t alo = ((a_t + (uint32_t)(dy * RW + (KC + 2 * j) * GS)) & 0x3FFFu) | LBO_A;
-                            const uint32_t blk = w_base + (uint32_t)((dy * (KC / 2) + j) * 2 * Cfg::NR1);
-                            const uint32_t bhi = (blk & 0x3FFFu) | ((uint32_t)Cfg::NR1 << 16), blo = ((blk + 3 * NT) & 0x3FFFu) | ((uint32_t)Cfg::NR1 << 16);
-                            Wgmma<3 * NT, BF>::mma(d, desc64(ahi), desc64(bhi), (dy | j) != 0);
-                            if (SW) Wgmma<3 * NT, BF>::mma(d, desc64(ahi), desc64(blo), 1);
-                            if (SA) Wgmma<3 * NT, BF>::mma(d, desc64(alo), desc64(bhi), 1);
-                        }
-                    }
-                } else {
-#pragma unroll
-                    for (int dy = 0; dy < 3; dy++) {
-                        constexpr int PL = In::PLANE;
-                        const int py = (dy == 1) ? 0 : 1, ro = (dy == 0) ? 0 : 1;
-#pragma unroll
-                        for (int j = 0; j < KC / 2; j++) {
-                            const uint32_t blk = w_base + (uint32_t)((dy * (KC / 2) + j) * 2 * (Cfg::NRO + Cfg::NRE));
-                            const uint32_t bo_hi = (blk & 0x3FFFu) | ((uint32_t)Cfg::NRO << 16), bo_lo = ((blk + 2 * NT) & 0x3FFFu) | ((uint32_t)Cfg::NRO << 16);
-                            const uint32_t be = blk + 2 * Cfg::NRO;
-                            const uint32_t be_hi = (be & 0x3FFFu) | ((uint32_t)Cfg::NRE << 16), be_lo = ((be + NT) & 0x3FFFu) | ((uint32_t)Cfg::NRE << 16);
-                            // odd-x plane (px = 1): taps dx = 0 and dx = 2 -> columns [0, 2 NT)
-                            const uint32_t ao = a_t + (uint32_t)((py * 2 + 1) * PL + ro * RW);
-                            const uint32_t ao_hi = ((ao + (uint32_t)(2 * j * GS)) & 0x3FFFu) | LBO_A, ao_lo = ((ao + (uint32_t)((KC + 2 * j) * GS)) & 0x3FFFu) | LBO_A;
-                            Wgmma<2 * NT, BF>::mma(d, desc64(ao_hi), desc64(bo_hi), (dy | j) != 0);
-                            if (SW) Wgmma<2 * NT, BF>::mma(d, desc64(ao_hi), desc64(bo_lo), 1);
-                            if (SA) Wgmma<2 * NT, BF>::mma(d, desc64(ao_lo), desc64(bo_hi), 1);
-                            // even-x plane (px = 0): tap dx = 1 -> columns [2 NT, 3 NT) = fragment registers from NT on
-                            const uint32_t ae = a_t + (uint32_t)((py * 2 + 0) * PL + ro * RW);
-                            const uint32_t ae_hi = ((ae + (uint32_t)(2 * j * GS)) & 0x3FFFu) | LBO_A, ae_lo = ((ae + (uint32_t)((KC + 2 * j) * GS)) & 0x3FFFu) | LBO_A;
-                            Wgmma<NT, BF>::mma(d + NT, desc64(ae_hi), desc64(be_hi), (dy | j) != 0);
-                            if (SW) Wgmma<NT, BF>::mma(d + NT, desc64(ae_hi), desc64(be_lo), 1);
-                            if (SA) Wgmma<NT, BF>::mma(d + NT, desc64(ae_lo), desc64(be_hi), 1);
-                        }
-                    }
-                }
-                wgmma_commit();
-                wgmma_wait<0>();
-                wgmma_reg_fence<ACCW / 2>(d);
-                // ===== epilogue from the fragment: rows r = 64 b + 16 wq + lane/4 + 8 h, columns 8 j + 2 (lane % 4) + e of each NT block =====
-                int pis[2];
-                unsigned char* obase[2];
-                unsigned char* obase8[2];     // OSA = 2: byte residual planes behind the hi planes
-                bool has_l[2], has_r[2];      // the left / right neighbour lies inside the image row (else: zero padding)
-                bool ok[2];
-                size_t lo_off = 0;
-#pragma unroll
-                for (int h = 0; h < 2; h++) {
-                    const int r = b * 64 + wq * 16 + (lane >> 2) + 8 * h;
-                    int y, x, pi;
-                    if (PAIR) { y = r >> 4; x = r & 7; pi = 2 * u + ((r >> 3) & 1); }
-                    else { y = r / W; x = r - y * W; pi = u; }
-                    pis[h] = pi;
-                    ok[h] = pvalid(pi);
-                    has_l[h] = x > 0; has_r[h] = x < W - 1;
-                    if (OUT == L_HEAD) {
-                        obase[h] = reinterpret_cast<unsigned char*>(a.out) + (((size_t)(pi >> 7) * (HOUT * HOUT * COUT / 8) + (size_t)(y * HOUT + x) * (COUT / 8)) * 128 + (pi & 127)) * 16;
-                        lo_off = (size_t)((a.n + 127) >> 7) * (HOUT * HOUT * COUT / 8) * 128 * 16;
-                        obase8[h] = nullptr;
-                    } else {
-                        const int ou = layout_pair(OUT) ? (pi >> 1) : pi;
-                        obase[h] = reinterpret_cast<unsigned char*>(a.out) + (size_t)ou * Cfg::UNIT_OUT_BYTES + (size_t)layout_slot(OUT, y, x, pi & 1) * 16;
-                        lo_off = (size_t)(COUT / 8) * layout_slots(OUT) * 16;
-                        obase8[h] = reinterpret_cast<unsigned char*>(a.out) + (size_t)ou * Cfg::UNIT_OUT_BYTES + Cfg::HI_OUT_BYTES + (size_t)layout_slot(OUT, y, x, pi & 1) * 8;
-                    }
-                }
-                (void)pis;
-#pragma unroll
-                for (int j = 0; j < NT / 8; j++) {
-                    const int c = j * 8 + 2 * (lane & 3);
-                    float v[2][2];
-#pragma unroll
-                    for (int e = 0; e < 2; e++) {
-                        // stride 1: blocks dx0 | dx1 | dx2;  stride 2: odd dx0 | odd dx2 | even dx1
-                        const float c00 = d[4 * j + e], c01 = d[4 * j + 2 + e];                                   // block 0, rows h = 0 / 1
-                        const float c10 = d[4 * (j + NT / 8) + e], c11 = d[4 * (j + NT / 8) + 2 + e];             // block 1
-                        const float c20 = d[4 * (j + 2 * NT / 8) + e], c21 = d[4 * (j + 2 * NT / 8) + 2 + e];     // block 2
-                        float l0, l1;
-                        frag_left(c00, c01, lane, l0, l1);
-                        // zero padding by selects: the same roundings as adding the neighbour (fmaf(l, 1, t) == l + t), and a NaN of a
-                        // skipped pair partner stays out of the valid patch
-                        float acc0, acc1;
-                        if (STRIDE == 1) {
-                            float r0, r1;
-                            frag_right(c20, c21, lane, r0, r1);
-                            const float t0 = has_r[0] ? r0 + c10 : c10, t1 = has_r[1] ? r1 + c11 : c11;
-                            acc0 = has_l[0] ? l0 + t0 : t0;
-                            acc1 = has_l[1] ? l1 + t1 : t1;
-                        } else {
-                            const float t0 = c10 + c20, t1 = c11 + c21;
-                            acc0 = has_l[0] ? l0 + t0 : t0;
-                            acc1 = has_l[1] ? l1 + t1 : t1;
-                        }
-                        v[0][e] = fmaxf(fmaf(acc0, a.inv_scale, s_bias[c + e]), 0.f);
-                        v[1][e] = fmaxf(fmaf(acc1, a.inv_scale, s_bias[c + e]), 0.f);
-                    }
-                    const int ch = split * NT + c;       // output channel of the pair
-                    const size_t goff = ((OUT == L_HEAD) ? (size_t)(ch / 8) * 128 * 16 : (size_t)(ch / 8) * layout_slots(OUT) * 16) + (ch & 7) * 2;
-#pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        if (!ok[h]) continue;
-                        uint32_t hi, lo;
-                        split_pack2<OSA, BF>(v[h][0], v[h][1], hi, lo);
-                        *reinterpret_cast<uint32_t*>(obase[h] + goff) = hi;
-                        if (OSA == 1) *reinterpret_cast<uint32_t*>(obase[h] + lo_off + goff) = lo;
-                        if (OSA == 2) *reinterpret_cast<uint16_t*>(obase8[h] + (size_t)(ch / 8) * layout_slots(OUT) * 8 + (ch & 7)) = pack_lo8_2(lo);
-                    }
-                }
+                xconv_block_mma<Cfg, BF>(d, st_base + (uint32_t)(b * 64), w_base);
+                xconv_block_epilogue<Cfg, BF>(d, a, s_bias, u, b, split, wq, lane);
             }
             bar_sync(3 + wg, 128);   // every warp of the warpgroup has finished its MMAs on this stage
             if ((threadIdx.x & 127) == 0) {
                 if (MC) { mbar_arrive_cluster(&empty[s], 0); mbar_arrive_cluster(&empty[s], 1); }
                 else mbar_arrive(&empty[s]);
             }
-            it++;
-        }
-    } else if (LO8) {
-        // ===== converters (NCONV warps, regions dealt round robin): byte residual planes -> fp16 in place (byte j of a slot pair becomes the
-        // fp16 with that high byte).  The bytes sit in the upper half of the plane's place; a warp reads a whole region (16 bytes per lane and
-        // step) into registers before it writes the expanded 32 bytes per lane and step, so nothing is overwritten before it is read =====
-        constexpr int NST = In::DATA / 64;                    // steps of 32 lanes x 16 bytes per region
-        const int cw = warp - 9;
-        int it = 0;
-        for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-            if (!uvalid(u)) continue;
-            const int s = it % STAGES;
-            mbar_wait(&full[s], (it / STAGES) & 1);
-#pragma unroll 1
-            for (int r = cw; r < KC * In::NPLANES; r += Cfg::NCONV) {
-                const int g = KC + r / In::NPLANES, pl = r % In::NPLANES;
-                unsigned char* region = sIn + ((size_t)g * GS + (size_t)s * In::SLOT_STAGE + (size_t)pl * In::PLANE + RW) * 16;
-                uint4 bb[NST];
-#pragma unroll
-                for (int k = 0; k < NST; k++) bb[k] = *reinterpret_cast<const uint4*>(region + In::DATA * 8 + (k * 32 + lane) * 16);
-                __syncwarp();
-#pragma unroll
-                for (int k = 0; k < NST; k++) {
-                    *reinterpret_cast<uint4*>(region + (k * 32 + lane) * 32) =
-                        make_uint4(__byte_perm(bb[k].x, 0u, 0x1404), __byte_perm(bb[k].x, 0u, 0x3424), __byte_perm(bb[k].y, 0u, 0x1404), __byte_perm(bb[k].y, 0u, 0x3424));
-                    *reinterpret_cast<uint4*>(region + (k * 32 + lane) * 32 + 16) =
-                        make_uint4(__byte_perm(bb[k].z, 0u, 0x1404), __byte_perm(bb[k].z, 0u, 0x3424), __byte_perm(bb[k].w, 0u, 0x1404), __byte_perm(bb[k].w, 0u, 0x3424));
-                }
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&cfull[s]);
             it++;
         }
     }

@@ -1,4 +1,5 @@
-// First two conv layers of AffNet / OriNet / HardNet in ONE kernel, second-generation formulation (see tcx_conv.cuh):
+// First two conv layers of AffNet / OriNet / HardNet in ONE kernel (AffNet / OriNet: three, L3 below), second-generation formulation
+// (see tcx_conv.cuh):
 //
 //   sampler (LAF.py:313-372) -> input_norm (architectures.py:231-235) -> conv3x3(1 -> C1)+BN+ReLU -> conv3x3(C1 -> COUT)+BN+ReLU
 //
@@ -9,19 +10,25 @@
 // taps of that row stacked along N (N = 3*COUT); the epilogue shifts the dx = 0 / dx = 2 blocks by one pixel with warp shuffles, and
 // through shared memory where an image row continues in the next warp (a warp holds 16 accumulator rows, half an image row).
 // Split precision: the input and layer-1 weights always carry fp16 residual planes; SA / SW / OSA as in tcx_conv.cuh.
+// L3 = 1 (AffNet / OriNet): layer 3 (stride 2, 32x32 -> 16x16) runs in the same kernel.  Layer 2's epilogue then writes its hi / lo
+// values into shared memory, in the parity planes a stride-2 tcx_conv_kernel would load (a zero row, then 256 data slots per plane),
+// instead of to HBM, and once both warpgroups are done each runs layer 3's blocks wg, wg + 2 with tcx_conv_kernel's own block functions
+// (xconv_block_mma / xconv_block_epilogue), writing L_S1_16 hi + lo planes to HBM.  The 64 KiB per patch of layer 2's output never
+// leave the SM.  To make room, the layer-1 stage is single-buffered (see the consumer loop).
 //
 // Warp roles (16 warps): 0-7 sampler + input_norm + P planes (two halves with their own barriers, so that the producers build one
 // half while the MMAs read the other) | 8-15 two consumer warpgroups: layer 1 of a patch (MMA, then bias/ReLU -> fp16 stage in shared
-// memory), then its layer 2 (MMA, then x shifts -> bias/ReLU -> fp16 -> global, stride-2 consumer layout); warpgroup g takes the
-// blocks g, g + 2, ... of each layer.
+// memory), then its layer 2 (MMA, then x shifts -> bias/ReLU -> fp16 -> global, stride-2 consumer layout; L3: -> shared memory, then
+// layer 3); warpgroup g takes the blocks g, g + 2, ... of each layer.
 #pragma once
 #include "tcx_conv.cuh"
 
 namespace ag {
 namespace tcx {
 
-template <int C1, int COUT, int SA, int SW, int OSA>
+template <int C1, int COUT, int SA, int SW, int OSA, int L3 = 0>
 struct XFirstCfg {
+    using X3 = XCfg<COUT, 2 * COUT, 32, 2, 1, 1, L_S1_16, 1, 1, 1>;   // layer 3 (L3 = 1): its input planes as ONE stage in shared memory
     static constexpr int KC = C1 / 8, NT = COUT;
     static constexpr int BLOCKS = 16;                          // M = 64 blocks of a patch
     static constexpr int NPIXP = 18 * 32;                      // slots of one HALF P plane: 18 window rows (16 image rows of outputs + 2 rows of look-ahead)
@@ -31,25 +38,32 @@ struct XFirstCfg {
     static constexpr int ACCW = 3 * NT;
     static constexpr int G = KC * (1 + SA);
     static constexpr int SLOT_STAGE = 1024 + 32;               // zero row + 32 data rows; the zero row below is the next stage's / the trailing one
-    static constexpr int GS = 2 * SLOT_STAGE + 32;
+    static constexpr int NSTAGE = L3 ? 1 : 2;                  // layer-1 stages (L3: single-buffered)
+    static constexpr int GS = NSTAGE * SLOT_STAGE + 32;
     static constexpr int NR = (1 + SW) * 3 * NT;               // weight rows per K group of a (dy, k step) block
     static constexpr uint32_t W_BYTES = 9u * C1 * NT * 2u * (1 + SW);
     static constexpr uint32_t IN_BYTES = (uint32_t)G * GS * 16u;
     static constexpr uint32_t W1_BYTES = 2u * 2u * C1 * 16;    // [K chunk 0|1][hi rows | lo rows][8]
     static constexpr uint32_t P_BYTES = 2u * 2u * NPIXP * 16;   // [half][hi | lo][NPIXP]: the halves are built and consumed alternately
     static constexpr uint32_t XCH_BYTES = 2u * 2u * 4u * 2u * NT * 4u;   // [warpgroup][block parity][warp][left | right][NT] row-boundary values
-    static constexpr size_t SMEM = 1024 + (size_t)W_BYTES + IN_BYTES + P_BYTES + W1_BYTES + 2 * SX * 4 + 256 + XCH_BYTES;
+    static constexpr uint32_t W3_BYTES = L3 ? X3::W_BYTES : 0u;     // layer-3 weights
+    static constexpr uint32_t IN3_BYTES = L3 ? X3::IN_BYTES : 0u;   // layer-3 input planes = layer 2's output
+    static constexpr size_t SMEM = 1024 + (size_t)W_BYTES + W3_BYTES + IN_BYTES + IN3_BYTES + P_BYTES + W1_BYTES + 2 * SX * 4 + 256 + XCH_BYTES;
     static constexpr size_t HI_OUT_BYTES = (size_t)(COUT / 8) * 1024 * 16;
-    static constexpr size_t UNIT_OUT_BYTES = HI_OUT_BYTES + (OSA == 1 ? HI_OUT_BYTES : OSA == 2 ? HI_OUT_BYTES / 2 : 0);   // OSA = 2: byte residual planes
+    static constexpr size_t UNIT_OUT_BYTES = HI_OUT_BYTES * (1 + OSA);
     static constexpr int THREADS = 512;
     static_assert(C1 % 16 == 0 && NT % 16 == 0 && ACCW <= 256, "shape");
+    static_assert(SA <= 1 && SW <= 1 && OSA <= 1, "split-precision switches are 0 | 1");
+    static_assert(!L3 || (OSA == 1 && X3::NT <= 32), "layer 3 reads hi + lo planes; its bias fits smem[640, 768)");
     static_assert(C1 == 16 || C1 == 32, "layer-1 accumulator width");
     static_assert(SMEM <= 232448, "shared memory budget");
 };
 
-template <int C1, int COUT, int SA, int SW, int OSA, int BF = 0>
-__global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const FirstSrc src) {
-    using Cfg = XFirstCfg<C1, COUT, SA, SW, OSA>;
+// a: layer 2 (L3 = 0: a.out receives its output), a3: layer 3 (L3 = 1 only; a3.in unused)
+template <int C1, int COUT, int SA, int SW, int OSA, int BF = 0, int L3 = 0>
+__global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const FirstSrc src, const XArgs a3) {
+    using Cfg = XFirstCfg<C1, COUT, SA, SW, OSA, L3>;
+    using X3 = typename Cfg::X3;
     constexpr int KC = Cfg::KC, NT = Cfg::NT, ACCW = Cfg::ACCW, NPIXP = Cfg::NPIXP, SX = Cfg::SX, GS = Cfg::GS;
     extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t* wbar = reinterpret_cast<uint64_t*>(smem);
@@ -57,9 +71,12 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
     uint64_t* p_empty = p_full + 2;                         // [2] layer-1 MMAs done with the half (2 warpgroups)
     float* s_bias1 = reinterpret_cast<float*>(smem + 384);  // [C1]
     float* s_bias = reinterpret_cast<float*>(smem + 512);   // [NT]
+    float* s_bias3 = reinterpret_cast<float*>(smem + 640);  // [X3::NT] (L3)
     unsigned char* sW = smem + 1024;
-    unsigned char* sIn = sW + Cfg::W_BYTES;                 // [G][2 stages][zero row | 32 data rows] + trailing zero row
-    unsigned char* sP = sIn + Cfg::IN_BYTES;                // [half][hi|lo][NPIXP][8] fp16
+    unsigned char* sW3 = sW + Cfg::W_BYTES;                 // layer-3 weights (L3)
+    unsigned char* sIn = sW3 + Cfg::W3_BYTES;               // [G][NSTAGE stages][zero row | 32 data rows] + trailing zero row
+    unsigned char* sIn3 = sIn + Cfg::IN_BYTES;              // (L3) [X3::G][4 parity planes][zero row | 256 data slots]
+    unsigned char* sP = sIn3 + Cfg::IN3_BYTES;              // [half][hi|lo][NPIXP][8] fp16
     unsigned char* sW1 = sP + Cfg::P_BYTES;                 // [chunk][hi|lo][C1][8] fp16
     float* s_x = reinterpret_cast<float*>(sW1 + Cfg::W1_BYTES);   // [2][SX]
     float* s_red = s_x + 2 * SX;                            // [2][8][2]
@@ -75,6 +92,7 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
     // ---- one-time setup by all threads ----
     if (threadIdx.x < NT) s_bias[threadIdx.x] = a.bias[threadIdx.x];
     if (threadIdx.x < C1) s_bias1[threadIdx.x] = src.b1[threadIdx.x];
+    if (L3 && threadIdx.x < X3::NT) s_bias3[threadIdx.x] = a3.bias[threadIdx.x];
     if (threadIdx.x == 0) {
         mbar_init(wbar, 1);
         for (int hh = 0; hh < 2; hh++) { mbar_init(&p_full[hh], 256); mbar_init(&p_empty[hh], 2); }
@@ -91,7 +109,8 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
         }
         reinterpret_cast<unsigned short*>(sW1)[i] = (unsigned short)(pack2<BF>(v, 0.f) & 0xFFFFu);
     }
-    for (int i = threadIdx.x; i < (int)((Cfg::IN_BYTES + Cfg::P_BYTES) / 16); i += blockDim.x) reinterpret_cast<uint4*>(sIn)[i] = make_uint4(0, 0, 0, 0);
+    // zero rows of the stages and of the layer-3 planes: written once, the epilogues only ever write data slots
+    for (int i = threadIdx.x; i < (int)((Cfg::IN_BYTES + Cfg::IN3_BYTES + Cfg::P_BYTES) / 16); i += blockDim.x) reinterpret_cast<uint4*>(sIn)[i] = make_uint4(0, 0, 0, 0);
     for (int i = threadIdx.x; i < 2 * SX; i += blockDim.x) s_x[i] = 0.f;
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
@@ -100,17 +119,21 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
         // ===== consumers =====
         const int wg = (warp - 8) >> 2, wq = warp & 3;
         if (threadIdx.x == 256) {
-            mbar_expect_tx(wbar, Cfg::W_BYTES);
+            mbar_expect_tx(wbar, Cfg::W_BYTES + Cfg::W3_BYTES);
             bulk_g2s(sW, a.wpk, Cfg::W_BYTES, wbar);
+            if (L3) bulk_g2s(sW3, a3.wpk, Cfg::W3_BYTES, wbar);
         }
         mbar_wait(wbar, 0);
         const uint32_t w_base = smem_u32(sW) >> 4, in_base = smem_u32(sIn) >> 4;
+        const uint32_t w3_base = smem_u32(sW3) >> 4, in3_base = smem_u32(sIn3) >> 4;
         const uint32_t w1_lo = desc_lo(smem_u32(sW1), 2 * C1 * 16u);       // K chunks are 2*C1 rows apart (hi rows, then lo rows)
         const uint32_t p_lo = desc_lo(smem_u32(sP), 2 * 32 * 16u);          // leading-byte offset = two image rows
         constexpr uint32_t LBO_A = ((uint32_t)GS) << 16;
         int it = 0, nblk = 0;
         for (int pi = next_valid(blockIdx.x); pi < a.n; pi = next_valid(pi + gridDim.x), it++) {
-            const int s = it & 1;
+            // L3: one stage.  Layer 1 of the next patch overwrites it only after the barrier between layers 2 and 3 below, which
+            // both warpgroups reach after their last layer-2 MMAs have completed (wgmma_wait): nobody still reads it.
+            const int s = L3 ? 0 : (it & 1);
             unsigned char* st = sIn + (size_t)s * Cfg::SLOT_STAGE * 16;
             // ---- layer 1, half plane by half plane -> fp16 (hi [+lo]) stage of layer 2 ----
 #pragma unroll 1
@@ -156,7 +179,7 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
             bar_sync(2, 256);   // the whole stage is written (both warpgroups)
             // ---- layer 2 ----
-            unsigned char* outp = reinterpret_cast<unsigned char*>(a.out) + (size_t)pi * Cfg::UNIT_OUT_BYTES;
+            unsigned char* outp = L3 ? nullptr : reinterpret_cast<unsigned char*>(a.out) + (size_t)pi * Cfg::UNIT_OUT_BYTES;
             const uint32_t st_base = in_base + (uint32_t)(s * Cfg::SLOT_STAGE);
 #pragma unroll 1
             for (int b = wg; b < Cfg::BLOCKS; b += 2, nblk++) {
@@ -224,14 +247,33 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
 #pragma unroll
                     for (int h = 0; h < 2; h++) {
                         const int slot = layout_slot(L_S2_16, y0, x0 + 8 * h, 0);
-                        const size_t goff = (size_t)(c / 8) * 1024 * 16;
                         uint32_t hi, lo;
                         split_pack2<OSA, BF>(v[h][0], v[h][1], hi, lo);
-                        *reinterpret_cast<uint32_t*>(outp + goff + (size_t)slot * 16 + (c & 7) * 2) = hi;
-                        if (OSA == 1) *reinterpret_cast<uint32_t*>(outp + (size_t)(COUT / 8) * 1024 * 16 + goff + (size_t)slot * 16 + (c & 7) * 2) = lo;
-                        if (OSA == 2) *reinterpret_cast<uint16_t*>(outp + Cfg::HI_OUT_BYTES + ((size_t)(c / 8) * 1024 + slot) * 8 + (c & 7)) = pack_lo8_2(lo);
+                        if (L3) {   // plane slot -> the same slot behind the plane's zero row in shared memory
+                            using In3 = typename X3::In;
+                            const size_t s3 = (size_t)(slot / In3::DATA) * In3::PLANE + In3::RW + slot % In3::DATA;
+                            *reinterpret_cast<uint32_t*>(sIn3 + ((size_t)(c / 8) * X3::GS + s3) * 16 + (c & 7) * 2) = hi;
+                            *reinterpret_cast<uint32_t*>(sIn3 + ((size_t)(X3::KC + c / 8) * X3::GS + s3) * 16 + (c & 7) * 2) = lo;
+                        } else {
+                            const size_t goff = (size_t)(c / 8) * 1024 * 16;
+                            *reinterpret_cast<uint32_t*>(outp + goff + (size_t)slot * 16 + (c & 7) * 2) = hi;
+                            if (OSA) *reinterpret_cast<uint32_t*>(outp + (size_t)(COUT / 8) * 1024 * 16 + goff + (size_t)slot * 16 + (c & 7) * 2) = lo;
+                        }
                     }
                 }
+            }
+            if (L3) {
+                // ---- layer 3: both warpgroups' layer-2 planes are written (and their layer-2 MMAs are done with the stage) ----
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                bar_sync(2, 256);
+#pragma unroll 1
+                for (int b = wg; b < X3::BLOCKS; b += 2) {
+                    float d3[X3::ACCW / 2];
+                    xconv_block_mma<X3, BF>(d3, in3_base + (uint32_t)(b * 64), w3_base);
+                    xconv_block_epilogue<X3, BF>(d3, a3, s_bias3, pi, b, 0, wq, lane);
+                }
+                // the planes are rewritten by the next patch's layer-2 epilogue only after that patch's "stage written" barrier, which
+                // the other warpgroup reaches after its layer-3 MMAs here have completed
             }
         }
     } else {
