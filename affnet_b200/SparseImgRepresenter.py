@@ -43,7 +43,7 @@ class ScaleSpaceAffinePatchExtractor(nn.Module):
             raise NotImplementedError("custom RespNet: only the fused Hessian response is implemented")
         if th is None and int(1.5 * num_features if num_Baum_iters > 0 else num_features) > 16384:
             raise L.AffnetB200Error("num_features=%d: the device-side selection sorts at most 16384 keypoints in shared memory "
-                                    "(num_features <= 10922 with a shape estimator, <= 16384 without)" % num_features)
+                                    "(num_features <= 10923 with a shape estimator, <= 16384 without)" % num_features)
         # SparseImgRepresenter.py:42-49: the hand-crafted estimators are the defaults
         self.OriNet = OriNet if OriNet is not None else OrientationDetector(patch_size=19)
         self.AffNet = AffNet if AffNet is not None else AffineShapeEstimator(patch_size=19)

@@ -134,4 +134,43 @@ __device__ __forceinline__ void laf_sample_xy(const float* __restrict__ L, int h
     py = __fsub_rn(__fmaf_rn(a21, xj, __fmaf_rn(a22, yi, ty)), 0.5f);
 }
 
+// Pyramid geometry passed by value to the kernels that sample pyr[oct][lvl] directly.
+struct PyrGeom {
+    int n_octaves, n_levels, B;
+    int h[AG_MAX_OCTAVES], w[AG_MAX_OCTAVES];
+    long long off[AG_MAX_OCTAVES][AG_MAX_LEVELS];
+};
+
+inline PyrGeom make_geom(const ag_pyramid_plan_t* p) {
+    PyrGeom g;
+    g.n_octaves = p->n_octaves; g.n_levels = p->n_levels; g.B = p->B;
+    for (int o = 0; o < AG_MAX_OCTAVES; o++) {
+        g.h[o] = p->h[o]; g.w[o] = p->w[o];
+        for (int l = 0; l < AG_MAX_LEVELS; l++) g.off[o][l] = p->level_offset[o][l];
+    }
+    return g;
+}
+
+// Hand-crafted estimators sampling the pyramid (handcrafted.cu), used by the batched pipeline.  `gk` is the module's Gaussian window
+// (PS x PS, host memory: copied into the launch parameters).  Rows at or beyond d_count[b] are neither read nor written.
+//   orientation_hist_pyr: d_R [B,cap,2,2] = [[cos, sin], [-sin, cos]] of the gradient-histogram angle at pyr[oct][lvl]
+//   baumberg_pyr:         d_A [B,cap,2,2] = base_A after `iters` Baumberg iterations (SparseImgRepresenter.py:127-141)
+int orientation_hist_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                         const int* d_count, int cap, int PS, const float* gk, float* d_R, void* stream);
+int baumberg_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                 const int* d_count, int cap, int PS, int iters, const float* gk, float* d_A, void* stream);
+
+// 2x2 products of the Baumberg chain in torch.bmm's fp32 operation order (row-by-column, two products added left to right); used by
+// mat2_compose_kernel / lafs_left_multiply_kernel (geometry.cu) and baumberg_pyr_kernel (handcrafted.cu).
+// out = A * B   (base_A <- A base_A, SparseImgRepresenter.py:133)
+__device__ __forceinline__ void mat2_mul(const float (&a)[4], const float (&b)[4], float (&o)[4]) {
+    o[0] = __fmaf_rn(a[1], b[2], __fmul_rn(a[0], b[0])); o[1] = __fmaf_rn(a[1], b[3], __fmul_rn(a[0], b[1]));
+    o[2] = __fmaf_rn(a[3], b[2], __fmul_rn(a[2], b[0])); o[3] = __fmaf_rn(a[3], b[3], __fmul_rn(a[2], b[1]));
+}
+// out = [A * L[:, :2] | L[:, 2]]   (the working LAF of the next Baumberg iteration, SparseImgRepresenter.py:134-135)
+__device__ __forceinline__ void laf_left_mul(const float (&a)[4], const float (&l)[6], float (&o)[6]) {
+    o[0] = __fmaf_rn(a[1], l[3], __fmul_rn(a[0], l[0])); o[1] = __fmaf_rn(a[1], l[4], __fmul_rn(a[0], l[1])); o[2] = l[2];
+    o[3] = __fmaf_rn(a[3], l[3], __fmul_rn(a[2], l[0])); o[4] = __fmaf_rn(a[3], l[4], __fmul_rn(a[2], l[1])); o[5] = l[5];
+}
+
 }  // namespace ag

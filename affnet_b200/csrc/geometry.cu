@@ -158,24 +158,28 @@ __global__ void lafs_to_ell_kernel(const float* __restrict__ lafs, float* __rest
 using namespace ag;
 
 namespace ag {
-// out = A * B for [n,2,2] batches, in torch.bmm's fp32 operation order (row-by-column, two products added left to right): the Baumberg
-// chain base_A <- A base_A of SparseImgRepresenter.py:133
+// out = A * B for [n,2,2] batches (mat2_mul, common.cuh): the Baumberg chain base_A <- A base_A of SparseImgRepresenter.py:133
 __global__ void mat2_compose_kernel(const float* __restrict__ A, const float* __restrict__ B, float* __restrict__ out, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float a0 = A[i * 4], a1 = A[i * 4 + 1], a2 = A[i * 4 + 2], a3 = A[i * 4 + 3];
-    const float b0 = B[i * 4], b1 = B[i * 4 + 1], b2 = B[i * 4 + 2], b3 = B[i * 4 + 3];
-    out[i * 4 + 0] = __fmaf_rn(a1, b2, __fmul_rn(a0, b0)); out[i * 4 + 1] = __fmaf_rn(a1, b3, __fmul_rn(a0, b1));
-    out[i * 4 + 2] = __fmaf_rn(a3, b2, __fmul_rn(a2, b0)); out[i * 4 + 3] = __fmaf_rn(a3, b3, __fmul_rn(a2, b1));
+    const float a[4] = {A[i * 4], A[i * 4 + 1], A[i * 4 + 2], A[i * 4 + 3]};
+    const float b[4] = {B[i * 4], B[i * 4 + 1], B[i * 4 + 2], B[i * 4 + 3]};
+    float o[4];
+    mat2_mul(a, b, o);
+#pragma unroll
+    for (int q = 0; q < 4; q++) out[i * 4 + q] = o[q];
 }
-// out = [A * L[:, :, :2] | L[:, :, 2]] : the working LAF of the next Baumberg iteration (SparseImgRepresenter.py:134-135)
+// out = [A * L[:, :, :2] | L[:, :, 2]] (laf_left_mul, common.cuh): the working LAF of the next Baumberg iteration (SparseImgRepresenter.py:134-135)
 __global__ void lafs_left_multiply_kernel(const float* __restrict__ A, const float* __restrict__ Lf, float* __restrict__ out, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float a0 = A[i * 4], a1 = A[i * 4 + 1], a2 = A[i * 4 + 2], a3 = A[i * 4 + 3];
-    const float l0 = Lf[i * 6], l1 = Lf[i * 6 + 1], l3 = Lf[i * 6 + 3], l4 = Lf[i * 6 + 4];
-    out[i * 6 + 0] = __fmaf_rn(a1, l3, __fmul_rn(a0, l0)); out[i * 6 + 1] = __fmaf_rn(a1, l4, __fmul_rn(a0, l1)); out[i * 6 + 2] = Lf[i * 6 + 2];
-    out[i * 6 + 3] = __fmaf_rn(a3, l3, __fmul_rn(a2, l0)); out[i * 6 + 4] = __fmaf_rn(a3, l4, __fmul_rn(a2, l1)); out[i * 6 + 5] = Lf[i * 6 + 5];
+    const float a[4] = {A[i * 4], A[i * 4 + 1], A[i * 4 + 2], A[i * 4 + 3]};
+    float l[6], o[6];
+#pragma unroll
+    for (int q = 0; q < 6; q++) l[q] = Lf[i * 6 + q];
+    laf_left_mul(a, l, o);
+#pragma unroll
+    for (int q = 0; q < 6; q++) out[i * 6 + q] = o[q];
 }
 }  // namespace ag
 

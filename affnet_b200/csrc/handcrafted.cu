@@ -1,6 +1,8 @@
 // Hand-crafted orientation and affine shape (SURVEY.md §8(f) rows 1 and 2): the estimators the reference uses when no OriNet /
 // AffNet is given.  Replaces OrientationDetector.forward (HandCraftedModules.py:168-192) and AffineShapeEstimator.forward
-// (HandCraftedModules.py:94-132).  One warp per patch; the patch (PS x PS, PS <= 41) is staged in shared memory.
+// (HandCraftedModules.py:94-132).  One warp per patch; the patch (PS x PS, PS <= 41) is staged in shared memory, either loaded from
+// materialised patches (ag_orientation_hist / ag_baumberg_shape) or sampled from the pyramid (orientation_hist_pyr / baumberg_pyr, the
+// batched pipeline).  Both kinds of kernel call the same per-warp estimator bodies.
 #include <math.h>
 
 #include "common.cuh"
@@ -21,19 +23,11 @@ __device__ __forceinline__ void grad_at(const float* p, int PS, int i, int j, fl
     gy = __fadd_rn(__fmul_rn(wm, p[im * PS + j]), __fmul_rn(wp, p[ip * PS + j]));
 }
 
-__global__ void __launch_bounds__(HC_WARPS * 32) orientation_hist_kernel(const float* __restrict__ patches, int n, int PS, const float* __restrict__ gk,
-                                                                        float* __restrict__ angle) {
-    __shared__ float s_p[HC_WARPS][HC_MAXPS * HC_MAXPS];
-    __shared__ float s_w[HC_WARPS][HC_MAXPS * HC_MAXPS];
-    __shared__ unsigned char s_b[HC_WARPS][HC_MAXPS * HC_MAXPS];
-    __shared__ float s_h[HC_WARPS][40];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int pi = blockIdx.x * HC_WARPS + warp;
-    if (pi >= n) return;
+// OrientationDetector.forward on the PS x PS patch `p` (shared memory) of one warp; s_w [PS*PS], s_b [PS*PS], s_h [40] are the warp's
+// scratch.  Returns the angle on every lane.
+__device__ __forceinline__ float orientation_hist_warp(const float* p, int PS, const float* gk, float* s_w, unsigned char* s_b, float* s_h,
+                                                       int lane) {
     const int NP = PS * PS;
-    float* p = s_p[warp];
-    for (int i = lane; i < NP; i += 32) p[i] = patches[(size_t)pi * NP + i];
-    __syncwarp();
     const float PI_F = 3.14159265358979323846f;
     for (int i = lane; i < NP; i += 32) {
         float gx, gy;
@@ -44,23 +38,23 @@ __global__ void __launch_bounds__(HC_WARPS * 32) orientation_hist_kernel(const f
         float bo0 = floorf(o_big);
         const float wo1 = __fsub_rn(o_big, bo0);
         bo0 = fmodf(bo0, 36.0f);
-        s_b[warp][i] = (unsigned char)(int)bo0;
-        s_w[warp][i] = __fmul_rn(__fsub_rn(1.0f, wo1), mag);   // only the lower-bin weight is accumulated (as the reference does)
+        s_b[i] = (unsigned char)(int)bo0;
+        s_w[i] = __fmul_rn(__fsub_rn(1.0f, wo1), mag);   // only the lower-bin weight is accumulated (as the reference does)
     }
     __syncwarp();
     // deterministic histogram: lane b sums bin b (and b+32) over all pixels in raster order
     for (int b = lane; b < 36; b += 32) {
         float acc = 0.f;
         for (int i = 0; i < NP; i++)
-            if (s_b[warp][i] == b) acc += s_w[warp][i];
-        s_h[warp][b + 1] = acc / (float)NP;   // adaptive_avg_pool2d -> mean
+            if (s_b[i] == b) acc += s_w[i];
+        s_h[b + 1] = acc / (float)NP;   // adaptive_avg_pool2d -> mean
     }
-    if (lane == 0) { s_h[warp][0] = 0.f; s_h[warp][37] = 0.f; }   // conv1d zero padding
+    if (lane == 0) { s_h[0] = 0.f; s_h[37] = 0.f; }   // conv1d zero padding
     __syncwarp();
     float best = -INFINITY;
     int bidx = 0;
     for (int b = lane; b < 36; b += 32) {
-        const float v = fmaf(0.33f, s_h[warp][b + 2], fmaf(0.34f, s_h[warp][b + 1], 0.33f * s_h[warp][b]));
+        const float v = fmaf(0.33f, s_h[b + 2], fmaf(0.34f, s_h[b + 1], 0.33f * s_h[b]));
         if (v > best) { best = v; bidx = b; }
     }
     // first maximum wins (torch.max on CPU)
@@ -69,19 +63,12 @@ __global__ void __launch_bounds__(HC_WARPS * 32) orientation_hist_kernel(const f
         const int oi = __shfl_xor_sync(0xffffffffu, bidx, o);
         if (ov > best || (ov == best && oi < bidx)) { best = ov; bidx = oi; }
     }
-    if (lane == 0) angle[pi] = -__fsub_rn(__fdiv_rn(__fmul_rn(2.0f * PI_F, (float)bidx), 36.0f), PI_F);
+    return -__fsub_rn(__fdiv_rn(__fmul_rn(2.0f * PI_F, (float)bidx), 36.0f), PI_F);
 }
 
-__global__ void __launch_bounds__(HC_WARPS * 32) baumberg_kernel(const float* __restrict__ patches, int n, int PS, const float* __restrict__ gk,
-                                                                float* __restrict__ A) {
-    __shared__ float s_p[HC_WARPS][HC_MAXPS * HC_MAXPS];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int pi = blockIdx.x * HC_WARPS + warp;
-    if (pi >= n) return;
+// AffineShapeEstimator.forward on the PS x PS patch `p` (shared memory) of one warp -> up-is-up rectified A, on every lane.
+__device__ __forceinline__ void baumberg_warp(const float* p, int PS, const float* gk, int lane, float (&A)[4]) {
     const int NP = PS * PS;
-    float* p = s_p[warp];
-    for (int i = lane; i < NP; i += 32) p[i] = patches[(size_t)pi * NP + i];
-    __syncwarp();
     float a = 0.f, b = 0.f, c = 0.f;
     for (int i = lane; i < NP; i += 32) {
         float gx, gy;
@@ -90,7 +77,6 @@ __global__ void __launch_bounds__(HC_WARPS * 32) baumberg_kernel(const float* __
         a += gx * gx * g; b += gx * gy * g; c += gy * gy * g;
     }
     a = warp_sum_f(a) / (float)NP; b = warp_sum_f(b) / (float)NP; c = warp_sum_f(c) / (float)NP;
-    if (lane != 0) return;
     // invSqrt (HandCraftedModules.py:94-117)
     const float eps = 1e-12f;
     const float mask = (b != 0.f) ? 1.f : 0.f;
@@ -110,9 +96,174 @@ __global__ void __launch_bounds__(HC_WARPS * 32) baumberg_kernel(const float* __
     const float a00 = na, a01 = nb, a10 = nb, a11 = nc;
     const float det = sqrtf(fabsf(a00 * a11 - a10 * a01 + 1e-10f));
     const float b2a2 = sqrtf(a01 * a01 + a00 * a00);
+    A[0] = b2a2 / det; A[1] = 0.f;
+    A[2] = (a11 * a01 + a10 * a00) / (b2a2 * det); A[3] = det / b2a2;
+}
+
+__global__ void __launch_bounds__(HC_WARPS * 32) orientation_hist_kernel(const float* __restrict__ patches, int n, int PS, const float* __restrict__ gk,
+                                                                        float* __restrict__ angle) {
+    __shared__ float s_p[HC_WARPS][HC_MAXPS * HC_MAXPS];
+    __shared__ float s_w[HC_WARPS][HC_MAXPS * HC_MAXPS];
+    __shared__ unsigned char s_b[HC_WARPS][HC_MAXPS * HC_MAXPS];
+    __shared__ float s_h[HC_WARPS][40];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int pi = blockIdx.x * HC_WARPS + warp;
+    if (pi >= n) return;
+    const int NP = PS * PS;
+    float* p = s_p[warp];
+    for (int i = lane; i < NP; i += 32) p[i] = patches[(size_t)pi * NP + i];
+    __syncwarp();
+    const float ang = orientation_hist_warp(p, PS, gk, s_w[warp], s_b[warp], s_h[warp], lane);
+    if (lane == 0) angle[pi] = ang;
+}
+
+__global__ void __launch_bounds__(HC_WARPS * 32) baumberg_kernel(const float* __restrict__ patches, int n, int PS, const float* __restrict__ gk,
+                                                                float* __restrict__ A) {
+    __shared__ float s_p[HC_WARPS][HC_MAXPS * HC_MAXPS];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int pi = blockIdx.x * HC_WARPS + warp;
+    if (pi >= n) return;
+    const int NP = PS * PS;
+    float* p = s_p[warp];
+    for (int i = lane; i < NP; i += 32) p[i] = patches[(size_t)pi * NP + i];
+    __syncwarp();
+    float a[4];
+    baumberg_warp(p, PS, gk, lane, a);
+    if (lane != 0) return;
     float* o = A + (size_t)pi * 4;
-    o[0] = b2a2 / det; o[1] = 0.f;
-    o[2] = (a11 * a01 + a10 * a00) / (b2a2 * det); o[3] = det / b2a2;
+    o[0] = a[0]; o[1] = a[1]; o[2] = a[2]; o[3] = a[3];
+}
+
+// ---- the estimators sampling the pyramid directly (batched pipeline) ----------------------------------------------------------------
+// One warp per keypoint (b, i), i < count[b]; the PS x PS patch is sampled from pyr[oct][lvl] into shared memory with the arithmetic of
+// extract_patches_pyr_kernel (laf_sample_xy + bilinear_zero), so the estimators see the bits ag_extract_patches_pyr would write to HBM.
+constexpr int HC_PYR_WARPS = 4;
+
+struct HcPyrParams {
+    PyrGeom G;
+    const float* pyr;
+    const float* lafs;   // [B,cap,2,3] normalised
+    const int* oct;
+    const int* lvl;
+    const int* count;    // [B]
+    int cap, PS, iters;
+    float* out;          // [B,cap,2,2]
+    float gk[HC_MAXPS * HC_MAXPS];
+};
+
+// floats of shared memory per warp: patch + weights + histogram (40) + bin bytes (orientation) or the patch alone (Baumberg)
+__host__ __device__ inline int hc_ori_warp_floats(int PS) { return 2 * PS * PS + 40 + (PS * PS + 3) / 4; }
+__host__ __device__ inline int hc_baum_warp_floats(int PS) { return PS * PS; }
+
+// the row of warp `warp` in this block, or -1 when it is at or beyond the image's count (a count of -1 = overflow: nothing to do)
+__device__ __forceinline__ long long hc_pyr_row(const HcPyrParams& P, int warp) {
+    const int b = blockIdx.y, i = blockIdx.x * HC_PYR_WARPS + warp;
+    if (i >= P.cap || i >= P.count[b]) return -1;
+    return (long long)b * P.cap + i;
+}
+
+__device__ __forceinline__ void sample_patch_warp(const HcPyrParams& P, long long row, const float* L, float* p, int lane) {
+    const int o = clampi(P.oct[row], 0, P.G.n_octaves - 1), l = clampi(P.lvl[row], 0, P.G.n_levels - 1);
+    const int h = P.G.h[o], w = P.G.w[o];
+    const float* img = P.pyr + P.G.off[o][l] + (size_t)blockIdx.y * h * w;
+    const int PS = P.PS, NP = PS * PS;
+    for (int t = lane; t < NP; t += 32) {
+        const int i = t / PS, j = t - i * PS;
+        float px, py;
+        laf_sample_xy(L, h, w, i, j, 1.0f / (float)PS, px, py);
+        p[t] = bilinear_zero(img, h, w, px, py);
+    }
+    __syncwarp();
+}
+
+__global__ void __launch_bounds__(HC_PYR_WARPS * 32) orientation_hist_pyr_kernel(const __grid_constant__ HcPyrParams P) {
+    extern __shared__ float hc_smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long row = hc_pyr_row(P, warp);
+    if (row < 0) return;
+    const int NP = P.PS * P.PS;
+    float* p = hc_smem + (size_t)warp * hc_ori_warp_floats(P.PS);
+    float* s_w = p + NP;
+    float* s_h = s_w + NP;
+    unsigned char* s_b = (unsigned char*)(s_h + 40);
+    sample_patch_warp(P, row, P.lafs + row * 6, p, lane);
+    const float ang = orientation_hist_warp(p, P.PS, P.gk, s_w, s_b, s_h, lane);
+    if (lane == 0) {   // angles2A (LAF.py:306-311)
+        const float c = cosf(ang), s = sinf(ang);
+        float* o = P.out + row * 4;
+        o[0] = c; o[1] = s; o[2] = -s; o[3] = c;
+    }
+}
+
+// getAffineShape's loop (SparseImgRepresenter.py:127-141) with AffineShapeEstimator, all iterations in one launch: sample at the working
+// LAF, Baumberg step A, base_A <- A base_A (the first iteration takes A as is), working LAF <- [base_A LAF_A | t] if another follows.
+__global__ void __launch_bounds__(HC_PYR_WARPS * 32) baumberg_pyr_kernel(const __grid_constant__ HcPyrParams P) {
+    extern __shared__ float hc_smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long row = hc_pyr_row(P, warp);
+    if (row < 0) return;
+    float* p = hc_smem + (size_t)warp * hc_baum_warp_floats(P.PS);
+    float L0[6], cur[6], base[4];
+#pragma unroll
+    for (int q = 0; q < 6; q++) L0[q] = cur[q] = P.lafs[row * 6 + q];
+    for (int it = 0; it < P.iters; it++) {
+        sample_patch_warp(P, row, cur, p, lane);
+        float A[4];
+        baumberg_warp(p, P.PS, P.gk, lane, A);
+        if (it == 0) {
+#pragma unroll
+            for (int q = 0; q < 4; q++) base[q] = A[q];
+        } else {
+            float nb[4];
+            mat2_mul(A, base, nb);
+#pragma unroll
+            for (int q = 0; q < 4; q++) base[q] = nb[q];
+        }
+        if (it != P.iters - 1) laf_left_mul(base, L0, cur);
+        __syncwarp();   // every lane is done with this patch before the next one overwrites it
+    }
+    if (lane == 0) {
+        float* o = P.out + row * 4;
+        o[0] = base[0]; o[1] = base[1]; o[2] = base[2]; o[3] = base[3];
+    }
+}
+
+static int launch_hc_pyr(bool ori, const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                         const int* d_count, int cap, int PS, int iters, const float* gk, float* d_out, cudaStream_t st) {
+    AG_REQUIRE(plan && d_pyr && d_lafs && d_oct && d_lvl && d_count && gk && d_out, "NULL argument");
+    AG_REQUIRE(PS >= 3 && PS <= HC_MAXPS, "patch size out of range (3..41)");
+    AG_REQUIRE(cap >= 1 && plan->B >= 1 && plan->B <= 65535 && iters >= 1, "bad sizes");
+    HcPyrParams P;
+    P.G = make_geom(plan);
+    P.pyr = d_pyr; P.lafs = d_lafs; P.oct = d_oct; P.lvl = d_lvl; P.count = d_count;
+    P.cap = cap; P.PS = PS; P.iters = iters; P.out = d_out;
+    memcpy(P.gk, gk, sizeof(float) * PS * PS);
+    const size_t smem = sizeof(float) * HC_PYR_WARPS * (size_t)(ori ? hc_ori_warp_floats(PS) : hc_baum_warp_floats(PS));   // <= 59 KiB at PS 41
+    static SmemAttrOnce attr_ori, attr_baum;
+    if (smem > 48 * 1024) {
+        const int rc = ori ? attr_ori.ensure(orientation_hist_pyr_kernel, smem, "orientation_hist_pyr smem attr")
+                           : attr_baum.ensure(baumberg_pyr_kernel, smem, "baumberg_pyr smem attr");
+        if (rc != AG_OK) return rc;
+    }
+    const dim3 grid(cdiv(cap, HC_PYR_WARPS), plan->B);
+    if (ori) {
+        orientation_hist_pyr_kernel<<<grid, HC_PYR_WARPS * 32, smem, st>>>(P);
+        AG_CHECK_LAUNCH("orientation_hist_pyr_kernel");
+    } else {
+        baumberg_pyr_kernel<<<grid, HC_PYR_WARPS * 32, smem, st>>>(P);
+        AG_CHECK_LAUNCH("baumberg_pyr_kernel");
+    }
+    return AG_OK;
+}
+
+int orientation_hist_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                         const int* d_count, int cap, int PS, const float* gk, float* d_R, void* stream) {
+    return launch_hc_pyr(true, plan, d_pyr, d_lafs, d_oct, d_lvl, d_count, cap, PS, 1, gk, d_R, (cudaStream_t)stream);
+}
+
+int baumberg_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                 const int* d_count, int cap, int PS, int iters, const float* gk, float* d_A, void* stream) {
+    return launch_hc_pyr(false, plan, d_pyr, d_lafs, d_oct, d_lvl, d_count, cap, PS, iters, gk, d_A, (cudaStream_t)stream);
 }
 
 }  // namespace ag

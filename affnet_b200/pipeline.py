@@ -1,20 +1,52 @@
 """Batched detect-and-describe for B same-sized images (new API; the reference handles one image at a time):
 the whole ScaleSpaceAffinePatchExtractor.forward + extract_patches_from_pyr + HardNet chain as one fixed kernel
-sequence with device-side counters, optionally replayed as a CUDA graph."""
+sequence with device-side counters, optionally replayed as a CUDA graph.  The estimators follow ScaleSpaceAffinePatchExtractor's
+constructor (SparseImgRepresenter.py:26-49): AffNet or Baumberg iterations or no shape step, OriNet or gradient-histogram orientation."""
 import ctypes as C
 
 import torch
 
 from . import _lib as L
+from .architectures import AffNetFast, OriNetFast
+from .HandCraftedModules import AffineShapeEstimator, OrientationDetector
+
+
+def estimators(AffNet, OriNet, do_ori, num_Baum_iters):
+    """ScaleSpaceAffinePatchExtractor's choice of estimators (SparseImgRepresenter.py:26-49, 189-209) as (ag_pipeline_estimators_t,
+    AffNetFast or None, OriNetFast or None): the native nets the chosen mode runs.  num_Baum_iters <= 0: no shape step; AffNetFast:
+    AffNet iterations; AffineShapeEstimator or None: Baumberg iterations at the module's patch size (19 for None).  With do_ori:
+    OriNetFast, or OrientationDetector / None (patch size 19) for the gradient histogram.  Estimators the mode does not use are ignored."""
+    est = L.PipelineEstimators(L.SHAPE_NONE, 0, 0, L.ORI_NONE, 0)
+    aff = ori = None
+    if num_Baum_iters > 0:
+        est.num_baum_iters = int(num_Baum_iters)
+        if isinstance(AffNet, AffNetFast):
+            est.shape, aff = L.SHAPE_AFFNET, AffNet
+        elif AffNet is None or isinstance(AffNet, AffineShapeEstimator):
+            est.shape, est.shape_ps = L.SHAPE_BAUMBERG, 19 if AffNet is None else int(AffNet.PS)
+        else:
+            raise L.AffnetB200Error("AffNet: expected AffNetFast, AffineShapeEstimator or None, got %s" % type(AffNet).__name__)
+    if do_ori:
+        if isinstance(OriNet, OriNetFast):
+            est.ori, ori = L.ORI_ORINET, OriNet
+        elif OriNet is None or isinstance(OriNet, OrientationDetector):
+            est.ori, est.ori_ps = L.ORI_HISTOGRAM, 19 if OriNet is None else int(OriNet.PS)
+        else:
+            raise L.AffnetB200Error("OriNet: expected OriNetFast, OrientationDetector or None, got %s" % type(OriNet).__name__)
+    return est, aff, ori
 
 
 class DetectDescribePipeline:
     def __init__(self, B, H, W, AffNet, HardNet, OriNet=None, num_features=2000, border=5, mrSize=5.192, nlevels=3,
-                 init_sigma=1.6, do_ori=True, cand_cap=0, device="cuda", outputs=None):
+                 init_sigma=1.6, do_ori=True, cand_cap=0, device="cuda", outputs=None, num_Baum_iters=1):
         """outputs: optional list of (lafs [B,K,2,3], desc [B,K,128], count [B] int32) CUDA tensors, one tuple per output slot, that the
-        kernels write into directly (e.g. DescriptorExchange.outputs(): the blocks an all-gather sends); default: one private slot."""
+        kernels write into directly (e.g. DescriptorExchange.outputs(): the blocks an all-gather sends); default: one private slot.
+        AffNet / OriNet / do_ori / num_Baum_iters select the estimators as ScaleSpaceAffinePatchExtractor does (see `estimators`):
+        e.g. AffNet=AffineShapeEstimator(19), num_Baum_iters=16 is the HesAff baseline, num_Baum_iters=0 the plain detector."""
         self.cfg = L.PipelineConfig(B, H, W, num_features, nlevels, border, float(init_sigma), float(mrSize), 1 if do_ori else 0, cand_cap)
+        self.est, aff, ori = estimators(AffNet, OriNet, do_ori, num_Baum_iters)
         self.nets = (AffNet, OriNet, HardNet)  # keep the modules alive; the C pipeline only BORROWS their ag_net_t handles
+        self._used = (aff, ori, HardNet)      # the native nets the chosen mode runs (None: not used, or a hand-crafted estimator)
         self._h = None
         self._net_handles = None
         self._bind_nets()
@@ -41,17 +73,16 @@ class DetectDescribePipeline:
         change (load_state_dict, .to(), in-place edits): the pipeline must never touch the freed handle, so every run()/replay() compares
         the handle objects it was built with against the modules' and rebinds (run) or refuses (replay: the captured graph holds the
         old weight pointers) when they differ."""
-        AffNet, OriNet, HardNet = self.nets
-        hs = (AffNet.handle(), OriNet.handle() if OriNet is not None else None, HardNet.handle())
+        hs = tuple(n.handle() if n is not None else None for n in self._used)
         if self._h is not None:
             L.lib().ag_pipeline_destroy(self._h)
             self._h = None
         h = C.c_void_p()
-        L.check(L.lib().ag_pipeline_create(C.byref(self.cfg), hs[0], hs[1], hs[2], C.byref(h)))
+        L.check(L.lib().ag_pipeline_create_ex(C.byref(self.cfg), C.byref(self.est), hs[0], hs[1], hs[2], C.byref(h)))
         self._h, self._net_handles, self._graph = h, hs, None
 
     def _nets_current(self):
-        return all(n is None or n._handle is h for n, h in zip(self.nets, self._net_handles))
+        return all(n is None or n._handle is h for n, h in zip(self._used, self._net_handles))
 
     def __del__(self):
         try:
@@ -67,7 +98,7 @@ class DetectDescribePipeline:
         """imgs CUDA float32 [B,1,H,W] or [B,H,W] -> (lafs [B,K,2,3] px, resp [B,K], desc [B,K,128], count [B]) of output slot `slot`.
         Rows >= count[b] are unspecified.  No host synchronisation."""
         imgs = L.f32c(imgs, "imgs")
-        if not self._nets_current() or any(n is not None and n.handle() is not h for n, h in zip(self.nets, self._net_handles)):
+        if not self._nets_current() or any(n is not None and n.handle() is not h for n, h in zip(self._used, self._net_handles)):
             self._bind_nets()      # a net was reloaded / moved since the pipeline was built
         if imgs.numel() != self.B * self.H * self.W:
             raise L.AffnetB200Error("expected %d x %d x %d pixels" % (self.B, self.H, self.W))

@@ -268,7 +268,8 @@ int ag_match_snn(const float* d_desc1, int n1, const float* d_desc2, int n2, int
 /* ------------------------------------------------------------------------------------------
  * Batched end-to-end pipeline (new; the reference processes one image at a time):
  * pyramid -> detect -> select(1.5K) -> sample -> AffNet -> filter(K) -> [sample -> OriNet -> rotate]
- * -> denormalise -> level select -> sample -> HardNet.       = ScaleSpaceAffinePatchExtractor.forward
+ * -> denormalise -> level select -> sample -> HardNet (ag_pipeline_create; ag_pipeline_create_ex selects the other
+ * estimators: Baumberg or no shape step, gradient-histogram orientation).    = ScaleSpaceAffinePatchExtractor.forward
  * + extract_patches_from_pyr + HardNet.forward (train_AffNet_test_on_graffity.py:255-260) for B images.
  * ------------------------------------------------------------------------------------------ */
 typedef struct ag_pipeline ag_pipeline_t;
@@ -285,9 +286,36 @@ typedef struct {
 } ag_pipeline_config_t;
 
 /* Nets are borrowed (must outlive the pipeline).  The pipeline owns no device memory: the caller passes one
- * workspace of ag_pipeline_workspace_bytes() bytes. */
+ * workspace of ag_pipeline_workspace_bytes() bytes.  = ag_pipeline_create_ex with {AG_SHAPE_AFFNET, 1, -, do_ori ? AG_ORI_ORINET : AG_ORI_NONE, -}. */
 int ag_pipeline_create(const ag_pipeline_config_t* cfg, const ag_net_t* affnet, const ag_net_t* orinet,
                        const ag_net_t* hardnet, ag_pipeline_t** out);
+
+/* Estimators of the pipeline (ScaleSpaceAffinePatchExtractor's AffNet / OriNet / num_Baum_iters, SparseImgRepresenter.py:26-49):
+ *   shape  AG_SHAPE_NONE      num_Baum_iters = 0: K keypoints straight from the detector, no prefilter and no shape filter;
+ *          AG_SHAPE_AFFNET    num_baum_iters AffNet iterations (affnet), then the shape filter;
+ *          AG_SHAPE_BAUMBERG  num_baum_iters iterations of AffineShapeEstimator(patch_size = shape_ps) (HandCraftedModules.py:81-132),
+ *                             all in one launch that samples the pyramid directly, then the shape filter;
+ *   ori    AG_ORI_NONE, AG_ORI_ORINET (orinet), AG_ORI_HISTOGRAM: OrientationDetector(patch_size = ori_ps) (HandCraftedModules.py:133-192)
+ *          sampling the pyramid directly.
+ * The hand-crafted estimators' patches never reach memory; their Gaussian windows are computed at create time. */
+#define AG_SHAPE_NONE 0
+#define AG_SHAPE_AFFNET 1
+#define AG_SHAPE_BAUMBERG 2
+#define AG_ORI_NONE 0
+#define AG_ORI_ORINET 1
+#define AG_ORI_HISTOGRAM 2
+typedef struct {
+    int shape;           /* AG_SHAPE_* */
+    int num_baum_iters;  /* >= 1 with a shape estimator; ignored with AG_SHAPE_NONE */
+    int shape_ps;        /* AG_SHAPE_BAUMBERG patch size, 3..41 (the reference's 19) */
+    int ori;             /* AG_ORI_*; must agree with cfg->do_ori */
+    int ori_ps;          /* AG_ORI_HISTOGRAM patch size, 3..41 (the reference's 19) */
+} ag_pipeline_estimators_t;
+/* Nets the mode does not use may be NULL and are ignored.  AG_ERR_INVALID: a missing net for the chosen mode, num_baum_iters < 1 with
+ * a shape estimator, a patch size outside 3..41, cfg->do_ori inconsistent with est->ori.  AG_ERR_CAPACITY: a prefilter of
+ * int(1.5 K) > 16384 keypoints with a shape estimator (K > 10923), K > 16384 without. */
+int ag_pipeline_create_ex(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_net_t* affnet,
+                          const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
 void ag_pipeline_destroy(ag_pipeline_t* p);
 size_t ag_pipeline_workspace_bytes(const ag_pipeline_t* p);
 const ag_pyramid_plan_t* ag_pipeline_plan(const ag_pipeline_t* p);
