@@ -265,6 +265,25 @@ size_t ag_match_snn_workspace_bytes(int n1, int n2);
 int ag_match_snn(const float* d_desc1, int n1, const float* d_desc2, int n2, int dim, float ratio, void* d_ws, size_t ws_bytes, int* d_idx2,
                  float* d_min, float* d_second, unsigned char* d_keep, void* stream);
 
+/* Batched SNN matcher (new; the reference matches one pair at a time): ag_match_snn's rule for every pair p = (i, j) of a list, between
+ * image i of set 1 (d_desc1 [S1,cap1,dim], d_count1 [S1]) and image j of set 2 (d_desc2 [S2,cap2,dim], d_count2 [S2]), on
+ * d_desc1[i, :count1[i]] and d_desc2[j, :count2[j]].  Set 2 may be set 1.  A NULL count array means every image has cap rows;
+ * d_pairs [P,2] int32, or NULL for pair p = (p, p) (then S1 == S2 == P).  Counts and pair indices are read on the device.
+ * Per pair: nearest neighbour (min, lowest column among the minima, NaN ignored, (+inf, 0) for a row with nothing below +inf), the
+ * columns that are the nearest neighbour of any row of the pair set to 100000, the second minimum (fminf), keep = min/(second+1e-8) <=
+ * ratio, and the kept rows compacted in ascending order: d_tent[p, t] = (row, idx2[row]) for t < d_ntent[p].
+ *   d_idx2, d_min, d_second, d_keep [P,cap1]; d_tent [P,cap1,2] and d_ntent [P] (both may be NULL: no compaction).
+ *   d_ntent[p] = -1 for a pair with an index out of range or a count outside 0..cap (the pipeline's -1 overflow count), 0 when either
+ *   image has no rows; nothing else of such a pair is written.  Rows at or beyond count1[i] and tentative rows at or beyond d_ntent[p]
+ *   are not written.  The distance matrix is never stored: d_ws holds the row norms and a column mask per pair.
+ * Enqueues 4 or 5 launches and a memset whatever P is; no allocation, no synchronisation (CUDA-graph capturable).
+ * AG_ERR_INVALID: NULL descriptors, workspace or outputs, dim / S / cap / P < 1, d_pairs == NULL with S1 != S2 or P != S1, cap1 above
+ * 4194240.  AG_ERR_CAPACITY: ws_bytes below ag_match_pairs_workspace_bytes().  Both are checked before any CUDA call. */
+size_t ag_match_pairs_workspace_bytes(int S1, int cap1, int S2, int cap2, int P);
+int ag_match_pairs(const float* d_desc1, const int* d_count1, int S1, int cap1, const float* d_desc2, const int* d_count2, int S2, int cap2,
+                   int dim, const int* d_pairs, int P, float ratio, void* d_ws, size_t ws_bytes, int* d_idx2, float* d_min, float* d_second,
+                   unsigned char* d_keep, int* d_tent, int* d_ntent, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Batched end-to-end pipeline (new; the reference processes one image at a time):
  * pyramid -> detect -> select(1.5K) -> sample -> AffNet -> filter(K) -> [sample -> OriNet -> rotate]
