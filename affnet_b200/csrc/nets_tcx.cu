@@ -260,4 +260,27 @@ int ag_debug_tcx_layer(const ag_net_t* net, const float* d_patches, int n, int u
     return AG_OK;
 }
 
+#ifdef AG_FIRST_TIMELINE
+// Developer builds with -DAG_FIRST_TIMELINE only (scripts/first_kernel_timeline.py): copy the per-warp state cycle sums of
+// tcx_first_kernel, uint64 [TL_LAUNCHES][TL_CTAS][16 warps][TL_STATES] in launch order since the last reset, to `host`; reset != 0
+// then clears them.  dims (may be NULL) receives TL_LAUNCHES, TL_CTAS, TL_STATES.
+int ag_first_timeline_read(unsigned long long* host, int* dims, int reset) {
+    constexpr size_t n = (size_t)tcx::TL_LAUNCHES * tcx::TL_CTAS * 16 * tcx::TL_STATES;
+    if (dims) { dims[0] = tcx::TL_LAUNCHES; dims[1] = tcx::TL_CTAS; dims[2] = tcx::TL_STATES; }
+    cudaDeviceSynchronize();
+    if (host) {
+        const int rc = check_cuda(cudaMemcpyFromSymbol(host, tcx::g_first_tl, n * 8), "timeline read");
+        if (rc != AG_OK) return rc;
+    }
+    if (reset) {
+        static unsigned long long zeros[n];
+        static int zl[tcx::TL_CTAS];
+        int rc = check_cuda(cudaMemcpyToSymbol(tcx::g_first_tl, zeros, sizeof(zeros)), "timeline reset");
+        if (rc == AG_OK) rc = check_cuda(cudaMemcpyToSymbol(tcx::g_first_tl_launch, zl, sizeof(zl)), "timeline reset");
+        return rc;
+    }
+    return AG_OK;
+}
+#endif
+
 }  // extern "C"

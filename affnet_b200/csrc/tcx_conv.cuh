@@ -183,10 +183,11 @@ __device__ __forceinline__ void frag_right(float v0, float v1, int lane, float& 
 __device__ __forceinline__ bool xpatch_valid(const XArgs& a, int pi) { return pi < a.n && (a.count == nullptr || (pi % a.group) < a.count[pi / a.group]); }
 
 // The MMAs of one M = 64 block of a layer (Cfg: XCfg) into d[ACCW / 2]: a_t = the block's first slot in shared memory, w_base = the
-// layer's packed weights (both in 16-byte units).  The input's channel groups are Cfg::GS slots apart.  Used by tcx_conv_kernel and by
-// the layer-3 stage of tcx_first_kernel.
+// layer's packed weights (both in 16-byte units).  The input's channel groups are Cfg::GS slots apart.  xconv_block_issue issues and
+// commits them as one wgmma group and returns at once (the caller waits before it reads d); xconv_block_mma also waits for them.
+// tcx_conv_kernel runs xconv_block_mma, the layer-3 stage of tcx_first_kernel xconv_block_issue.
 template <class Cfg, int BF>
-__device__ __forceinline__ void xconv_block_mma(float* d, uint32_t a_t, uint32_t w_base) {
+__device__ __forceinline__ void xconv_block_issue(float* d, uint32_t a_t, uint32_t w_base) {
     using In = typename Cfg::In;
     constexpr int KC = Cfg::KC, NT = Cfg::NT, GS = Cfg::GS, RW = In::RW, SA = Cfg::SPLIT_A, SW = Cfg::SPLIT_W;
     constexpr uint32_t LBO_A = ((uint32_t)GS) << 16;      // (bytes >> 4) << 16
@@ -232,6 +233,10 @@ __device__ __forceinline__ void xconv_block_mma(float* d, uint32_t a_t, uint32_t
         }
     }
     wgmma_commit();
+}
+template <class Cfg, int BF>
+__device__ __forceinline__ void xconv_block_mma(float* d, uint32_t a_t, uint32_t w_base) {
+    xconv_block_issue<Cfg, BF>(d, a_t, w_base);
     wgmma_wait<0>();
     wgmma_reg_fence<Cfg::ACCW / 2>(d);
 }

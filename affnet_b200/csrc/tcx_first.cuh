@@ -13,18 +13,39 @@
 // L3 = 1 (AffNet / OriNet): layer 3 (stride 2, 32x32 -> 16x16) runs in the same kernel.  Layer 2's epilogue then writes its hi / lo
 // values into shared memory, in the parity planes a stride-2 tcx_conv_kernel would load (a zero row, then 256 data slots per plane),
 // instead of to HBM, and once both warpgroups are done each runs layer 3's blocks wg, wg + 2 with tcx_conv_kernel's own block functions
-// (xconv_block_mma / xconv_block_epilogue), writing L_S1_16 hi + lo planes to HBM.  The 64 KiB per patch of layer 2's output never
+// (xconv_block_issue / xconv_block_epilogue), writing L_S1_16 hi + lo planes to HBM.  The 64 KiB per patch of layer 2's output never
 // leave the SM.  To make room, the layer-1 stage is single-buffered (see the consumer loop).
 //
 // Warp roles (16 warps): 0-7 sampler + input_norm + P planes (two halves with their own barriers, so that the producers build one
 // half while the MMAs read the other) | 8-15 two consumer warpgroups: layer 1 of a patch (MMA, then bias/ReLU -> fp16 stage in shared
 // memory), then its layer 2 (MMA, then x shifts -> bias/ReLU -> fp16 -> global, stride-2 consumer layout; L3: -> shared memory, then
 // layer 3); warpgroup g takes the blocks g, g + 2, ... of each layer.
+// Within a layer each consumer warpgroup keeps two blocks in flight: it issues and commits the MMAs of its next block, waits until only
+// that group is pending (wgmma_wait<1>) and runs the epilogue of the previous one, so the tensor core works through one block while
+// the warpgroup's epilogue of the other runs.  The second accumulator set is what the producers' registers pay for (setmaxnreg:
+// producers 96, consumers 160 per thread).
 #pragma once
 #include "tcx_conv.cuh"
 
+// AG_FIRST_TIMELINE (developer builds, scripts/first_kernel_timeline.py): every warp of CTAs 0 .. TL_CTAS - 1 adds up the SM cycles
+// (clock64) it spends in each TL_* state and stores the sums per launch in g_first_tl; ag_first_timeline_read copies them out.
+#ifdef AG_FIRST_TIMELINE
+#define AG_TL(state, ...) do { const long long t_ = clock64(); __VA_ARGS__; tl[state] += (unsigned long long)(clock64() - t_); } while (0)
+#else
+#define AG_TL(state, ...) do { __VA_ARGS__; } while (0)
+#endif
+
 namespace ag {
 namespace tcx {
+
+// timeline states: consumers  TOTAL | wait p_full | issue MMAs | wgmma_wait | warpgroup barrier | barrier of both warpgroups
+//                  producers  TOTAL | wait p_empty | -          | -          | barrier 1 (input_norm) | - | build the P planes
+enum { TL_TOTAL, TL_WAIT_P, TL_ISSUE, TL_MMA_WAIT, TL_WG_BAR, TL_STAGE_BAR, TL_PBUILD, TL_STATES };
+#ifdef AG_FIRST_TIMELINE
+constexpr int TL_CTAS = 4, TL_LAUNCHES = 8;
+__device__ unsigned long long g_first_tl[TL_LAUNCHES][TL_CTAS][16][TL_STATES];
+__device__ int g_first_tl_launch[TL_CTAS];
+#endif
 
 template <int C1, int COUT, int SA, int SW, int OSA, int L3 = 0>
 struct XFirstCfg {
@@ -52,6 +73,9 @@ struct XFirstCfg {
     static constexpr size_t HI_OUT_BYTES = (size_t)(COUT / 8) * 1024 * 16;
     static constexpr size_t UNIT_OUT_BYTES = HI_OUT_BYTES * (1 + OSA);
     static constexpr int THREADS = 512;
+    static constexpr int REG_PRODUCER = 96, REG_CONSUMER = 160;   // setmaxnreg: 256 threads of each role share the 64 Ki registers
+    static_assert(256 * (REG_PRODUCER + REG_CONSUMER) <= 65536 && REG_PRODUCER % 8 == 0 && REG_CONSUMER % 8 == 0, "register split");
+    static_assert(BLOCKS % 4 == 0 && (!L3 || X3::BLOCKS == 4), "two blocks in flight per warpgroup: an even count of blocks each");
     static_assert(C1 % 16 == 0 && NT % 16 == 0 && ACCW <= 256, "shape");
     static_assert(SA <= 1 && SW <= 1 && OSA <= 1, "split-precision switches are 0 | 1");
     static_assert(!L3 || (OSA == 1 && X3::NT <= 32), "layer 3 reads hi + lo planes; its bias fits smem[640, 768)");
@@ -98,6 +122,11 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
         for (int hh = 0; hh < 2; hh++) { mbar_init(&p_full[hh], 256); mbar_init(&p_empty[hh], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+#ifdef AG_FIRST_TIMELINE
+    int* s_tl_slot = reinterpret_cast<int*>(smem + 128);    // this launch's slot in g_first_tl (TL_LAUNCHES: not recorded)
+    if (threadIdx.x == 0) *s_tl_slot = blockIdx.x < TL_CTAS ? min(atomicAdd(&g_first_tl_launch[blockIdx.x], 1), TL_LAUNCHES) : TL_LAUNCHES;
+    unsigned long long tl[TL_STATES] = {};
+#endif
     for (int i = threadIdx.x; i < 2 * 2 * C1 * 8; i += blockDim.x) {   // W1[chunk][hi rows | lo rows][e]: chunk 0 = kernel rows 0 (e 0..2), 1 (e 4..6); chunk 1 = kernel row 2
         const int e = i & 7, co = (i >> 3) % C1, part = (i / (8 * C1)) & 1, ch = i / (8 * C1 * 2);
         const int dy = ch == 0 ? (e >> 2) : 2, dx = e & 3;
@@ -114,9 +143,13 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
     for (int i = threadIdx.x; i < 2 * SX; i += blockDim.x) s_x[i] = 0.f;
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
+#ifdef AG_FIRST_TIMELINE
+    const long long tl_start = clock64();
+#endif
 
     if (warp >= 8) {
         // ===== consumers =====
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(Cfg::REG_CONSUMER));
         const int wg = (warp - 8) >> 2, wq = warp & 3;
         if (threadIdx.x == 256) {
             mbar_expect_tx(wbar, Cfg::W_BYTES + Cfg::W3_BYTES);
@@ -129,61 +162,75 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
         const uint32_t w1_lo = desc_lo(smem_u32(sW1), 2 * C1 * 16u);       // K chunks are 2*C1 rows apart (hi rows, then lo rows)
         const uint32_t p_lo = desc_lo(smem_u32(sP), 2 * 32 * 16u);          // leading-byte offset = two image rows
         constexpr uint32_t LBO_A = ((uint32_t)GS) << 16;
+        // layer 1 of block b (of half plane hh): issue and commit its MMAs into d1
+        auto l1_issue = [&](float* d1, int hh, int b) {
+            const uint32_t alo = p_lo + (uint32_t)(hh * 2 * NPIXP + (b & 7) * 64);
+            wgmma_fence();
+            if (Cfg::S1) {   // x_hi * [w_hi ; w_lo] in one MMA, then x_lo * w_hi
+                Wgmma<2 * C1, BF>::mma(d1, desc64(alo), desc64(w1_lo), 0);
+                Wgmma<C1, BF>::mma(d1, desc64(alo + (uint32_t)NPIXP), desc64(w1_lo), 1);
+            } else {
+                Wgmma<C1, BF>::mma(d1, desc64(alo), desc64(w1_lo), 0);
+                Wgmma<C1, BF>::mma(d1, desc64(alo + (uint32_t)NPIXP), desc64(w1_lo), 1);             // x_lo * w_hi
+                Wgmma<C1, BF>::mma(d1, desc64(alo), desc64(w1_lo + (uint32_t)C1), 1);                 // x_hi * w_lo (lo rows follow the hi rows)
+            }
+            wgmma_commit();
+        };
+        // its epilogue, once the MMAs have completed: bias / ReLU -> fp16 (hi [+lo]) into stage st of layer 2
+        auto l1_epilogue = [&](float* d1, unsigned char* st, int b) {
+            wgmma_reg_fence<Cfg::ACC1 / 2>(d1);
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int slot = b * 64 + wq * 16 + (lane >> 2) + 8 * h + 32;      // pixel m sits one (zero) row into the stage
+#pragma unroll
+                for (int j = 0; j < C1 / 8; j++) {
+                    const int c = j * 8 + 2 * (lane & 3);
+                    float v0 = d1[4 * j + 2 * h], v1 = d1[4 * j + 2 * h + 1];
+                    if (Cfg::S1) { v0 += d1[4 * (j + 2) + 2 * h]; v1 += d1[4 * (j + 2) + 2 * h + 1]; }   // [x*w_hi | x_hi*w_lo] side by side
+                    v0 = fmaxf(fmaf(v0, src.w1_inv, s_bias1[c]), 0.f);
+                    v1 = fmaxf(fmaf(v1, src.w1_inv, s_bias1[c + 1]), 0.f);
+                    uint32_t hi, lo;
+                    split_pack2<SA, BF>(v0, v1, hi, lo);
+                    *reinterpret_cast<uint32_t*>(st + ((size_t)j * GS + slot) * 16 + (c & 7) * 2) = hi;
+                    if (SA) *reinterpret_cast<uint32_t*>(st + ((size_t)(KC + j) * GS + slot) * 16 + (c & 7) * 2) = lo;
+                }
+            }
+        };
+        // block k = 0 .. 7 of this warpgroup's layer-1 blocks: half plane k / 4, block 8 (k / 4) + wg + 2 (k % 4)
+        auto l1_block = [&](int k) -> int { return (k >> 2) * 8 + wg + 2 * (k & 3); };
         int it = 0, nblk = 0;
         for (int pi = next_valid(blockIdx.x); pi < a.n; pi = next_valid(pi + gridDim.x), it++) {
             // L3: one stage.  Layer 1 of the next patch overwrites it only after the barrier between layers 2 and 3 below, which
-            // both warpgroups reach after their last layer-2 MMAs have completed (wgmma_wait): nobody still reads it.
+            // both warpgroups reach after their last layer-2 MMAs have completed (the layer-2 loop ends in wgmma_wait<0>): nobody
+            // still reads it.
             const int s = L3 ? 0 : (it & 1);
             unsigned char* st = sIn + (size_t)s * Cfg::SLOT_STAGE * 16;
-            // ---- layer 1, half plane by half plane -> fp16 (hi [+lo]) stage of layer 2 ----
-#pragma unroll 1
-            for (int hh = 0; hh < 2; hh++) {
-                mbar_wait(&p_full[hh], it & 1);
-#pragma unroll 1
-                for (int k = 0; k < 4; k++) {
-                    const int b = hh * 8 + wg + 2 * k;
-                    float d1[Cfg::ACC1 / 2];
-                    const uint32_t alo = p_lo + (uint32_t)(hh * 2 * NPIXP + (b & 7) * 64);
-                    wgmma_fence();
-                    if (Cfg::S1) {   // x_hi * [w_hi ; w_lo] in one MMA, then x_lo * w_hi
-                        Wgmma<2 * C1, BF>::mma(d1, desc64(alo), desc64(w1_lo), 0);
-                        Wgmma<C1, BF>::mma(d1, desc64(alo + (uint32_t)NPIXP), desc64(w1_lo), 1);
-                    } else {
-                        Wgmma<C1, BF>::mma(d1, desc64(alo), desc64(w1_lo), 0);
-                        Wgmma<C1, BF>::mma(d1, desc64(alo + (uint32_t)NPIXP), desc64(w1_lo), 1);             // x_lo * w_hi
-                        Wgmma<C1, BF>::mma(d1, desc64(alo), desc64(w1_lo + (uint32_t)C1), 1);                 // x_hi * w_lo (lo rows follow the hi rows)
-                    }
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    wgmma_reg_fence<Cfg::ACC1 / 2>(d1);
+            // ---- layer 1, half plane by half plane -> fp16 (hi [+lo]) stage of layer 2; block k + 1's MMAs run during block k's
+            // epilogue (the second half plane is waited for before its first block is issued) ----
+            float d1[2][Cfg::ACC1 / 2];
+            AG_TL(TL_WAIT_P, mbar_wait(&p_full[0], it & 1));
+            AG_TL(TL_ISSUE, l1_issue(d1[0], 0, l1_block(0)));
 #pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        const int slot = b * 64 + wq * 16 + (lane >> 2) + 8 * h + 32;      // pixel m sits one (zero) row into the stage
-#pragma unroll
-                        for (int j = 0; j < C1 / 8; j++) {
-                            const int c = j * 8 + 2 * (lane & 3);
-                            float v0 = d1[4 * j + 2 * h], v1 = d1[4 * j + 2 * h + 1];
-                            if (Cfg::S1) { v0 += d1[4 * (j + 2) + 2 * h]; v1 += d1[4 * (j + 2) + 2 * h + 1]; }   // [x*w_hi | x_hi*w_lo] side by side
-                            v0 = fmaxf(fmaf(v0, src.w1_inv, s_bias1[c]), 0.f);
-                            v1 = fmaxf(fmaf(v1, src.w1_inv, s_bias1[c + 1]), 0.f);
-                            uint32_t hi, lo;
-                            split_pack2<SA, BF>(v0, v1, hi, lo);
-                            *reinterpret_cast<uint32_t*>(st + ((size_t)j * GS + slot) * 16 + (c & 7) * 2) = hi;
-                            if (SA) *reinterpret_cast<uint32_t*>(st + ((size_t)(KC + j) * GS + slot) * 16 + (c & 7) * 2) = lo;
-                        }
-                    }
+            for (int k = 0; k < 8; k++) {
+                if (k < 7) {
+                    if (k == 3) AG_TL(TL_WAIT_P, mbar_wait(&p_full[1], it & 1));
+                    AG_TL(TL_ISSUE, l1_issue(d1[(k + 1) & 1], (k + 1) >> 2, l1_block(k + 1)));
+                    AG_TL(TL_MMA_WAIT, wgmma_wait<1>());
+                } else {
+                    AG_TL(TL_MMA_WAIT, wgmma_wait<0>());
                 }
-                bar_sync(3 + wg, 128);
-                if ((threadIdx.x & 127) == 0) mbar_arrive(&p_empty[hh]);
+                l1_epilogue(d1[k & 1], st, l1_block(k));
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> visible to the tensor core
-            bar_sync(2, 256);   // the whole stage is written (both warpgroups)
-            // ---- layer 2 ----
+            AG_TL(TL_STAGE_BAR, bar_sync(2, 256));   // the whole stage is written (both warpgroups)
+            // p_empty means "the layer-1 MMAs of both warpgroups have completed on the half", not merely been issued: every consumer
+            // thread passed its wgmma_wait<0> above before the barrier.  Both halves are released here, the producers build the
+            // next patch's planes during this patch's layer 2.
+            if ((threadIdx.x & 127) == 0) { mbar_arrive(&p_empty[0]); mbar_arrive(&p_empty[1]); }
+            // ---- layer 2: block k + 1's MMAs run during block k's epilogue ----
             unsigned char* outp = L3 ? nullptr : reinterpret_cast<unsigned char*>(a.out) + (size_t)pi * Cfg::UNIT_OUT_BYTES;
             const uint32_t st_base = in_base + (uint32_t)(s * Cfg::SLOT_STAGE);
-#pragma unroll 1
-            for (int b = wg; b < Cfg::BLOCKS; b += 2, nblk++) {
-                float d[ACCW / 2];
+            auto l2_issue = [&](float* d, int b) {
                 const uint32_t a_t = st_base + (uint32_t)(b * 64);
                 wgmma_fence();
 #pragma unroll
@@ -200,11 +247,16 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
                     }
                 }
                 wgmma_commit();
-                wgmma_wait<0>();
+            };
+            // epilogue of block b, the warpgroup's nb-th layer-2 block, once its MMAs have completed
+            auto l2_epilogue = [&](float* d, int b, int nb) {
                 wgmma_reg_fence<ACCW / 2>(d);
                 // rows r = 16 wq + lane/4 + 8 h of the block: pixel m = 64 b + r, y = m / 32, x = m % 32.  Warps 2k and 2k+1 share an image
                 // row: the last row of an even warp and the first of the odd one exchange their dx = 0 / dx = 2 values through shared memory.
-                float* xw = s_xch + (size_t)((wg * 2 + (nblk & 1)) * 4) * 2 * NT;
+                // The exchange is double-buffered by block parity and a warpgroup runs its epilogues one at a time in block order (the
+                // second block in flight is in MMAs, not in an epilogue): a warp rewrites a buffer only after every warp of the warpgroup
+                // has passed the barrier of the following block, so after it read the buffer.
+                float* xw = s_xch + (size_t)((wg * 2 + (nb & 1)) * 4) * 2 * NT;
                 if (lane >= 28) {
 #pragma unroll
                     for (int j = 0; j < NT / 8; j++) {
@@ -219,7 +271,7 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
                         xw[(wq * 2 + 1) * NT + c] = d[4 * (j + 2 * NT / 8)]; xw[(wq * 2 + 1) * NT + c + 1] = d[4 * (j + 2 * NT / 8) + 1];   // row 0, dx = 2
                     }
                 }
-                bar_sync(3 + wg, 128);
+                AG_TL(TL_WG_BAR, bar_sync(3 + wg, 128));
                 const int y0 = (b * 64 + wq * 16) >> 5;
                 const int x0 = (wq & 1) * 16 + (lane >> 2);             // h = 0; h = 1 is x0 + 8
                 const float ml0 = x0 > 0 ? 1.f : 0.f, mr1 = x0 + 8 < 31 ? 1.f : 0.f;
@@ -261,23 +313,45 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
                         }
                     }
                 }
+            };
+            // this warpgroup's blocks wg + 2 k, k = 0 .. 7: d[k & 1].  Unrolled: with MMAs in flight across a loop's back edge ptxas
+            // serialises the wgmma pipeline.
+            float d[2][ACCW / 2];
+            AG_TL(TL_ISSUE, l2_issue(d[0], wg));
+#pragma unroll
+            for (int k = 0; k < Cfg::BLOCKS / 2; k++) {
+                if (k + 1 < Cfg::BLOCKS / 2) {
+                    AG_TL(TL_ISSUE, l2_issue(d[(k + 1) & 1], wg + 2 * (k + 1)));
+                    AG_TL(TL_MMA_WAIT, wgmma_wait<1>());
+                } else {
+                    // the last layer-2 MMAs on the stage have completed: the barrier below (L3) or the next patch's "stage written"
+                    // barrier releases the stage to the next layer-1 epilogue that writes it
+                    AG_TL(TL_MMA_WAIT, wgmma_wait<0>());
+                }
+                l2_epilogue(d[k & 1], wg + 2 * k, nblk + k);
             }
+            nblk += Cfg::BLOCKS / 2;
             if (L3) {
                 // ---- layer 3: both warpgroups' layer-2 planes are written (and their layer-2 MMAs are done with the stage) ----
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                bar_sync(2, 256);
-#pragma unroll 1
-                for (int b = wg; b < X3::BLOCKS; b += 2) {
-                    float d3[X3::ACCW / 2];
-                    xconv_block_mma<X3, BF>(d3, in3_base + (uint32_t)(b * 64), w3_base);
-                    xconv_block_epilogue<X3, BF>(d3, a3, s_bias3, pi, b, 0, wq, lane);
-                }
-                // the planes are rewritten by the next patch's layer-2 epilogue only after that patch's "stage written" barrier, which
-                // the other warpgroup reaches after its layer-3 MMAs here have completed
+                AG_TL(TL_STAGE_BAR, bar_sync(2, 256));
+                // both of the warpgroup's blocks (wg, wg + 2) in flight, the second one's MMAs run during the first one's epilogue
+                float d3[2][X3::ACCW / 2];
+                AG_TL(TL_ISSUE, xconv_block_issue<X3, BF>(d3[0], in3_base + (uint32_t)(wg * 64), w3_base));
+                AG_TL(TL_ISSUE, xconv_block_issue<X3, BF>(d3[1], in3_base + (uint32_t)((wg + 2) * 64), w3_base));
+                AG_TL(TL_MMA_WAIT, wgmma_wait<1>());
+                wgmma_reg_fence<X3::ACCW / 2>(d3[0]);
+                xconv_block_epilogue<X3, BF>(d3[0], a3, s_bias3, pi, wg, 0, wq, lane);
+                AG_TL(TL_MMA_WAIT, wgmma_wait<0>());
+                wgmma_reg_fence<X3::ACCW / 2>(d3[1]);
+                xconv_block_epilogue<X3, BF>(d3[1], a3, s_bias3, pi, wg + 2, 0, wq, lane);
+                // sIn3 is rewritten by the next patch's layer-2 epilogue only after that patch's "stage written" barrier, which the
+                // other warpgroup reaches after its layer-3 MMAs here have completed (wgmma_wait<0> above)
             }
         }
     } else {
         // ===== producers (8 warps): sampler (or patch load) -> input_norm -> sliding-window planes P_hi / P_lo =====
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::REG_PRODUCER));
         const int pw = warp;                                 // 0..7
         const int pt = pw * 32 + lane;                       // 0..255
         float tp[4][4], fx[4], fy[4];
@@ -318,22 +392,25 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
             float sm = (v[0] + v[1]) + (v[2] + v[3]);
             for (int o = 16; o > 0; o >>= 1) sm += __shfl_xor_sync(0xffffffffu, sm, o);
             if (lane == 0) red[pw * 2] = sm;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
+            AG_TL(TL_WG_BAR, asm volatile("bar.sync 1, 256;" ::: "memory"));
             const float mean = (((red[0] + red[2]) + (red[4] + red[6])) + ((red[8] + red[10]) + (red[12] + red[14]))) / 1024.f;
             float qs = 0.f;
 #pragma unroll
             for (int k = 0; k < 4; k++) { const float d = v[k] - mean; qs = fmaf(d, d, qs); }
             for (int o = 16; o > 0; o >>= 1) qs += __shfl_xor_sync(0xffffffffu, qs, o);
             if (lane == 0) red[pw * 2 + 1] = qs;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
+            AG_TL(TL_WG_BAR, asm volatile("bar.sync 1, 256;" ::: "memory"));
             const float inv = 1.f / (sqrtf((((red[1] + red[3]) + (red[5] + red[7])) + ((red[9] + red[11]) + (red[13] + red[15]))) / 1023.f) + 1e-7f);
 #pragma unroll
             for (int k = 0; k < 4; k++) { const int p = pix_of(k); sx[((p >> 5) + 1) * 34 + (p & 31) + 1] = (v[k] - mean) * inv; }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
+            AG_TL(TL_WG_BAR, asm volatile("bar.sync 1, 256;" ::: "memory"));
             // P planes, half by half
 #pragma unroll 1
             for (int hh = 0; hh < 2; hh++) {
-                mbar_wait(&p_empty[hh], (it & 1) ^ 1);   // layer-1 MMAs of the previous patch have consumed this half
+                AG_TL(TL_WAIT_P, mbar_wait(&p_empty[hh], (it & 1) ^ 1));   // layer-1 MMAs of the previous patch have completed on this half
+#ifdef AG_FIRST_TIMELINE
+                const long long tb = clock64();
+#endif
                 unsigned char* ph = sP + (size_t)hh * 2 * NPIXP * 16;
                 // one 16-byte window per thread and step: consecutive lanes read consecutive pixels and write consecutive slots (no bank
                 // conflicts; the shared-memory pipe is this kernel's busiest unit)
@@ -350,11 +427,19 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
                 }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                 mbar_arrive(&p_full[hh]);
+#ifdef AG_FIRST_TIMELINE
+                tl[TL_PBUILD] += (unsigned long long)(clock64() - tb);
+#endif
             }
             it++;
             pi = pn;
         }
     }
+#ifdef AG_FIRST_TIMELINE
+    tl[TL_TOTAL] = (unsigned long long)(clock64() - tl_start);
+    if (lane == 0 && *s_tl_slot < TL_LAUNCHES)
+        for (int i = 0; i < TL_STATES; i++) g_first_tl[*s_tl_slot][blockIdx.x][warp][i] = tl[i];
+#endif
 }
 
 }  // namespace tcx
