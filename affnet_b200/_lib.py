@@ -57,6 +57,13 @@ class PipelineEstimators(C.Structure):
     _fields_ = [("shape", C.c_int), ("num_baum_iters", C.c_int), ("shape_ps", C.c_int), ("ori", C.c_int), ("ori_ps", C.c_int)]
 
 
+DESC_HARDNET, DESC_SIFT = 0, 1
+
+
+class PipelineDescriptor(C.Structure):
+    _fields_ = [("kind", C.c_int), ("ps", C.c_int), ("clipval", C.c_float)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/affnet_b200.h
 vp, i32, f32, f64, sz = C.c_void_p, C.c_int, C.c_float, C.c_double, C.c_size_t
 PROTOTYPES = {
@@ -100,6 +107,9 @@ PROTOTYPES = {
     "ag_circular_gauss_kernel": (i32, [i32, f64, vp]),
     "ag_orientation_hist": (i32, [vp, i32, i32, vp, vp, vp]),
     "ag_baumberg_shape": (i32, [vp, i32, i32, vp, vp, vp]),
+    "ag_sift_windows": (i32, [i32, vp, vp, C.POINTER(i32), C.POINTER(i32)]),
+    "ag_sift_describe": (i32, [vp, i32, i32, f32, vp, vp]),
+    "ag_sift_describe_pyr": (i32, [C.POINTER(PyramidPlan), vp, vp, vp, vp, vp, i32, i32, f32, vp, vp]),
     "ag_distance_matrix": (i32, [vp, i32, vp, i32, i32, vp, vp]),
     "ag_match_snn_workspace_bytes": (sz, [i32, i32]),
     "ag_match_snn": (i32, [vp, i32, vp, i32, i32, f32, vp, sz, vp, vp, vp, vp, vp]),
@@ -107,6 +117,8 @@ PROTOTYPES = {
     "ag_match_pairs": (i32, [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, i32, f32, vp, sz, vp, vp, vp, vp, vp, vp, vp]),
     "ag_pipeline_create": (i32, [C.POINTER(PipelineConfig), vp, vp, vp, C.POINTER(vp)]),
     "ag_pipeline_create_ex": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), vp, vp, vp, C.POINTER(vp)]),
+    "ag_pipeline_create_desc": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), C.POINTER(PipelineDescriptor), vp, vp, vp,
+                                      C.POINTER(vp)]),
     "ag_pipeline_destroy": (None, [vp]),
     "ag_pipeline_workspace_bytes": (sz, [vp]),
     "ag_pipeline_plan": (C.POINTER(PyramidPlan), [vp]),

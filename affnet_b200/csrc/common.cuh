@@ -134,6 +134,14 @@ __device__ __forceinline__ void laf_sample_xy(const float* __restrict__ L, int h
     py = __fsub_rn(__fmaf_rn(a21, xj, __fmaf_rn(a22, yi, ty)), 0.5f);
 }
 
+// Gradient of a PS x PS patch with replicate padding; (wm, wp) = (w_minus, w_plus) of the (1x3) / (3x1) cross-correlation.  Used by the
+// hand-crafted estimators (handcrafted.cu) and the SIFT descriptor (sift.cu).
+__device__ __forceinline__ void grad_at(const float* p, int PS, int i, int j, float wm, float wp, float& gx, float& gy) {
+    const int jm = max(j - 1, 0), jp = min(j + 1, PS - 1), im = max(i - 1, 0), ip = min(i + 1, PS - 1);
+    gx = __fadd_rn(__fmul_rn(wm, p[i * PS + jm]), __fmul_rn(wp, p[i * PS + jp]));
+    gy = __fadd_rn(__fmul_rn(wm, p[im * PS + j]), __fmul_rn(wp, p[ip * PS + j]));
+}
+
 // Pyramid geometry passed by value to the kernels that sample pyr[oct][lvl] directly.
 struct PyrGeom {
     int n_octaves, n_levels, B;
@@ -159,6 +167,15 @@ int orientation_hist_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, cons
                          const int* d_count, int cap, int PS, const float* gk, float* d_R, void* stream);
 int baumberg_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
                  const int* d_count, int cap, int PS, int iters, const float* gk, float* d_A, void* stream);
+
+// SIFT descriptor (sift.cu).  sift_geometry: false unless 16 <= PS <= 65 and the pooling grid is 4 x 4, else k and s of
+// get_bin_weight_kernel_size_and_stride.  sift_windows: SIFTNet's Gaussian window gk [PS,PS] and pooling kernel pk [k,k] (host).
+// sift_pyr: ag_sift_describe_pyr with the windows given (the pipeline computes them once at create time).
+constexpr int SIFT_MIN_PS = 16, SIFT_MAX_PS = 65, SIFT_MAX_K = 25;
+bool sift_geometry(int PS, int* k, int* s);
+void sift_windows(int PS, int k, float* gk, float* pk);
+int sift_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl, const int* d_count,
+             int cap, int PS, int k, int s, const float* gk, const float* pk, float clipval, float* d_out, void* stream);
 
 // 2x2 products of the Baumberg chain in torch.bmm's fp32 operation order (row-by-column, two products added left to right); used by
 // mat2_compose_kernel / lafs_left_multiply_kernel (geometry.cu) and baumberg_pyr_kernel (handcrafted.cu).

@@ -16,13 +16,6 @@ __device__ __forceinline__ float warp_sum_f(float v) {
     return v;
 }
 
-// gradient with replicate padding; wx = (w_minus, w_plus) of the (1x3) cross-correlation
-__device__ __forceinline__ void grad_at(const float* p, int PS, int i, int j, float wm, float wp, float& gx, float& gy) {
-    const int jm = max(j - 1, 0), jp = min(j + 1, PS - 1), im = max(i - 1, 0), ip = min(i + 1, PS - 1);
-    gx = __fadd_rn(__fmul_rn(wm, p[i * PS + jm]), __fmul_rn(wp, p[i * PS + jp]));
-    gy = __fadd_rn(__fmul_rn(wm, p[im * PS + j]), __fmul_rn(wp, p[ip * PS + j]));
-}
-
 // OrientationDetector.forward on the PS x PS patch `p` (shared memory) of one warp; s_w [PS*PS], s_b [PS*PS], s_h [40] are the warp's
 // scratch.  Returns the angle on every lane.
 __device__ __forceinline__ float orientation_hist_warp(const float* p, int PS, const float* gk, float* s_w, unsigned char* s_b, float* s_h,

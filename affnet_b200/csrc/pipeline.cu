@@ -1,9 +1,11 @@
 // Batched end-to-end pipeline: ScaleSpaceAffinePatchExtractor.forward (SparseImgRepresenter.py:189-209) with any shape estimator
 // (AffNet or Baumberg, any number of iterations, or none) and orientation estimator (OriNet, gradient histogram or none)
-// + extract_patches_from_pyr (:181-188) + HardNet.forward for B images of one size, as a
+// + extract_patches_from_pyr (:181-188) + HardNet.forward or SIFTNet.forward for B images of one size, as a
 // fixed sequence of kernel launches on one stream with fixed-capacity buffers and device-side counters
 // (no host synchronisation, CUDA-graph capturable).  The reference processes one image at a time with
 // several .item()/nonzero host round trips (SURVEY.md §3); this is the on-device replacement.
+#include <math.h>
+
 #include <vector>
 
 #include "common.cuh"
@@ -11,7 +13,10 @@
 struct ag_pipeline {
     ag_pipeline_config_t cfg;
     ag_pipeline_estimators_t est;
-    std::vector<float> shape_gk, ori_gk;   // the hand-crafted estimators' Gaussian windows (HandCraftedModules._gauss_window), host copies
+    ag_pipeline_descriptor_t desc;
+    std::vector<float> shape_gk, ori_gk;
+    std::vector<float> sift_gk, sift_pk;   // SIFTNet's Gaussian window and pooling kernel (ag_sift_windows), host copies
+    int sift_k, sift_s;   // the hand-crafted estimators' Gaussian windows (HandCraftedModules._gauss_window), host copies
     ag_pyramid_plan_t plan;
     const ag_net_t* aff;
     const ag_net_t* ori;
@@ -26,7 +31,7 @@ struct ag_pipeline {
 
 using namespace ag;
 
-// ag_pipeline_create and ag_pipeline_create_ex: `fn` names the entry point the caller called in the error texts
+// ag_pipeline_create, ag_pipeline_create_ex and ag_pipeline_create_desc: `fn` names the entry point the caller called in the error texts
 #define PIPE_REQUIRE(cond, msg)                         \
     do {                                                \
         if (!(cond)) {                                  \
@@ -35,9 +40,18 @@ using namespace ag;
         }                                               \
     } while (0)
 
-static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_net_t* affnet,
-                           const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
-    PIPE_REQUIRE(cfg && est && hardnet && out, "NULL argument");
+static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est,
+                           const ag_pipeline_descriptor_t* desc, const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet,
+                           ag_pipeline_t** out) {
+    PIPE_REQUIRE(cfg && est && desc && out, "NULL argument");
+    PIPE_REQUIRE(desc->kind == AG_DESC_HARDNET || desc->kind == AG_DESC_SIFT, "unknown descriptor kind");
+    const bool sift = desc->kind == AG_DESC_SIFT;
+    PIPE_REQUIRE(sift || hardnet, "NULL argument: AG_DESC_HARDNET needs a HardNet");
+    PIPE_REQUIRE(sift || desc->ps == 32, "AG_DESC_HARDNET needs ps = 32");
+    int sift_k = 0, sift_s = 0;
+    PIPE_REQUIRE(!sift || sift_geometry(desc->ps, &sift_k, &sift_s),
+                 "AG_DESC_SIFT: unsupported ps (16..65 with a 4 x 4 pooling grid, not 17, 18, 23, 28, 38, 48, 58)");
+    PIPE_REQUIRE(!sift || (isfinite(desc->clipval) && desc->clipval > 0.f), "AG_DESC_SIFT: clipval must be finite and positive");
     PIPE_REQUIRE(est->shape == AG_SHAPE_NONE || est->shape == AG_SHAPE_AFFNET || est->shape == AG_SHAPE_BAUMBERG, "unknown shape estimator");
     PIPE_REQUIRE(est->ori == AG_ORI_NONE || est->ori == AG_ORI_ORINET || est->ori == AG_ORI_HISTOGRAM, "unknown orientation estimator");
     PIPE_REQUIRE(est->shape != AG_SHAPE_AFFNET || affnet, "AG_SHAPE_AFFNET needs an AffNet");
@@ -49,10 +63,10 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
     PIPE_REQUIRE(cfg->num_features >= 1, "num_features must be positive");
     const bool shape = est->shape != AG_SHAPE_NONE;
     ag_pipeline* p = new ag_pipeline();
-    p->cfg = *cfg; p->est = *est;
+    p->cfg = *cfg; p->est = *est; p->desc = *desc;
     p->aff = est->shape == AG_SHAPE_AFFNET ? affnet : nullptr;
     p->ori = est->ori == AG_ORI_ORINET ? orinet : nullptr;
-    p->hard = hardnet;
+    p->hard = sift ? nullptr : hardnet;
     int rc = ag_pyramid_plan(cfg->B, cfg->H, cfg->W, cfg->nlevels, cfg->init_sigma, cfg->border, &p->plan);
     if (rc != AG_OK) { delete p; return rc; }
     // the selection kernels sort in shared memory (ag_select_keypoints / ag_affine_shape_filter): fail here, not at run time
@@ -80,6 +94,12 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
         p->ori_gk.resize((size_t)ps * ps);
         ag_circular_gauss_kernel(ps, 0.0, p->ori_gk.data());
         for (float& v : p->ori_gk) v = v * 10.0f;
+    }
+    if (sift) {
+        p->sift_k = sift_k; p->sift_s = sift_s;
+        p->sift_gk.resize((size_t)desc->ps * desc->ps);
+        p->sift_pk.resize((size_t)sift_k * sift_k);
+        sift_windows(desc->ps, sift_k, p->sift_gk.data(), p->sift_pk.data());
     }
     p->M = shape ? (int)(1.5 * cfg->num_features) : cfg->num_features;  // SparseImgRepresenter.py:192-194
     p->cand_cap = cfg->cand_cap > 0 ? cfg->cand_cap : (cfg->H * cfg->W) / 8;
@@ -109,7 +129,7 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
         const size_t ob = ag_net_workspace_bytes(AG_NET_ORINET, (int)(B * K));
         if (ob > nb) nb = ob;
     }
-    size_t hb = ag_net_workspace_bytes(AG_NET_HARDNET, (int)(B * K));
+    const size_t hb = sift ? 0 : ag_net_workspace_bytes(AG_NET_HARDNET, (int)(B * K));
     p->net_bytes = nb > hb ? nb : hb;
     p->off_net = take(p->net_bytes);
     // AffNet with several iterations: the net's A of the current iteration, the other base_A buffer, the working LAFs
@@ -123,6 +143,8 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
 }
 #undef PIPE_REQUIRE
 
+static const ag_pipeline_descriptor_t HARDNET_DESC = {AG_DESC_HARDNET, 32, 0.2f};
+
 extern "C" {
 
 int ag_pipeline_create(const ag_pipeline_config_t* cfg, const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet,
@@ -130,12 +152,17 @@ int ag_pipeline_create(const ag_pipeline_config_t* cfg, const ag_net_t* affnet, 
     AG_REQUIRE(cfg && affnet && hardnet && out, "NULL argument");
     AG_REQUIRE(!cfg->do_ori || orinet, "do_ori needs an OriNet");
     const ag_pipeline_estimators_t est = {AG_SHAPE_AFFNET, 1, 0, cfg->do_ori ? AG_ORI_ORINET : AG_ORI_NONE, 0};
-    return pipeline_create(__func__, cfg, &est, affnet, orinet, hardnet, out);
+    return pipeline_create(__func__, cfg, &est, &HARDNET_DESC, affnet, orinet, hardnet, out);
 }
 
 int ag_pipeline_create_ex(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_net_t* affnet,
                           const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
-    return pipeline_create(__func__, cfg, est, affnet, orinet, hardnet, out);
+    return pipeline_create(__func__, cfg, est, &HARDNET_DESC, affnet, orinet, hardnet, out);
+}
+
+int ag_pipeline_create_desc(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
+                            const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
+    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, out);
 }
 
 void ag_pipeline_destroy(ag_pipeline_t* p) { delete p; }
@@ -212,9 +239,16 @@ int ag_pipeline_run(ag_pipeline_t* p, const float* d_img, void* d_ws, size_t ws_
     // denormalizeLAFs (LAF.py:407-417), then descriptor patches: level choice + normalizeLAFs (LAF.py:419-429)
     const float ms = (float)(c.H < c.W ? c.H : c.W);
     if ((rc = ag_lafs_scale(lafs2, d_lafs, B * K, ms, (float)c.W, (float)c.H, stream))) return rc;
-    if ((rc = ag_pyramid_level_for_lafs(&p->plan, d_lafs, B * K, 32, oct3, lvl3, stream))) return rc;
+    const int dps = p->desc.ps;
+    if ((rc = ag_pyramid_level_for_lafs(&p->plan, d_lafs, B * K, dps, oct3, lvl3, stream))) return rc;
     if ((rc = ag_lafs_scale(d_lafs, nlafs, B * K, 1.0f / ms, (float)(1.0 / (double)c.W), (float)(1.0 / (double)c.H), stream))) return rc;
-    if ((rc = ag_net_forward_pyr(p->hard, &p->plan, pyr, nlafs, oct3, lvl3, d_count, K, d_desc, netws, p->net_bytes, stream))) return rc;
+    if (p->desc.kind == AG_DESC_SIFT) {
+        if ((rc = sift_pyr(&p->plan, pyr, nlafs, oct3, lvl3, d_count, K, dps, p->sift_k, p->sift_s, p->sift_gk.data(), p->sift_pk.data(),
+                           p->desc.clipval, d_desc, stream)))
+            return rc;
+    } else if ((rc = ag_net_forward_pyr(p->hard, &p->plan, pyr, nlafs, oct3, lvl3, d_count, K, d_desc, netws, p->net_bytes, stream))) {
+        return rc;
+    }
     p->launches = g_launches - launches0;
     return AG_OK;
 }

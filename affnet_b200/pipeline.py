@@ -1,5 +1,5 @@
 """Batched detect-and-describe for B same-sized images (new API; the reference handles one image at a time):
-the whole ScaleSpaceAffinePatchExtractor.forward + extract_patches_from_pyr + HardNet chain as one fixed kernel
+the whole ScaleSpaceAffinePatchExtractor.forward + extract_patches_from_pyr + HardNet (or SIFTNet) chain as one fixed kernel
 sequence with device-side counters, optionally replayed as a CUDA graph.  The estimators follow ScaleSpaceAffinePatchExtractor's
 constructor (SparseImgRepresenter.py:26-49): AffNet or Baumberg iterations or no shape step, OriNet or gradient-histogram orientation."""
 import ctypes as C
@@ -9,6 +9,7 @@ import torch
 from . import _lib as L
 from .architectures import AffNetFast, OriNetFast
 from .HandCraftedModules import AffineShapeEstimator, OrientationDetector
+from .pytorch_sift import SIFTNet
 
 
 def estimators(AffNet, OriNet, do_ori, num_Baum_iters):
@@ -36,17 +37,27 @@ def estimators(AffNet, OriNet, do_ori, num_Baum_iters):
     return est, aff, ori
 
 
+def descriptor(HardNet):
+    """get_geometry_and_descriptors' `desc` as (ag_pipeline_descriptor_t, the native net or None): a SIFTNet describes with its patch size
+    and clipval and runs no net; anything else is HardNet on 32 x 32 patches."""
+    if isinstance(HardNet, SIFTNet):
+        return L.PipelineDescriptor(L.DESC_SIFT, HardNet.PS, HardNet.clipval), None
+    return L.PipelineDescriptor(L.DESC_HARDNET, 32, 0.2), HardNet
+
+
 class DetectDescribePipeline:
     def __init__(self, B, H, W, AffNet, HardNet, OriNet=None, num_features=2000, border=5, mrSize=5.192, nlevels=3,
                  init_sigma=1.6, do_ori=True, cand_cap=0, device="cuda", outputs=None, num_Baum_iters=1):
         """outputs: optional list of (lafs [B,K,2,3], desc [B,K,128], count [B] int32) CUDA tensors, one tuple per output slot, that the
         kernels write into directly (e.g. DescriptorExchange.outputs(): the blocks an all-gather sends); default: one private slot.
         AffNet / OriNet / do_ori / num_Baum_iters select the estimators as ScaleSpaceAffinePatchExtractor does (see `estimators`):
-        e.g. AffNet=AffineShapeEstimator(19), num_Baum_iters=16 is the HesAff baseline, num_Baum_iters=0 the plain detector."""
+        e.g. AffNet=AffineShapeEstimator(19), num_Baum_iters=16 is the HesAff baseline, num_Baum_iters=0 the plain detector.
+        HardNet may be a SIFTNet: the descriptors are then SIFTNet's at its patch size and clipval, and no checkpoint is needed."""
         self.cfg = L.PipelineConfig(B, H, W, num_features, nlevels, border, float(init_sigma), float(mrSize), 1 if do_ori else 0, cand_cap)
         self.est, aff, ori = estimators(AffNet, OriNet, do_ori, num_Baum_iters)
+        self.desc_cfg, hard = descriptor(HardNet)
         self.nets = (AffNet, OriNet, HardNet)  # keep the modules alive; the C pipeline only BORROWS their ag_net_t handles
-        self._used = (aff, ori, HardNet)      # the native nets the chosen mode runs (None: not used, or a hand-crafted estimator)
+        self._used = (aff, ori, hard)         # the native nets the chosen mode runs (None: not used, or a hand-crafted module)
         self._h = None
         self._net_handles = None
         self._bind_nets()
@@ -78,7 +89,7 @@ class DetectDescribePipeline:
             L.lib().ag_pipeline_destroy(self._h)
             self._h = None
         h = C.c_void_p()
-        L.check(L.lib().ag_pipeline_create_ex(C.byref(self.cfg), C.byref(self.est), hs[0], hs[1], hs[2], C.byref(h)))
+        L.check(L.lib().ag_pipeline_create_desc(C.byref(self.cfg), C.byref(self.est), C.byref(self.desc_cfg), hs[0], hs[1], hs[2], C.byref(h)))
         self._h, self._net_handles, self._graph = h, hs, None
 
     def _nets_current(self):

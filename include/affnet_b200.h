@@ -255,6 +255,23 @@ int ag_circular_gauss_kernel(int kernlen, double sigma, float* h_out);
 int ag_orientation_hist(const float* d_patches, int n, int PS, const float* d_gk, float* d_angle, void* stream);
 int ag_baumberg_shape(const float* d_patches, int n, int PS, const float* d_gk, float* d_A, void* stream);
 
+/* SIFT descriptor: replaces SIFTNet.forward (pytorch_sift.py:69-94) with 8 angle bins and 4 x 4 spatial bins -> [n,128] in
+ * [bin][cy][cx] order: (-1, 0, 1) gradients with replicate borders, magnitude times the module's Gaussian window, angle bins
+ * interpolated linearly, a k x k tent pooling with stride s per angle bin, L2 normalisation, clamp(0, clipval), L2 normalisation.
+ * Supported patch sizes: 16..65 where the pooling grid comes out 4 x 4 (all but 17, 18, 23, 28, 38, 48, 58); AG_ERR_INVALID otherwise.
+ *   ag_sift_windows       host only: SIFTNet.CircularGaussKernel h_gk [PS,PS] (centre PS/2, not normalised) and getPoolingKernel
+ *                         h_pk [k,k], with k = 2 s - 1 and s = round(2 floor(PS/2) / 5), as SIFTNet.__init__ builds them in float64 and
+ *                         rounds to fp32.  Any output may be NULL.
+ *   ag_sift_describe      d_patches [n,PS,PS] -> d_out [n,128].  clipval finite and positive (the reference's 0.2).
+ *   ag_sift_describe_pyr  samples each keypoint's patch from the pyramid as ag_extract_patches_pyr does (same layout, d_count [B] or
+ *                         NULL) and describes it without writing the patch: d_out [B,cap,128], bit-identical to ag_extract_patches_pyr
+ *                         followed by ag_sift_describe.  Rows at or beyond d_count[b] (all of them for a count of -1) are not written.
+ * Deterministic: a row's bits do not depend on the launch or the other rows.  One launch; no allocation. */
+int ag_sift_windows(int PS, float* h_gk, float* h_pk, int* k, int* stride);
+int ag_sift_describe(const float* d_patches, int n, int PS, float clipval, float* d_out, void* stream);
+int ag_sift_describe_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                         const int* d_count, int cap, int PS, float clipval, float* d_out, void* stream);
+
 /* Descriptor matching (SURVEY.md §8f row 3).
  *   ag_distance_matrix replaces distance_matrix_vector (Losses.py:5-13): out[n1,n2] = sqrt(|a|^2 + |b|^2 - 2 a.b + 1e-6)
  *   ag_match_snn       replaces the SNN-ratio block of train_AffNet_test_on_graffity.py:292-298: nearest neighbour, then
@@ -335,6 +352,23 @@ typedef struct {
  * int(1.5 K) > 16384 keypoints with a shape estimator (K > 10923), K > 16384 without. */
 int ag_pipeline_create_ex(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_net_t* affnet,
                           const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
+
+/* Descriptor of the pipeline (get_geometry_and_descriptors(img, det, desc)'s `desc`):
+ *   AG_DESC_HARDNET  HardNet (hardnet) on 32 x 32 patches; ps must be 32, clipval is ignored.
+ *   AG_DESC_SIFT     SIFTNet(patch_size = ps, clipval) (ag_sift_describe_pyr) in one launch that samples the pyramid directly; hardnet
+ *                    may be NULL.  The descriptor's pyramid level is chosen for ps (ag_pyramid_level_for_lafs).  The workspace holds no
+ *                    HardNet buffers, and no net buffers at all without AG_SHAPE_AFFNET and AG_ORI_ORINET.
+ * ag_pipeline_create_ex is ag_pipeline_create_desc with {AG_DESC_HARDNET, 32, -}.  AG_ERR_INVALID (before any CUDA call) additionally
+ * for an unknown kind, HardNet with ps != 32 or without a net, SIFT with an unsupported ps or a clipval that is not finite and positive. */
+#define AG_DESC_HARDNET 0
+#define AG_DESC_SIFT 1
+typedef struct {
+    int kind;       /* AG_DESC_* */
+    int ps;         /* descriptor patch size: 32 for HardNet; a supported ag_sift_windows size for SIFT (the reference's 65 by default) */
+    float clipval;  /* SIFT: the clip between the two L2 normalisations (the reference's 0.2) */
+} ag_pipeline_descriptor_t;
+int ag_pipeline_create_desc(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
+                            const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
 void ag_pipeline_destroy(ag_pipeline_t* p);
 size_t ag_pipeline_workspace_bytes(const ag_pipeline_t* p);
 const ag_pyramid_plan_t* ag_pipeline_plan(const ag_pipeline_t* p);
