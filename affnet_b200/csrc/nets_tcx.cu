@@ -42,10 +42,10 @@ static int ensure_smem_attr(const void* func, int bytes, bool* configured, const
     return rc;
 }
 
-template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int BF = 0, int MC = 0>
+template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int BF = 0, int MC = 0, int PPS = 0>
 static int launch_conv(const void* in, void* out, const __half* w, const float* b, float inv_scale, int n, int group, const int* count, cudaStream_t st) {
     using Cfg = XCfg<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA>;
-    auto kern = tcx_conv_kernel<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA, BF, MC>;
+    auto kern = tcx_conv_kernel<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA, BF, MC, PPS>;
     static bool configured[64] = {};   // per device (the attribute is per device)
     int rc = ensure_smem_attr((const void*)kern, (int)Cfg::SMEM, configured, "tcx_conv smem attr");
     if (rc != AG_OK) return rc;
@@ -184,6 +184,9 @@ size_t tcx_act_bytes(int n) { return (size_t)(n + 1) * 65536; }
 #ifndef AG_HARD_MC6
 #define AG_HARD_MC6 0
 #endif
+// tcx_conv_kernel's last template argument selects the ping-pong schedule (tcx_conv.cuh) for the layers it makes faster: AffNet / OriNet
+// layer 6 and HardNet layers 5 and 6 (H100, DESIGN.md section 4).  The 16x16-output layers and AffNet / OriNet layer 5 are close to their
+// HBM floor and were no faster with it (AffNet layer 5 3-5 % slower).
 // Layers 1-3 run in one kernel (layer 2's 32x32 output stays in shared memory).  upto = 2 runs the layers 1-2 kernel instead, which
 // writes layer 2's output to bufB for the debug decode.
 int tcx_trunk_affori(const ag_net* net, const tc::FirstSrc& src0, int n, int group, const int* count, void* bufA, void* bufB, void* feat,
@@ -200,7 +203,7 @@ int tcx_trunk_affori(const ag_net* net, const tc::FirstSrc& src0, int n, int gro
     if (upto <= 4) return AG_OK;
     if ((rc = launch_conv<32, 64, 16, 2, 1, 2, L_S1_8P, 1, 1, 1>(bufB, bufA, net->d_wx[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
     if (upto <= 5) return AG_OK;
-    return launch_conv<64, 64, 8, 1, 1, 2, L_HEAD, 1, 1, 1>(bufA, feat, net->d_wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
+    return launch_conv<64, 64, 8, 1, 1, 2, L_HEAD, 1, 1, 1, 0, 0, 1>(bufA, feat, net->d_wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
 }
 
 template <int BF>
@@ -217,9 +220,9 @@ static int trunk_hardnet_t(const ag_net* net, const tc::FirstSrc& src0, int n, i
     if (upto <= 3) return AG_OK;
     if ((rc = launch_conv<64, 64, 16, 1, 1, 2, L_S2_8P, 0, AG_HARD_SW4, 0, BF>(bufA, bufB, wx[3], net->d_b[3], net->w_inv_scale[3], n, group, count, st))) return rc;
     if (upto <= 4) return AG_OK;
-    if ((rc = launch_conv<64, 128, 16, 2, 2, 2, L_S1_8P, 0, 0, 0, BF, AG_HARD_MC5>(bufB, bufA, wx[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
+    if ((rc = launch_conv<64, 128, 16, 2, 2, 2, L_S1_8P, 0, 0, 0, BF, AG_HARD_MC5, 1>(bufB, bufA, wx[4], net->d_b[4], net->w_inv_scale[4], n, group, count, st))) return rc;
     if (upto <= 5) return AG_OK;
-    return launch_conv<128, 128, 8, 1, 2, 2, L_HEAD, 0, 0, 0, BF, AG_HARD_MC6>(bufA, headbuf, wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
+    return launch_conv<128, 128, 8, 1, 2, 2, L_HEAD, 0, 0, 0, BF, AG_HARD_MC6, 1>(bufA, headbuf, wx[5], net->d_b[5], net->w_inv_scale[5], n, group, count, st);
 }
 
 int tcx_trunk_hardnet(const ag_net* net, const tc::FirstSrc& src0, int n, int group, const int* count, void* bufA, void* bufB, void* headbuf,
@@ -280,6 +283,31 @@ int ag_first_timeline_read(unsigned long long* host, int* dims, int reset) {
         return rc;
     }
     return AG_OK;
+}
+#endif
+
+#ifdef AG_CONV_TIMELINE
+// Developer builds with -DAG_CONV_TIMELINE only (scripts/conv_kernel_timeline.py): copy the per-warp state cycle sums of
+// tcx_conv_kernel, uint64 [CT_LAUNCHES][CT_CTAS][9 warps][CT_STATES], and CTA 0's block events, uint64 [CT_LAUNCHES][2 warpgroups]
+// [CT_EVENTS][issue start | MMAs done | epilogue end] (0: no such block), in launch order since the last reset, to `sums` / `events`
+// (either may be NULL); reset != 0 then clears them.  dims (may be NULL) receives CT_LAUNCHES, CT_CTAS, CT_STATES, CT_EVENTS.
+int ag_conv_timeline_read(unsigned long long* sums, unsigned long long* events, int* dims, int reset) {
+    using namespace tcx;
+    if (dims) { dims[0] = CT_LAUNCHES; dims[1] = CT_CTAS; dims[2] = CT_STATES; dims[3] = CT_EVENTS; }
+    int rc = check_cuda(cudaDeviceSynchronize(), "timeline read");
+    if (rc == AG_OK && sums) rc = check_cuda(cudaMemcpyFromSymbol(sums, g_conv_tl, sizeof(g_conv_tl)), "timeline read");
+    if (rc == AG_OK && events) rc = check_cuda(cudaMemcpyFromSymbol(events, g_conv_ev, sizeof(g_conv_ev)), "timeline read");
+    if (rc == AG_OK && reset) {
+        void* p = nullptr;
+        const int zl[CT_CTAS] = {};
+        if (rc == AG_OK) rc = check_cuda(cudaGetSymbolAddress(&p, g_conv_tl), "timeline reset");
+        if (rc == AG_OK) rc = check_cuda(cudaMemset(p, 0, sizeof(g_conv_tl)), "timeline reset");
+        if (rc == AG_OK) rc = check_cuda(cudaGetSymbolAddress(&p, g_conv_ev), "timeline reset");
+        if (rc == AG_OK) rc = check_cuda(cudaMemset(p, 0, sizeof(g_conv_ev)), "timeline reset");
+        if (rc == AG_OK) rc = check_cuda(cudaMemcpyToSymbol(g_conv_tl_launch, zl, sizeof(zl)), "timeline reset");
+        if (rc == AG_OK) rc = check_cuda(cudaDeviceSynchronize(), "timeline reset");
+    }
+    return rc;
 }
 #endif
 

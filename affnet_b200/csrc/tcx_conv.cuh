@@ -27,16 +27,81 @@
 //
 // Warp roles: 0-7 two consumer warpgroups (warpgroup g takes the M = 64 blocks g, g + 2, ... of a unit: wgmma into registers, then the
 // epilogue from the accumulator fragment) | 8 loader (cp.async.bulk per channel group and plane).  The MMAs and the epilogue of one
-// block are xconv_block_mma / xconv_block_epilogue, which tcx_first_kernel also runs for layer 3 of AffNet / OriNet.
+// block are xconv_block_issue + wgmma_wait / xconv_block_epilogue, which tcx_first_kernel also runs for layer 3 of AffNet / OriNet.
+//
+// Ping-pong (template switch PPS, set per launch in nets_tcx.cu; used at 8x8 outputs, BLOCKS = 2: one block per warpgroup and unit,
+// where the MMAs are a large share of the time): the two warpgroups issue their blocks' MMAs in strict turns,
+// ordered by a pair of named barriers (warpgroup 0 unit k, warpgroup 1 unit k, warpgroup 0 unit k + 1, ...).  A warpgroup's MMAs are
+// then queued behind its partner's, and its epilogue runs while the tensor core works through the partner's block; without the order
+// both warpgroups issue together, wait together and leave the tensor core idle through both epilogues.  Each warp releases the stage
+// as soon as its MMAs on it have completed, before its epilogue, so the loader can refill it during the epilogue.  Both warpgroups
+// still share each unit: owning whole units would need a stage per warpgroup plus one to load into, and the 8x8 layers fit only two
+// (226 KB of shared memory at HardNet / AffNet layer 6).  The other launches keep the plain schedule (both warpgroups issue at once and
+// release the stage after their epilogues), and so does every launch in a build with AG_CONV_PINGPONG = 0 (A/B runs).
 #pragma once
 #include <cuda_bf16.h>
 
 #include "tc_conv.cuh"
 
+#ifndef AG_CONV_PINGPONG
+#define AG_CONV_PINGPONG 1
+#endif
+
 namespace ag {
 namespace tcx {
 
 using namespace ag::tc;
+
+constexpr int XORDER = 5;    // ping-pong: named barrier XORDER + g lets warpgroup g issue its next block's MMAs (3, 4: the warpgroups)
+
+// AG_CONV_TIMELINE (developer builds, scripts/conv_kernel_timeline.py): every warp of the split-0 CTAs 0 .. CT_CTAS - 1 adds up the SM
+// cycles (clock64) it spends in each CT_* state and stores the sums per launch in g_conv_tl; warp 0 of each consumer warpgroup of CTA 0
+// also logs, per block, when its MMA issue starts, when its MMAs have completed and when its epilogue ends (g_conv_ev), from which the
+// script derives how much of the epilogues overlap and how long no MMA was in flight.  ag_conv_timeline_read copies both out.
+// States: consumers  TOTAL | wait full | wait for the turn (ping-pong) | issue MMAs | wgmma_wait | epilogue | warpgroup barrier | - | other
+//         loader     TOTAL | -         | -                              | -          | -          | -        | -                 | wait empty | other
+enum { CT_TOTAL, CT_WAIT_FULL, CT_TURN, CT_ISSUE, CT_MMA_WAIT, CT_EPILOGUE, CT_WG_BAR, CT_WAIT_EMPTY, CT_OTHER, CT_STATES };
+#ifdef AG_CONV_TIMELINE
+constexpr int CT_CTAS = 4, CT_LAUNCHES = 16, CT_EVENTS = 2048;
+__device__ unsigned long long g_conv_tl[CT_LAUNCHES][CT_CTAS][9][CT_STATES];
+__device__ unsigned long long g_conv_ev[CT_LAUNCHES][2][CT_EVENTS][3];
+__device__ int g_conv_tl_launch[CT_CTAS];
+struct ConvTimeline {
+    unsigned long long t[CT_STATES];
+    long long start, mark;
+    int slot, warp, n_ev;   // slot CT_LAUNCHES: not recorded
+    // thread 0, before the block-wide barrier: this launch's slot in g_conv_tl, published in shared memory
+    __device__ static void claim(int* s_slot) {
+        if (threadIdx.x == 0)
+            *s_slot = (blockIdx.y == 0 && blockIdx.x < CT_CTAS) ? min(atomicAdd(&g_conv_tl_launch[blockIdx.x], 1), CT_LAUNCHES) : CT_LAUNCHES;
+    }
+    __device__ void init(const int* s_slot) {
+        for (int i = 0; i < CT_STATES; i++) t[i] = 0;
+        slot = *s_slot; warp = threadIdx.x >> 5; n_ev = 0;
+        start = mark = clock64();
+    }
+    // the cycles since the previous lap go to `state`
+    __device__ void lap(int state) { const long long now = clock64(); t[state] += (unsigned long long)(now - mark); mark = now; }
+    // event k of the current block (0 issue start, 1 MMAs done, 2 epilogue end) at the last lap's time
+    __device__ void event(int k) {
+        if (blockIdx.x == 0 && slot < CT_LAUNCHES && (threadIdx.x & 127) == 0 && n_ev < CT_EVENTS) g_conv_ev[slot][warp >> 2][n_ev][k] = (unsigned long long)mark;
+        if (k == 2) n_ev++;
+    }
+    __device__ void finish() {
+        t[CT_TOTAL] = (unsigned long long)(clock64() - start);
+        if ((threadIdx.x & 31) == 0 && slot < CT_LAUNCHES)
+            for (int i = 0; i < CT_STATES; i++) g_conv_tl[slot][blockIdx.x][warp][i] = t[i];
+    }
+};
+#else
+struct ConvTimeline {
+    __device__ static void claim(int*) {}
+    __device__ void init(const int*) {}
+    __device__ void lap(int) {}
+    __device__ void event(int) {}
+    __device__ void finish() {}
+};
+#endif
 
 enum XLayout { L_S2_16 = 0, L_S1_16 = 1, L_S2_8P = 2, L_S1_8P = 3, L_HEAD = 4 };
 
@@ -48,9 +113,12 @@ __device__ __forceinline__ void bulk_g2s_mc(void* dst, const void* src, uint32_t
                  "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask)
                  : "memory");
 }
-// arrive on the barrier at the same shared-memory offset of CTA `cta` of the cluster
+// arrive on the barrier at the same shared-memory offset of CTA `cta` of the cluster.  Release at CTA scope (the default semantics):
+// the consumers' arrivals on `empty` only have to follow their own completed wgmma reads of the stage (wgmma_wait), not their global
+// stores.  A cluster-scope release compiles to MEMBAR.ALL.GPU before the arrival, which waits for every store the warp still has in
+// flight (the previous block's epilogue) and stalled the consumers of the multicast layer for about a fifth of their cycles.
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-    asm volatile("{\n .reg .b32 ra;\n mapa.shared::cluster.u32 ra, %0, %1;\n mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n}\n" ::"r"(smem_u32(bar)), "r"(cta)
+    asm volatile("{\n .reg .b32 ra;\n mapa.shared::cluster.u32 ra, %0, %1;\n mbarrier.arrive.release.cta.shared::cluster.b64 _, [ra];\n}\n" ::"r"(smem_u32(bar)), "r"(cta)
                  : "memory");
 }
 __device__ __forceinline__ void cluster_sync() {
@@ -183,9 +251,8 @@ __device__ __forceinline__ void frag_right(float v0, float v1, int lane, float& 
 __device__ __forceinline__ bool xpatch_valid(const XArgs& a, int pi) { return pi < a.n && (a.count == nullptr || (pi % a.group) < a.count[pi / a.group]); }
 
 // The MMAs of one M = 64 block of a layer (Cfg: XCfg) into d[ACCW / 2]: a_t = the block's first slot in shared memory, w_base = the
-// layer's packed weights (both in 16-byte units).  The input's channel groups are Cfg::GS slots apart.  xconv_block_issue issues and
-// commits them as one wgmma group and returns at once (the caller waits before it reads d); xconv_block_mma also waits for them.
-// tcx_conv_kernel runs xconv_block_mma, the layer-3 stage of tcx_first_kernel xconv_block_issue.
+// layer's packed weights (both in 16-byte units).  The input's channel groups are Cfg::GS slots apart.  Issues and commits them as one
+// wgmma group and returns at once: the caller waits (wgmma_wait, wgmma_reg_fence) before it reads d.
 template <class Cfg, int BF>
 __device__ __forceinline__ void xconv_block_issue(float* d, uint32_t a_t, uint32_t w_base) {
     using In = typename Cfg::In;
@@ -234,14 +301,7 @@ __device__ __forceinline__ void xconv_block_issue(float* d, uint32_t a_t, uint32
     }
     wgmma_commit();
 }
-template <class Cfg, int BF>
-__device__ __forceinline__ void xconv_block_mma(float* d, uint32_t a_t, uint32_t w_base) {
-    xconv_block_issue<Cfg, BF>(d, a_t, w_base);
-    wgmma_wait<0>();
-    wgmma_reg_fence<Cfg::ACCW / 2>(d);
-}
-
-// Epilogue of one block from the accumulator fragment d (xconv_block_mma) of warp wq of a warpgroup: x shifts, bias, ReLU, fp16 hi [+ lo]
+// Epilogue of one block from the accumulator fragment d (xconv_block_issue, completed) of warp wq of a warpgroup: x shifts, bias, ReLU, fp16 hi [+ lo]
 // into a.out in the layout Cfg::OUTL.  Rows r = 64 b + 16 wq + lane/4 + 8 h of unit u, columns 8 j + 2 (lane % 4) + e of each NT block;
 // output channels from split * NT on.
 template <class Cfg, int BF>
@@ -313,13 +373,14 @@ __device__ __forceinline__ void xconv_block_epilogue(const float* d, const XArgs
 
 // MC = 1 (NSPLIT = 2 only): the two CTAs of a unit form a thread-block cluster (1 x 2); each loader fetches half of the unit's planes and
 // multicasts them to both, so the input crosses the L2 -> SM fabric once instead of twice.
-template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int BF = 0, int MC = 0>
+template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int BF = 0, int MC = 0, int PPS = 0>
 __global__ void __launch_bounds__(288, 1) tcx_conv_kernel(const XArgs a) {
     static_assert(MC == 0 || NSPLIT == 2, "multicast pairs the two channel-split CTAs");
     using Cfg = XCfg<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA>;
     using In = typename Cfg::In;
     constexpr int ACCW = Cfg::ACCW, BLOCKS = Cfg::BLOCKS, GS = Cfg::GS, RW = In::RW;
     constexpr int PAIR = In::PAIR;
+    constexpr bool PP = AG_CONV_PINGPONG && PPS;   // PPS: this launch runs the ping-pong schedule
     extern __shared__ __align__(1024) unsigned char smem[];
     uint64_t* full = reinterpret_cast<uint64_t*>(smem);  // [STAGES]
     uint64_t* empty = full + STAGES;                       // [STAGES]
@@ -332,18 +393,30 @@ __global__ void __launch_bounds__(288, 1) tcx_conv_kernel(const XArgs a) {
     const int split = blockIdx.y;
     const int n_units = PAIR ? (a.n + 1) >> 1 : a.n;
 
+    int* s_tl_slot = reinterpret_cast<int*>(smem + 496);    // AG_CONV_TIMELINE: after the barriers (2 STAGES + 1 <= 60 of them)
+
     if (threadIdx.x < Cfg::NT) s_bias[threadIdx.x] = a.bias[split * Cfg::NT + threadIdx.x];
     if (threadIdx.x == 0) {
-        // empty: one arrival per consumer warpgroup (MC: of both CTAs, the stage holds planes multicast by both loaders)
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2 * (1 + MC)); }
+        // empty, MC: arrivals of both CTAs, the stage holds planes multicast by both loaders
+        //   ping-pong: one arrival per consumer warp, when its last MMAs on the stage have completed
+        //   otherwise: one per consumer warpgroup, after its epilogues
+        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], (PP ? 8 : 2) * (1 + MC)); }
         mbar_init(wbar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    ConvTimeline::claim(s_tl_slot);
     // zero rows of every stage: written once, the loader only ever writes data rows
     for (int i = threadIdx.x; i < (int)(Cfg::IN_BYTES / 16); i += blockDim.x) reinterpret_cast<uint4*>(sIn)[i] = make_uint4(0, 0, 0, 0);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
     if (MC) cluster_sync();      // the peer's barriers are initialised before anything is multicast into this CTA
+    ConvTimeline tl;
+    tl.init(s_tl_slot);
+    // one consumer warp's arrival(s) on `empty`
+    auto release = [&](uint64_t* e) {
+        if (MC) { mbar_arrive_cluster(e, 0); mbar_arrive_cluster(e, 1); }
+        else mbar_arrive(e);
+    };
 
     auto uvalid = [&](int u) -> bool { return PAIR ? (xpatch_valid(a, 2 * u) || xpatch_valid(a, 2 * u + 1)) : xpatch_valid(a, u); };
 
@@ -356,7 +429,9 @@ __global__ void __launch_bounds__(288, 1) tcx_conv_kernel(const XArgs a) {
             for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
                 if (!uvalid(u)) continue;
                 const int s = it % STAGES;
+                tl.lap(CT_OTHER);
                 mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+                tl.lap(CT_WAIT_EMPTY);
                 mbar_expect_tx(&full[s], Cfg::UNIT_IN_BYTES);
                 const unsigned char* gsrc = reinterpret_cast<const unsigned char*>(a.in) + (size_t)u * Cfg::UNIT_IN_BYTES;
 #pragma unroll 1
@@ -370,9 +445,11 @@ __global__ void __launch_bounds__(288, 1) tcx_conv_kernel(const XArgs a) {
                     }
                 it++;
             }
+            tl.lap(CT_OTHER);
             if (MC) {   // drain: the peer's last arrivals on this CTA's `empty` barriers must have landed before the CTA may exit
                 for (int k = 0; k < STAGES && k < it; k++) { const int j = it - 1 - k; mbar_wait(&empty[j % STAGES], (j / STAGES) & 1); }
             }
+            tl.lap(CT_WAIT_EMPTY);
         }
     } else if (warp < 8) {
         // ===== consumers: warpgroup wg takes the M = 64 blocks wg, wg + 2, ... of every unit =====
@@ -384,22 +461,42 @@ __global__ void __launch_bounds__(288, 1) tcx_conv_kernel(const XArgs a) {
         for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
             if (!uvalid(u)) continue;
             const int s = it % STAGES;
+            tl.lap(CT_OTHER);
             mbar_wait(&full[s], (it / STAGES) & 1);
+            tl.lap(CT_WAIT_FULL);
             const uint32_t st_base = in_base + (uint32_t)(s * In::SLOT_STAGE);
 #pragma unroll 1
             for (int b = wg; b < BLOCKS; b += 2) {
                 float d[ACCW / 2];
-                xconv_block_mma<Cfg, BF>(d, st_base + (uint32_t)(b * 64), w_base);
+                // ping-pong: the turns alternate over the whole run, as both warpgroups take BLOCKS / 2 blocks of every unit.
+                // Warpgroup 0's first block is the only one not preceded by a partner block.
+                if (PP && (wg == 1 || it > 0 || b > 0)) bar_sync(XORDER + wg, 256);
+                tl.lap(CT_TURN);
+                tl.event(0);
+                xconv_block_issue<Cfg, BF>(d, st_base + (uint32_t)(b * 64), w_base);
+                if (PP) asm volatile("bar.arrive %0, 256;" ::"r"(XORDER + (wg ^ 1)) : "memory");   // the partner's turn
+                tl.lap(CT_ISSUE);
+                wgmma_wait<0>();
+                wgmma_reg_fence<ACCW / 2>(d);
+                tl.lap(CT_MMA_WAIT);
+                tl.event(1);
+                // ping-pong: this warp's last MMAs on the stage have completed; the epilogue reads registers only
+                if (PP && b + 2 >= BLOCKS && lane == 0) release(&empty[s]);
                 xconv_block_epilogue<Cfg, BF>(d, a, s_bias, u, b, split, wq, lane);
+                tl.lap(CT_EPILOGUE);
+                tl.event(2);
             }
-            bar_sync(3 + wg, 128);   // every warp of the warpgroup has finished its MMAs on this stage
-            if ((threadIdx.x & 127) == 0) {
-                if (MC) { mbar_arrive_cluster(&empty[s], 0); mbar_arrive_cluster(&empty[s], 1); }
-                else mbar_arrive(&empty[s]);
+            if (!PP) {
+                bar_sync(3 + wg, 128);   // every warp of the warpgroup has finished its MMAs on this stage
+                tl.lap(CT_WG_BAR);
+                if ((threadIdx.x & 127) == 0) release(&empty[s]);
             }
             it++;
         }
+        if (PP && wg == 0 && it > 0) bar_sync(XORDER, 256);   // warpgroup 1's arrival after its last block
+        tl.lap(CT_OTHER);
     }
+    tl.finish();
     __syncthreads();
     if (MC) cluster_sync();      // neither CTA leaves while the other may still signal its barriers
 }
