@@ -19,11 +19,18 @@
 //
 // Activations between layers (HBM): fp16, 16-byte slots of 8 channels, [unit][channel group (hi groups, then lo groups)][plane][slot],
 // data rows only (the consumer's loader places them between zero rows in shared memory):
-//   L_S2_16  stride-2 consumer on a 32x32 map   unit = patch   4 parity planes x 256 slots  slot = (y/2)*16 + x/2, plane = (y&1)*2 + (x&1)
-//   L_S1_16  stride-1 consumer on a 16x16 map   unit = patch   256 slots                    slot = y*16 + x
-//   L_S2_8P  stride-2 consumer on a 16x16 map   unit = PAIR    4 parity planes x 128 slots  slot = ((y/2)*2 + p)*8 + x/2
-//   L_S1_8P  stride-1 consumer on an 8x8 map    unit = PAIR    128 slots                    slot = (y*2 + p)*8 + x       (p = patch & 1)
+//   L_S2_16  stride-2 consumer on a 32x32 map   unit = patch   4 parity planes x 256 slots  slot = (y/2)*16 + rpos(x/2), plane = (y&1)*2 + (x&1)
+//   L_S1_16  stride-1 consumer on a 16x16 map   unit = patch   256 slots                    slot = y*16 + rpos(x)
+//   L_S2_8P  stride-2 consumer on a 16x16 map   unit = PAIR    4 parity planes x 128 slots  slot = (y/2)*16 + ppos(x/2, p)
+//   L_S1_8P  stride-1 consumer on an 8x8 map    unit = PAIR    128 slots                    slot = y*16 + ppos(x, p)       (p = patch & 1)
 //   L_HEAD   the 8x8 head GEMM's A operand (tc_head.cuh): [patch/128][pixel*C/8 + c/8][patch%128][8] (+ a residual plane behind it)
+// Neighbour-paired order inside every 16-slot row group (one row of 16 pixels, or the 8 pixels of patch 0 and of patch 1 of one row):
+// the even-x pixels first, then the odd-x pixels, so that M row i < 8 of a warp's 16 rows holds an even pixel and row i + 8 its right
+// neighbour, and a thread (rows lane/4 and lane/4 + 8) holds both:
+//   rpos(x) = (x&1)*8 + x/2                  x = 0 .. 15
+//   ppos(x, p) = (x&1)*8 + p*4 + x/2         x = 0 .. 7: rows 0-3 patch 0 at x = 0, 2, 4, 6, rows 4-7 patch 1, rows 8-15 the odd x
+// Whole rows stay whole rows, so the dy shift (one row further), the zero rows and the M = 64 blocks are those of the natural order.
+// The 32x32 layer-1 stage of tcx_first_kernel orders each half row of 16 pixels the same way.
 //
 // Warp roles: 0-7 two consumer warpgroups (warpgroup g takes the M = 64 blocks g, g + 2, ... of a unit: wgmma into registers, then the
 // epilogue from the accumulator fragment) | 8 loader (cp.async.bulk per channel group and plane).  The MMAs and the epilogue of one
@@ -167,12 +174,16 @@ __device__ __forceinline__ void split_pack2(float v0, float v1, uint32_t& hi, ui
 // slots per channel group and unit of an HBM activation layout, and patches per unit
 __host__ __device__ constexpr int layout_slots(int lay) { return lay == L_S2_16 ? 1024 : lay == L_S1_16 ? 256 : lay == L_S2_8P ? 512 : 128; }
 __host__ __device__ constexpr int layout_pair(int lay) { return (lay == L_S2_8P || lay == L_S1_8P) ? 1 : 0; }
+// position of pixel x inside a 16-slot row group (neighbour-paired order, see the top of this file): a row of 16 pixels, or of two
+// patches' 8 pixels each (p = patch parity)
+__host__ __device__ constexpr int rpos(int x) { return (x & 1) * 8 + (x >> 1); }
+__host__ __device__ constexpr int ppos(int x, int p) { return (x & 1) * 8 + p * 4 + (x >> 1); }
 // slot of pixel (y, x) of patch parity p in a layout
 __host__ __device__ constexpr int layout_slot(int lay, int y, int x, int p) {
-    return lay == L_S2_16 ? ((y & 1) * 2 + (x & 1)) * 256 + (y >> 1) * 16 + (x >> 1)
-         : lay == L_S1_16 ? y * 16 + x
-         : lay == L_S2_8P ? ((y & 1) * 2 + (x & 1)) * 128 + ((y >> 1) * 2 + p) * 8 + (x >> 1)
-                          : (y * 2 + p) * 8 + x;
+    return lay == L_S2_16 ? ((y & 1) * 2 + (x & 1)) * 256 + (y >> 1) * 16 + rpos(x >> 1)
+         : lay == L_S1_16 ? y * 16 + rpos(x)
+         : lay == L_S2_8P ? ((y & 1) * 2 + (x & 1)) * 128 + (y >> 1) * 16 + ppos(x >> 1, p)
+                          : y * 16 + ppos(x, p);
 }
 
 // Geometry of a layer's input in shared memory.  H: input map edge, STRIDE 1 | 2.
@@ -232,21 +243,15 @@ struct XCfg {
     static_assert(OUT == L_HEAD || layout_pair(OUT) || !In::PAIR, "a pair layer writes pair layouts or the head operand");
 };
 
-// Neighbours of an accumulator fragment value along x: v0 / v1 are the values of rows i = lane/4 and i + 8 of this warp's 16 rows.
-// Row i - 1 (left) and i + 1 (right); a neighbour outside the image row is garbage that callers must drop by a select, never by
-// multiplying with 0: in the pair layouts it is the other patch of the unit, whose input rows are stale workspace when that patch is
-// skipped (beyond a count, or the tail of an odd n).  NaN * 0 = NaN, and the ReLU's fmaxf(NaN, 0) = 0 then silently zeroes the valid
-// patch's border pixel.
-__device__ __forceinline__ void frag_left(float v0, float v1, int lane, float& l0, float& l1) {
-    const float s0 = __shfl_sync(0xffffffffu, v0, (lane + 28) & 31), s1 = __shfl_sync(0xffffffffu, v1, (lane + 28) & 31);
-    l0 = s0;
-    l1 = lane < 4 ? s0 : s1;
-}
-__device__ __forceinline__ void frag_right(float v0, float v1, int lane, float& r0, float& r1) {
-    const float t0 = __shfl_sync(0xffffffffu, v0, (lane + 4) & 31), t1 = __shfl_sync(0xffffffffu, v1, (lane + 4) & 31);
-    r0 = lane >= 28 ? t1 : t0;
-    r1 = t1;
-}
+// Neighbours along x of an accumulator fragment in the neighbour-paired order: a thread holds rows i = lane/4 (h = 0, an even pixel)
+// and i + 8 (h = 1, the odd pixel to its right) of its warp's 16 rows.  The even pixel's right neighbour and the odd pixel's left one
+// are the thread's own other value; the even pixel's left neighbour is the odd pixel of row i - 1 (lane - 4, its h = 1 value) and the
+// odd pixel's right neighbour the even pixel of row i + 1 (lane + 4, its h = 0 value).
+// A neighbour outside the image row is garbage that callers must drop by a select, never by multiplying with 0: in the pair layouts it
+// is the other patch of the unit, whose input rows are stale workspace when that patch is skipped (beyond a count, or the tail of an
+// odd n).  NaN * 0 = NaN, and the ReLU's fmaxf(NaN, 0) = 0 then silently zeroes the valid patch's border pixel.
+__device__ __forceinline__ float frag_left_even(float v1, int lane) { return __shfl_sync(0xffffffffu, v1, (lane + 28) & 31); }
+__device__ __forceinline__ float frag_right_odd(float v0, int lane) { return __shfl_sync(0xffffffffu, v0, (lane + 4) & 31); }
 
 __device__ __forceinline__ bool xpatch_valid(const XArgs& a, int pi) { return pi < a.n && (a.count == nullptr || (pi % a.group) < a.count[pi / a.group]); }
 
@@ -309,17 +314,17 @@ __device__ __forceinline__ void xconv_block_epilogue(const float* d, const XArgs
     using In = typename Cfg::In;
     constexpr int NT = Cfg::NT, HOUT = Cfg::HOUT, W = In::W, PAIR = In::PAIR, COUT = Cfg::CO, OUT = Cfg::OUTL, OSA = Cfg::SPLIT_O;
     unsigned char* obase[2];
-    bool has_l[2], has_r[2];      // the left / right neighbour lies inside the image row (else: zero padding)
     bool ok[2];
     size_t lo_off = 0;
+    // row group position i = lane/4: pixel x = 2i + h (PAIR: x = 2 (i % 4) + h of patch 2u + i / 4); only the even pixel's left
+    // neighbour (x = 0) and the odd pixel's right neighbour (x = W - 1) can fall outside the image row (else: zero padding)
+    const int i = lane >> 2, xi = PAIR ? (i & 3) : i;
+    const bool has_l0 = xi > 0, has_r1 = xi < W / 2 - 1;
+    static_assert(W == 16 || PAIR, "neighbour-paired row groups: 16 pixels, or 8 of each patch of a pair");
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-        const int r = b * 64 + wq * 16 + (lane >> 2) + 8 * h;
-        int y, x, pi;
-        if (PAIR) { y = r >> 4; x = r & 7; pi = 2 * u + ((r >> 3) & 1); }
-        else { y = r / W; x = r - y * W; pi = u; }
+        const int y = b * 4 + wq, x = 2 * xi + h, pi = PAIR ? 2 * u + (i >> 2) : u;   // a warp's 16 rows are image row y
         ok[h] = xpatch_valid(a, pi);
-        has_l[h] = x > 0; has_r[h] = x < W - 1;
         if (OUT == L_HEAD) {
             obase[h] = reinterpret_cast<unsigned char*>(a.out) + (((size_t)(pi >> 7) * (HOUT * HOUT * COUT / 8) + (size_t)(y * HOUT + x) * (COUT / 8)) * 128 + (pi & 127)) * 16;
             lo_off = (size_t)((a.n + 127) >> 7) * (HOUT * HOUT * COUT / 8) * 128 * 16;
@@ -339,21 +344,20 @@ __device__ __forceinline__ void xconv_block_epilogue(const float* d, const XArgs
             const float c00 = d[4 * j + e], c01 = d[4 * j + 2 + e];                                   // block 0, rows h = 0 / 1
             const float c10 = d[4 * (j + NT / 8) + e], c11 = d[4 * (j + NT / 8) + 2 + e];             // block 1
             const float c20 = d[4 * (j + 2 * NT / 8) + e], c21 = d[4 * (j + 2 * NT / 8) + 2 + e];     // block 2
-            float l0, l1;
-            frag_left(c00, c01, lane, l0, l1);
+            // left neighbours: even pixel from lane - 4, odd pixel c00 (stride 2: both in the odd-x plane, x - 1)
+            const float l0 = frag_left_even(c01, lane);
             // zero padding by selects: the same roundings as adding the neighbour (fmaf(l, 1, t) == l + t), and a NaN of a
-            // skipped pair partner stays out of the valid patch
+            // skipped pair partner stays out of the valid patch.  Every pixel: l + (r + centre)
             float acc0, acc1;
             if (Cfg::STRD == 1) {
-                float r0, r1;
-                frag_right(c20, c21, lane, r0, r1);
-                const float t0 = has_r[0] ? r0 + c10 : c10, t1 = has_r[1] ? r1 + c11 : c11;
-                acc0 = has_l[0] ? l0 + t0 : t0;
-                acc1 = has_l[1] ? l1 + t1 : t1;
+                const float r1 = frag_right_odd(c20, lane);     // right neighbours: even pixel c21, odd pixel from lane + 4
+                const float t0 = c21 + c10, t1 = has_r1 ? r1 + c11 : c11;
+                acc0 = has_l0 ? l0 + t0 : t0;
+                acc1 = c00 + t1;
             } else {
                 const float t0 = c10 + c20, t1 = c11 + c21;
-                acc0 = has_l[0] ? l0 + t0 : t0;
-                acc1 = has_l[1] ? l1 + t1 : t1;
+                acc0 = has_l0 ? l0 + t0 : t0;
+                acc1 = c00 + t1;
             }
             v[0][e] = fmaxf(fmaf(acc0, a.inv_scale, s_bias[c + e]), 0.f);
             v[1][e] = fmaxf(fmaf(acc1, a.inv_scale, s_bias[c + e]), 0.f);

@@ -4,7 +4,8 @@
 //   sampler (LAF.py:313-372) -> input_norm (architectures.py:231-235) -> conv3x3(1 -> C1)+BN+ReLU -> conv3x3(C1 -> COUT)+BN+ReLU
 //
 // 32x32 patches and the layer-1 activations never exist in HBM.  M = 64 blocks are 64 consecutive pixels = 2 image rows of 32 (16
-// blocks per patch, no padded columns).  Layer 1 (K = 9): the sliding-window plane P[y*32 + x] = {4 pixels of padded row y from
+// blocks per patch, no padded columns; each half row of 16 pixels in the neighbour-paired order of tcx_conv.cuh, even x first, which
+// the P planes set and every later stage keeps).  Layer 1 (K = 9): the sliding-window plane P[y*32 + x] = {4 pixels of padded row y from
 // column x | 4 pixels of padded row y+1} makes one K = 16 MMA cover kernel rows 0 and 1, the same plane two rows further (descriptor
 // leading-byte offset) kernel row 2.  Layer 2: for kernel row dy one MMA over the layer-1 stage advanced by dy rows with the three
 // taps of that row stacked along N (N = 3*COUT); the epilogue shifts the dx = 0 / dx = 2 blocks by one pixel with warp shuffles, and
@@ -47,6 +48,13 @@ __device__ unsigned long long g_first_tl[TL_LAUNCHES][TL_CTAS][16][TL_STATES];
 __device__ int g_first_tl_launch[TL_CTAS];
 #endif
 
+// Four 8x8 16-bit matrices to shared memory in one instruction.  r0 .. r3: the thread's packed accumulator-fragment word of each
+// (row lane/4, columns 2 (lane%4) and + 1); row: the 16-byte address of row lane%8 of matrix lane/8 that this lane supplies.
+__device__ __forceinline__ void stmatrix_x4(const void* row, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(smem_u32(row)), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
+
 template <int C1, int COUT, int SA, int SW, int OSA, int L3 = 0>
 struct XFirstCfg {
     using X3 = XCfg<COUT, 2 * COUT, 32, 2, 1, 1, L_S1_16, 1, 1, 1>;   // layer 3 (L3 = 1): its input planes as ONE stage in shared memory
@@ -80,6 +88,7 @@ struct XFirstCfg {
     static_assert(SA <= 1 && SW <= 1 && OSA <= 1, "split-precision switches are 0 | 1");
     static_assert(!L3 || (OSA == 1 && X3::NT <= 32), "layer 3 reads hi + lo planes; its bias fits smem[640, 768)");
     static_assert(C1 == 16 || C1 == 32, "layer-1 accumulator width");
+    static_assert(SA || KC % 2 == 0, "layer-1 epilogue: one stmatrix.x4 per channel group (hi + lo) or per two (hi only)");
     static_assert(SMEM <= 232448, "shared memory budget");
 };
 
@@ -177,23 +186,30 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
             wgmma_commit();
         };
         // its epilogue, once the MMAs have completed: bias / ReLU -> fp16 (hi [+lo]) into stage st of layer 2
+        // (M row = stage slot: the P planes are built in the stage's neighbour-paired order)
         auto l1_epilogue = [&](float* d1, unsigned char* st, int b) {
             wgmma_reg_fence<Cfg::ACC1 / 2>(d1);
+            uint32_t hi[KC][2], lo[KC][2];
 #pragma unroll
             for (int h = 0; h < 2; h++) {
-                const int slot = b * 64 + wq * 16 + (lane >> 2) + 8 * h + 32;      // pixel m sits one (zero) row into the stage
 #pragma unroll
-                for (int j = 0; j < C1 / 8; j++) {
+                for (int j = 0; j < KC; j++) {
                     const int c = j * 8 + 2 * (lane & 3);
                     float v0 = d1[4 * j + 2 * h], v1 = d1[4 * j + 2 * h + 1];
                     if (Cfg::S1) { v0 += d1[4 * (j + 2) + 2 * h]; v1 += d1[4 * (j + 2) + 2 * h + 1]; }   // [x*w_hi | x_hi*w_lo] side by side
                     v0 = fmaxf(fmaf(v0, src.w1_inv, s_bias1[c]), 0.f);
                     v1 = fmaxf(fmaf(v1, src.w1_inv, s_bias1[c + 1]), 0.f);
-                    uint32_t hi, lo;
-                    split_pack2<SA, BF>(v0, v1, hi, lo);
-                    *reinterpret_cast<uint32_t*>(st + ((size_t)j * GS + slot) * 16 + (c & 7) * 2) = hi;
-                    if (SA) *reinterpret_cast<uint32_t*>(st + ((size_t)(KC + j) * GS + slot) * 16 + (c & 7) * 2) = lo;
+                    split_pack2<SA, BF>(v0, v1, hi[j][h], lo[j][h]);
                 }
+            }
+            // matrix mx = lane / 8: rows h = mx % 2 of channel group j (SA: of the hi plane for mx < 2, else the lo plane; without
+            // SA: of group j + mx / 2)
+            const int mx = lane >> 3;
+            const int slot = b * 64 + wq * 16 + (lane & 7) + 8 * (mx & 1) + 32;     // pixel m sits one (zero) row into the stage
+#pragma unroll
+            for (int j = 0; j < KC; j += SA ? 1 : 2) {
+                if constexpr (SA) stmatrix_x4(st + ((size_t)((mx >> 1) * KC + j) * GS + slot) * 16, hi[j][0], hi[j][1], lo[j][0], lo[j][1]);
+                else stmatrix_x4(st + ((size_t)(j + (mx >> 1)) * GS + slot) * 16, hi[j][0], hi[j][1], hi[j + 1][0], hi[j + 1][1]);
             }
         };
         // block k = 0 .. 7 of this warpgroup's layer-1 blocks: half plane k / 4, block 8 (k / 4) + wg + 2 (k % 4)
@@ -251,8 +267,9 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
             // epilogue of block b, the warpgroup's nb-th layer-2 block, once its MMAs have completed
             auto l2_epilogue = [&](float* d, int b, int nb) {
                 wgmma_reg_fence<ACCW / 2>(d);
-                // rows r = 16 wq + lane/4 + 8 h of the block: pixel m = 64 b + r, y = m / 32, x = m % 32.  Warps 2k and 2k+1 share an image
-                // row: the last row of an even warp and the first of the odd one exchange their dx = 0 / dx = 2 values through shared memory.
+                // rows r = 16 wq + lane/4 + 8 h of the block: image row y = (64 b + 16 wq) / 32, x = 16 (wq % 2) + 2 (lane/4) + h
+                // (neighbour-paired half rows).  Warps 2k and 2k+1 share an image row: x = 15 (lanes 28-31, h = 1, of the even warp) and
+                // x = 16 (lanes 0-3, h = 0, of the odd one) exchange their dx = 0 / dx = 2 values through shared memory.
                 // The exchange is double-buffered by block parity and a warpgroup runs its epilogues one at a time in block order (the
                 // second block in flight is in MMAs, not in an epilogue): a warp rewrites a buffer only after every warp of the warpgroup
                 // has passed the barrier of the following block, so after it read the buffer.
@@ -273,9 +290,22 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
                 }
                 AG_TL(TL_WG_BAR, bar_sync(3 + wg, 128));
                 const int y0 = (b * 64 + wq * 16) >> 5;
-                const int x0 = (wq & 1) * 16 + (lane >> 2);             // h = 0; h = 1 is x0 + 8
-                const float ml0 = x0 > 0 ? 1.f : 0.f, mr1 = x0 + 8 < 31 ? 1.f : 0.f;
+                const int x0 = (wq & 1) * 16 + 2 * (lane >> 2);         // h = 0 (even pixel); h = 1 is x0 + 1
+                // Each pixel keeps the rounding it had when row i + 8 h of a warp was pixel 16 (wq % 2) + i + 8 h: the first 8 pixels
+                // of a half row (lanes 0-15 now) l + (r + c), with the left neighbour masked at x = 0, the last 8 (lanes 16-31)
+                // r + (l + c), with the right one masked at x = 31.  sum = fmaf(outer, mask, inner + c).
+                const bool first8 = lane < 16;
+                const float m0 = (first8 && x0 == 0) ? 0.f : 1.f, m1 = (!first8 && x0 + 1 == 31) ? 0.f : 1.f;
                 const bool from_prev = (wq & 1) && lane < 4, from_next = !(wq & 1) && lane >= 28;
+                // L3: the shared-memory row of the layer-3 planes that this lane supplies to stmatrix: row lane % 8 of matrix
+                // mx = lane / 8 = rows h = mx % 2 of the hi (mx < 2) or lo plane
+                size_t s3 = 0;
+                if (L3) {
+                    using In3 = typename X3::In;
+                    const int mx = lane >> 3;
+                    const int slot = layout_slot(L_S2_16, y0, (wq & 1) * 16 + 2 * (lane & 7) + (mx & 1), 0);
+                    s3 = (size_t)(mx >> 1) * X3::KC * X3::GS + (size_t)(slot / In3::DATA) * In3::PLANE + In3::RW + slot % In3::DATA;
+                }
 #pragma unroll
                 for (int j = 0; j < NT / 8; j++) {
                     const int c = j * 8 + 2 * (lane & 3);
@@ -285,31 +315,30 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
                         const float c00 = d[4 * j + e], c01 = d[4 * j + 2 + e];
                         const float c10 = d[4 * (j + NT / 8) + e], c11 = d[4 * (j + NT / 8) + 2 + e];
                         const float c20 = d[4 * (j + 2 * NT / 8) + e], c21 = d[4 * (j + 2 * NT / 8) + 2 + e];
-                        float l0, l1, r0, r1;
-                        frag_left(c00, c01, lane, l0, l1);
-                        frag_right(c20, c21, lane, r0, r1);
+                        // neighbours (tcx_conv.cuh, frag_left_even): x0 - 1 from lane - 4, x0 + 2 from lane + 4, or across the two
+                        // warps of the image row through shared memory
+                        float l0 = frag_left_even(c01, lane), r1 = frag_right_odd(c20, lane);
+                        const float l1 = c00, r0 = c21;
                         if (from_prev) l0 = xw[((wq - 1) * 2 + 0) * NT + c + e];
                         if (from_next) r1 = xw[((wq + 1) * 2 + 1) * NT + c + e];
-                        // 0/1 masks: zero padding outside the row (x = 0 for h = 0 of even warps' first lanes, x = 31 for h = 1 of odd warps' last lanes)
-                        const float acc0 = fmaf(l0, ml0, r0 + c10);
-                        const float acc1 = fmaf(r1, mr1, l1 + c11);
+                        // 0/1 masks: zero padding outside the row (x = 0: h = 0 of even warps' lanes 0-3, x = 31: h = 1 of odd warps' lanes 28-31)
+                        const float acc0 = fmaf(first8 ? l0 : r0, m0, (first8 ? r0 : l0) + c10);
+                        const float acc1 = fmaf(first8 ? l1 : r1, m1, (first8 ? r1 : l1) + c11);
                         v[0][e] = fmaxf(fmaf(acc0, a.inv_scale, s_bias[c + e]), 0.f);
                         v[1][e] = fmaxf(fmaf(acc1, a.inv_scale, s_bias[c + e]), 0.f);
                     }
+                    uint32_t hi[2], lo[2];
 #pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        const int slot = layout_slot(L_S2_16, y0, x0 + 8 * h, 0);
-                        uint32_t hi, lo;
-                        split_pack2<OSA, BF>(v[h][0], v[h][1], hi, lo);
-                        if (L3) {   // plane slot -> the same slot behind the plane's zero row in shared memory
-                            using In3 = typename X3::In;
-                            const size_t s3 = (size_t)(slot / In3::DATA) * In3::PLANE + In3::RW + slot % In3::DATA;
-                            *reinterpret_cast<uint32_t*>(sIn3 + ((size_t)(c / 8) * X3::GS + s3) * 16 + (c & 7) * 2) = hi;
-                            *reinterpret_cast<uint32_t*>(sIn3 + ((size_t)(X3::KC + c / 8) * X3::GS + s3) * 16 + (c & 7) * 2) = lo;
-                        } else {
+                    for (int h = 0; h < 2; h++) split_pack2<OSA, BF>(v[h][0], v[h][1], hi[h], lo[h]);
+                    if (L3) {   // rows h = 0 / 1 lie in the even-x / odd-x parity plane
+                        stmatrix_x4(sIn3 + ((size_t)j * X3::GS + s3) * 16, hi[0], hi[1], lo[0], lo[1]);
+                    } else {
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            const int slot = layout_slot(L_S2_16, y0, x0 + h, 0);
                             const size_t goff = (size_t)(c / 8) * 1024 * 16;
-                            *reinterpret_cast<uint32_t*>(outp + goff + (size_t)slot * 16 + (c & 7) * 2) = hi;
-                            if (OSA) *reinterpret_cast<uint32_t*>(outp + (size_t)(COUT / 8) * 1024 * 16 + goff + (size_t)slot * 16 + (c & 7) * 2) = lo;
+                            *reinterpret_cast<uint32_t*>(outp + goff + (size_t)slot * 16 + (c & 7) * 2) = hi[h];
+                            if (OSA) *reinterpret_cast<uint32_t*>(outp + (size_t)(COUT / 8) * 1024 * 16 + goff + (size_t)slot * 16 + (c & 7) * 2) = lo[h];
                         }
                     }
                 }
@@ -412,11 +441,12 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
                 const long long tb = clock64();
 #endif
                 unsigned char* ph = sP + (size_t)hh * 2 * NPIXP * 16;
-                // one 16-byte window per thread and step: consecutive lanes read consecutive pixels and write consecutive slots (no bank
-                // conflicts; the shared-memory pipe is this kernel's busiest unit)
+                // one 16-byte window per thread and step: slot s0 holds the window of the pixel that M row s0 stands for (each half row
+                // of 16 in the neighbour-paired order, tcx_conv.cuh), so a warp reads the 32 pixels of one row and writes consecutive
+                // slots (no bank conflicts; the shared-memory pipe is this kernel's busiest unit)
 #pragma unroll 1
                 for (int s0 = pt; s0 < NPIXP; s0 += 256) {
-                    const float* rowp = sx + (hh * 16 + (s0 >> 5)) * 34 + (s0 & 31);
+                    const float* rowp = sx + (hh * 16 + (s0 >> 5)) * 34 + (s0 & 16) + 2 * (s0 & 7) + ((s0 >> 3) & 1);   // x with rpos(x & 15) = s0 & 15
                     float xv[8];
 #pragma unroll
                     for (int e = 0; e < 4; e++) { xv[e] = rowp[e]; xv[4 + e] = rowp[34 + e]; }
