@@ -1,0 +1,509 @@
+// Geometric verification of the batched matcher's tentatives (after ag_match_pairs), one CTA per pair:
+//   ag_homography_ransac         homography RANSAC (the notebook's ransac_validate: findHomography(src, dst, 2.0, 0.99, 50000))
+//   ag_gt_correspondences_pairs  ReprojectionStuff.get_GT_correspondence_indexes (the reference's "true matches" count), per pair
+//
+// RANSAC is deterministic and restated line by line in numpy by tests/oracle_ransac.py, so its decisions (samples, degeneracy, inlier
+// counts, the stopping point) are reproduced exactly.  For that reason all its arithmetic is fp64 and this file is compiled with
+// -fmad=false (build.sh): numpy rounds every product and sum separately, so fused multiply-adds here would move near-threshold decisions.
+// The block reductions of the refit run in a fixed order (strided per-thread sums, an xor butterfly per warp, warps in ascending order)
+// that the restatement repeats.
+#include "common.cuh"
+
+namespace ag {
+
+constexpr int VT = 256;              // threads per CTA = hypotheses per chunk: the stopping rule is checked after each chunk
+constexpr int VTILE = 2048;          // tentative centres per shared-memory tile (32 KB)
+constexpr int MAX_DRAWS = 64;        // draws per hypothesis before it is counted as degenerate (fewer than 4 distinct indices)
+constexpr double COLLINEAR_EPS = 1e-6;   // |cross(b - a, c - a)| <= eps * (|dx1| + |dy1|) * (|dx2| + |dy2|): collinear
+constexpr int JACOBI_SWEEPS = 10;
+constexpr int REFIT_ROUNDS = 3;
+constexpr int MAX_TCAP = 4194240;    // ag_match_pairs' cap1 limit
+
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
+    uint64_t z = x + 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+// Index of draw d of hypothesis h in [0, n): splitmix64(splitmix64((h << 32) | d) ^ seed), high 32 bits scaled by n.
+__device__ __forceinline__ int draw_index(uint64_t seed, int h, int d, int n) {
+    const uint64_t r = splitmix64(splitmix64(((uint64_t)(uint32_t)h << 32) | (uint32_t)d) ^ seed);
+    return (int)(((r >> 32) * (uint64_t)(uint32_t)n) >> 32);
+}
+
+// Pair p = (i, j) -> n tentatives, or -1 when the pair cannot be verified (an image index out of range, ntent outside 0..tcap).
+__device__ __forceinline__ int pair_tentatives(const int* __restrict__ pairs, int p, int S1, int S2, const int* __restrict__ ntent, int tcap,
+                                               int& i, int& j) {
+    i = pairs ? pairs[2 * (size_t)p] : p;
+    j = pairs ? pairs[2 * (size_t)p + 1] : p;
+    const int n = ntent[p];
+    if (i < 0 || i >= S1 || j < 0 || j >= S2 || n < 0 || n > tcap) return -1;
+    return n;
+}
+
+// Block-wide: true when every tentative row of the pair indexes a row inside its set's cap (nothing is read otherwise).
+__device__ bool rows_in_range(const int* __restrict__ tent, int n, int cap1, int cap2) {
+    bool bad = false;
+    for (int t = threadIdx.x; t < n; t += VT) {
+        const int r1 = tent[2 * (size_t)t], r2 = tent[2 * (size_t)t + 1];
+        bad |= r1 < 0 || r1 >= cap1 || r2 < 0 || r2 >= cap2;
+    }
+    return !__syncthreads_or(bad);
+}
+
+// Centres of tentative t: (x1, y1) in image 1, (x2, y2) in image 2 (the LAF's third column).
+__device__ __forceinline__ float4 tent_centres(const float* __restrict__ L1, const float* __restrict__ L2, const int* __restrict__ tent, int t) {
+    const float* a = L1 + (size_t)tent[2 * (size_t)t] * 6;
+    const float* b = L2 + (size_t)tent[2 * (size_t)t + 1] * 6;
+    return make_float4(a[2], a[5], b[2], b[5]);
+}
+
+// ---- fp64 3x3 helpers (row-major), in the restatement's operation order ------------------------------------------------------------
+__device__ __forceinline__ void adj3(const double* m, double* o) {
+    o[0] = m[4] * m[8] - m[5] * m[7]; o[1] = m[2] * m[7] - m[1] * m[8]; o[2] = m[1] * m[5] - m[2] * m[4];
+    o[3] = m[5] * m[6] - m[3] * m[8]; o[4] = m[0] * m[8] - m[2] * m[6]; o[5] = m[2] * m[3] - m[0] * m[5];
+    o[6] = m[3] * m[7] - m[4] * m[6]; o[7] = m[1] * m[6] - m[0] * m[7]; o[8] = m[0] * m[4] - m[1] * m[3];
+}
+__device__ __forceinline__ void mul3(const double* a, const double* b, double* o) {
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+#pragma unroll
+        for (int c = 0; c < 3; c++) o[3 * r + c] = a[3 * r] * b[c] + a[3 * r + 1] * b[3 + c] + a[3 * r + 2] * b[6 + c];
+}
+// H /= H[2][2]; false when that is zero or the result is not finite.
+__device__ __forceinline__ bool normalise_h(double* H) {
+    const double s = H[8];
+    bool ok = s != 0.0;
+#pragma unroll
+    for (int k = 0; k < 9; k++) {
+        H[k] = H[k] / s;
+        ok &= isfinite(H[k]);
+    }
+    return ok;
+}
+
+// Inlier test: positive denominator and squared forward error <= th2.
+__device__ __forceinline__ bool is_inlier(const double* H, float4 c, double th2) {
+    const double x = c.x, y = c.y;
+    const double w = H[6] * x + H[7] * y + H[8];
+    if (!(w > 0.0)) return false;
+    const double u = (H[0] * x + H[1] * y + H[2]) / w - (double)c.z;
+    const double v = (H[3] * x + H[4] * y + H[5]) / w - (double)c.w;
+    return u * u + v * v <= th2;
+}
+
+__device__ __forceinline__ double cross3(double ax, double ay, double bx, double by, double cx, double cy, bool& collinear) {
+    const double dx1 = bx - ax, dy1 = by - ay, dx2 = cx - ax, dy2 = cy - ay;
+    const double cr = dx1 * dy2 - dx2 * dy1;
+    collinear |= fabs(cr) <= COLLINEAR_EPS * ((fabs(dx1) + fabs(dy1)) * (fabs(dx2) + fabs(dy2)));
+    return cr;
+}
+
+// Basis map of 4 points: M = [p0 p1 p2] diag(adj([p0 p1 p2]) p3), p = (x, y, 1).
+__device__ __forceinline__ void basis_map(const double* x, const double* y, double* M) {
+    const double P[9] = {x[0], x[1], x[2], y[0], y[1], y[2], 1.0, 1.0, 1.0};
+    double A[9];
+    adj3(P, A);
+    double l[3];
+#pragma unroll
+    for (int r = 0; r < 3; r++) l[r] = A[3 * r] * x[3] + A[3 * r + 1] * y[3] + A[3 * r + 2];
+#pragma unroll
+    for (int r = 0; r < 3; r++)
+#pragma unroll
+        for (int c = 0; c < 3; c++) M[3 * r + c] = P[3 * r + c] * l[c];
+}
+
+// Hypothesis from 4 correspondences; false for a degenerate sample (collinear triplet in either image, a mixed orientation of the four
+// triplets between the images, or H[2][2] zero / non-finite).
+__device__ bool minimal_homography(const float4 (&c)[4], double* H) {
+    double x1[4], y1[4], x2[4], y2[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) { x1[k] = c[k].x; y1[k] = c[k].y; x2[k] = c[k].z; y2[k] = c[k].w; }
+    constexpr int tt[4][3] = {{0, 1, 2}, {1, 2, 3}, {0, 2, 3}, {0, 1, 3}};
+    bool col = false;
+    int neg = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const int a = tt[k][0], b = tt[k][1], d = tt[k][2];
+        const double c1 = cross3(x1[a], y1[a], x1[b], y1[b], x1[d], y1[d], col);
+        const double c2 = cross3(x2[a], y2[a], x2[b], y2[b], x2[d], y2[d], col);
+        neg += (c1 * c2 < 0.0) ? 1 : 0;
+    }
+    if (col || (neg != 0 && neg != 4)) return false;
+    double M1[9], M2[9], A1[9];
+    basis_map(x1, y1, M1);
+    basis_map(x2, y2, M2);
+    adj3(M1, A1);
+    mul3(M2, A1, H);
+    return normalise_h(H);
+}
+
+// Sum of K doubles over the block in the fixed order described at the top, into out[0..K) (shared), valid for every thread on return.
+template <int K>
+__device__ __forceinline__ void block_sum(double (&v)[K], double (*red)[K], double* out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] = v[k] + __shfl_xor_sync(0xffffffffu, v[k], o);
+    }
+    if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < K; k++) red[warp][k] = v[k];
+    __syncthreads();
+    if (threadIdx.x < K) {
+        double s = red[0][threadIdx.x];
+        for (int w = 1; w < VT / 32; w++) s = s + red[w][threadIdx.x];
+        out[threadIdx.x] = s;
+    }
+    __syncthreads();
+}
+
+struct RansacShared {
+    float4 tile[VTILE];
+    double H[9], Hr[9];
+    double red[VT / 32][45];
+    double sums[45];
+    double A[81], V[81];
+    unsigned long long key[VT / 32];
+    int count[VT / 32];
+    int bad;
+};
+
+// Inliers of H over all n tentatives (thread t handles rows t, t + VT, ...); writes the mask when `inl` is not NULL.  Block total.
+__device__ int score_rows(const double* H, const float* L1, const float* L2, const int* tent, int n, double th2, unsigned char* inl,
+                          RansacShared& s) {
+    int cnt = 0;
+    for (int t = threadIdx.x; t < n; t += VT) {
+        const bool in = is_inlier(H, tent_centres(L1, L2, tent, t), th2);
+        cnt += in;
+        if (inl) inl[t] = in;
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if (lane == 0) s.count[warp] = cnt;
+    __syncthreads();
+    int tot = 0;
+#pragma unroll
+    for (int w = 0; w < VT / 32; w++) tot += s.count[w];
+    __syncthreads();
+    return tot;
+}
+
+// Normalised-DLT least squares on the rows of the mask `inl` (Hartley normalisation, 9x9 normal matrix, smallest eigenvector by
+// cyclic Jacobi on warp 0).  Writes s.Hr; false when the inliers do not determine a finite homography.
+__device__ bool refit(const float* L1, const float* L2, const int* tent, int n, const unsigned char* inl, int cnt, RansacShared& s) {
+    // centroids and mean squared radii of both point sets
+    double st[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    for (int t = threadIdx.x; t < n; t += VT) {
+        const float4 c = tent_centres(L1, L2, tent, t);
+        const bool in = inl[t];
+        const double x1 = in ? (double)c.x : 0.0, y1 = in ? (double)c.y : 0.0, x2 = in ? (double)c.z : 0.0, y2 = in ? (double)c.w : 0.0;
+        st[0] = st[0] + x1; st[1] = st[1] + y1; st[2] = st[2] + x1 * x1; st[3] = st[3] + y1 * y1;
+        st[4] = st[4] + x2; st[5] = st[5] + y2; st[6] = st[6] + x2 * x2; st[7] = st[7] + y2 * y2;
+    }
+    block_sum<8>(st, reinterpret_cast<double(*)[8]>(&s.red[0][0]), s.sums);
+    const double nd = (double)cnt;
+    const double c1x = s.sums[0] / nd, c1y = s.sums[1] / nd, c2x = s.sums[4] / nd, c2y = s.sums[5] / nd;
+    const double var1 = (s.sums[2] + s.sums[3]) / nd - (c1x * c1x + c1y * c1y);
+    const double var2 = (s.sums[6] + s.sums[7]) / nd - (c2x * c2x + c2y * c2y);
+    if (!(var1 > 0.0) || !(var2 > 0.0)) return false;   // uniform across the block: every thread returns
+    const double s1 = sqrt(2.0 / var1), s2 = sqrt(2.0 / var2);
+    // normal matrix: upper triangle, row by row
+    double nm[45];
+#pragma unroll
+    for (int k = 0; k < 45; k++) nm[k] = 0.0;
+    for (int t = threadIdx.x; t < n; t += VT) {
+        const float4 c = tent_centres(L1, L2, tent, t);
+        const bool in = inl[t];
+        const double u = (c.x - c1x) * s1, v = (c.y - c1y) * s1, up = (c.z - c2x) * s2, vp = (c.w - c2y) * s2;
+        const double a1[9] = {-u, -v, -1.0, 0.0, 0.0, 0.0, up * u, up * v, up};
+        const double a2[9] = {0.0, 0.0, 0.0, -u, -v, -1.0, vp * u, vp * v, vp};
+        int e = 0;
+#pragma unroll
+        for (int k = 0; k < 9; k++)
+#pragma unroll
+            for (int l = k; l < 9; l++, e++) nm[e] = nm[e] + (in ? a1[k] * a1[l] + a2[k] * a2[l] : 0.0);
+    }
+    block_sum<45>(nm, s.red, s.sums);
+    if (threadIdx.x < 81) {
+        const int r = threadIdx.x / 9, c = threadIdx.x % 9, lo = min(r, c), hi = max(r, c);
+        s.A[threadIdx.x] = s.sums[lo * 9 - lo * (lo - 1) / 2 + (hi - lo)];
+        s.V[threadIdx.x] = r == c ? 1.0 : 0.0;
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const int k = threadIdx.x;
+        for (int sweep = 0; sweep < JACOBI_SWEEPS; sweep++)
+            for (int p = 0; p < 8; p++)
+                for (int q = p + 1; q < 9; q++) {
+                    const double apq = s.A[9 * p + q], app = s.A[9 * p + p], aqq = s.A[9 * q + q];
+                    __syncwarp();
+                    if (apq == 0.0) continue;
+                    const double theta = (aqq - app) / (2.0 * apq);
+                    const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+                    const double cs = 1.0 / sqrt(t * t + 1.0), sn = t * cs;
+                    if (k < 9) {
+                        const double akp = s.A[9 * k + p], akq = s.A[9 * k + q];
+                        s.A[9 * k + p] = cs * akp - sn * akq;
+                        s.A[9 * k + q] = sn * akp + cs * akq;
+                    }
+                    __syncwarp();
+                    if (k < 9) {
+                        const double apk = s.A[9 * p + k], aqk = s.A[9 * q + k];
+                        s.A[9 * p + k] = cs * apk - sn * aqk;
+                        s.A[9 * q + k] = sn * apk + cs * aqk;
+                        const double vkp = s.V[9 * k + p], vkq = s.V[9 * k + q];
+                        s.V[9 * k + p] = cs * vkp - sn * vkq;
+                        s.V[9 * k + q] = sn * vkp + cs * vkq;
+                    }
+                    __syncwarp();
+                }
+        if (k == 0) {
+            int m = 0;
+            for (int e = 1; e < 9; e++)
+                if (s.A[9 * e + e] < s.A[9 * m + m]) m = e;
+            double Hn[9], tmp[9];
+            for (int e = 0; e < 9; e++) Hn[e] = s.V[9 * e + m];
+            const double T1[9] = {s1, 0.0, -(s1 * c1x), 0.0, s1, -(s1 * c1y), 0.0, 0.0, 1.0};
+            const double T2i[9] = {1.0 / s2, 0.0, c2x, 0.0, 1.0 / s2, c2y, 0.0, 0.0, 1.0};
+            mul3(T2i, Hn, tmp);
+            mul3(tmp, T1, s.Hr);
+            s.bad = !normalise_h(s.Hr);
+        }
+    }
+    __syncthreads();
+    return !s.bad;
+}
+
+__global__ void __launch_bounds__(VT) ransac_kernel(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2, int S2,
+                                                    int cap2, const int* __restrict__ pairs, const int* __restrict__ tent_all,
+                                                    const int* __restrict__ ntent, int tcap, double th2, double log1mconf, int max_iters,
+                                                    uint64_t seed, float* __restrict__ Hout, unsigned char* __restrict__ inl_all,
+                                                    int* __restrict__ ninl, int* __restrict__ iters) {
+    __shared__ RansacShared s;
+    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int i, j;
+    const int n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
+    const int* tent = tent_all + (size_t)p * tcap * 2;
+    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
+        if (tid == 0) ninl[p] = -1;
+        return;
+    }
+    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
+    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
+    unsigned char* inl = inl_all + (size_t)p * tcap;
+    int best = 0, h_done = 0;
+    if (n >= 4) {
+        const int ntiles = (n + VTILE - 1) / VTILE;
+        for (int h0 = 0;; h0 += VT) {
+            const int h = h0 + tid;
+            double H[9];
+            bool ok = h < max_iters;
+            if (ok) {
+                int idx[4], got = 0;
+                for (int d = 0; d < MAX_DRAWS && got < 4; d++) {
+                    const int v = draw_index(seed, h, d, n);
+                    bool dup = false;
+                    for (int q = 0; q < got; q++) dup |= idx[q] == v;
+                    if (!dup) idx[got++] = v;
+                }
+                ok = got == 4;
+                if (ok) {
+                    float4 c[4];
+#pragma unroll
+                    for (int q = 0; q < 4; q++) c[q] = tent_centres(L1, L2, tent, idx[q]);
+                    ok = minimal_homography(c, H);
+                }
+            }
+            int cnt = 0;
+            for (int tb = 0; tb < ntiles; tb++) {
+                const int t0 = tb * VTILE, m = min(VTILE, n - t0);
+                if (ntiles > 1 || h0 == 0) {
+                    __syncthreads();
+                    for (int t = tid; t < m; t += VT) s.tile[t] = tent_centres(L1, L2, tent, t0 + t);
+                    __syncthreads();
+                }
+                if (ok)
+                    for (int t = 0; t < m; t++) cnt += is_inlier(H, s.tile[t], th2);
+            }
+            // best of the chunk: highest count, then lowest h
+            const unsigned long long mine = ok ? ((unsigned long long)cnt << 32) | (unsigned)~(unsigned)h : 0ull;
+            unsigned long long key = mine;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const unsigned long long ok2 = __shfl_xor_sync(0xffffffffu, key, o);
+                key = ok2 > key ? ok2 : key;
+            }
+            if (lane == 0) s.key[warp] = key;
+            __syncthreads();
+            unsigned long long bk = 0;
+#pragma unroll
+            for (int w = 0; w < VT / 32; w++) bk = s.key[w] > bk ? s.key[w] : bk;
+            const int bc = (int)(bk >> 32);
+            if (bk != 0 && bc > best) {
+                if (mine == bk) {
+#pragma unroll
+                    for (int k = 0; k < 9; k++) s.H[k] = H[k];
+                }
+                best = bc;
+            }
+            h_done = min(h0 + VT, max_iters);
+            double need;   // adaptive number of hypotheses for `confidence`
+            const double pr = (double)best / (double)n, p4 = pr * pr * pr * pr;
+            if (p4 >= 1.0) need = 0.0;
+            else if (p4 <= 0.0) need = INFINITY;
+            else need = ceil(log1mconf / log(1.0 - p4));
+            __syncthreads();
+            if ((double)h_done >= fmin(need, (double)max_iters)) break;
+        }
+    }
+    if (best > 0) {
+        int cnt = score_rows(s.H, L1, L2, tent, n, th2, inl, s);   // = best
+        for (int r = 0; r < REFIT_ROUNDS && cnt >= 4; r++) {
+            if (!refit(L1, L2, tent, n, inl, cnt, s)) break;
+            const int c2 = score_rows(s.Hr, L1, L2, tent, n, th2, nullptr, s);
+            if (c2 < cnt) break;
+            cnt = c2;
+            if (tid < 9) s.H[tid] = s.Hr[tid];
+            __syncthreads();
+            score_rows(s.H, L1, L2, tent, n, th2, inl, s);
+        }
+        best = cnt;
+    } else {
+        for (int t = tid; t < n; t += VT) inl[t] = 0;
+    }
+    if (tid < 9) Hout[(size_t)p * 9 + tid] = best > 0 ? (float)s.H[tid] : 0.f;
+    if (tid == 0) {
+        ninl[p] = best;
+        if (iters) iters[p] = h_done;
+    }
+}
+
+// ---- ground-truth check (ReprojectionStuff.py:126-137) ----------------------------------------------------------------------------
+constexpr int GT_TILE = 2048;
+
+__global__ void __launch_bounds__(VT) gt_kernel(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2, int S2,
+                                                int cap2, const int* __restrict__ pairs, const int* __restrict__ tent_all,
+                                                const int* __restrict__ ntent, int tcap, const float* __restrict__ H1to2, float th,
+                                                float* __restrict__ min_dist, int* __restrict__ idx2, int* __restrict__ true_all,
+                                                int* __restrict__ ntrue) {
+    __shared__ float4 tile[GT_TILE];   // (x, y, |x|^2, -) of the image-2 centres mapped into image 1
+    __shared__ double Hi[9];
+    __shared__ int wsum[VT / 32];
+    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int i, j;
+    const int n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
+    const int* tent = tent_all + (size_t)p * tcap * 2;
+    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
+        if (tid == 0) ntrue[p] = -1;
+        return;
+    }
+    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
+    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
+    if (tid == 0) {   // H1to2^-1 = adj(H) / det(H), in fp64
+        double H[9], A[9];
+        for (int k = 0; k < 9; k++) H[k] = H1to2[(size_t)p * 9 + k];
+        adj3(H, A);
+        const double det = H[0] * A[0] + H[1] * A[3] + H[2] * A[6];
+        for (int k = 0; k < 9; k++) Hi[k] = A[k] / det;
+    }
+    __syncthreads();
+    const size_t base = (size_t)p * tcap;
+    int run = 0;
+    for (int r0 = 0; r0 < n; r0 += VT) {
+        const int t = r0 + tid;
+        float ax = 0.f, ay = 0.f, na = 0.f, best = INFINITY;
+        int bi = 0;
+        if (t < n) {
+            const float4 c = tent_centres(L1, L2, tent, t);
+            ax = c.x; ay = c.y;
+            na = __fadd_rn(__fmul_rn(ax, ax), __fmul_rn(ay, ay));
+        }
+        for (int u0 = 0; u0 < n; u0 += GT_TILE) {
+            const int m = min(GT_TILE, n - u0);
+            __syncthreads();
+            for (int u = tid; u < m; u += VT) {
+                const float4 c = tent_centres(L1, L2, tent, u0 + u);
+                const double x = c.z, y = c.w, w = Hi[6] * x + Hi[7] * y + Hi[8];
+                const float px = (float)((Hi[0] * x + Hi[1] * y + Hi[2]) / w), py = (float)((Hi[3] * x + Hi[4] * y + Hi[5]) / w);
+                tile[u] = make_float4(px, py, __fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), 0.f);
+            }
+            __syncthreads();
+            if (t < n)
+                for (int u = 0; u < m; u++) {
+                    const float4 q = tile[u];
+                    // sqrt(|(|p|^2 + |a|^2) - 2 a.p + 1e-12|), the rounding steps of ReprojectionStuff.distance_matrix_vector
+                    const float dot = __fmaf_rn(ay, q.y, __fmul_rn(ax, q.x));
+                    const float v = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fadd_rn(q.z, na), __fmul_rn(2.f, dot)), 1e-12f)));
+                    if (v < best) { best = v; bi = u0 + u; }   // ascending u: the lowest index among the minima
+                }
+        }
+        const bool keep = t < n && best <= th;
+        if (t < n) { min_dist[base + t] = best; idx2[base + t] = bi; }
+        const unsigned b = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) wsum[warp] = __popc(b);
+        __syncthreads();
+        int off = run, tot = 0;
+#pragma unroll
+        for (int w = 0; w < VT / 32; w++) {
+            off += w < warp ? wsum[w] : 0;
+            tot += wsum[w];
+        }
+        if (keep) true_all[base + off + __popc(b & ((1u << lane) - 1u))] = t;
+        run += tot;
+        __syncthreads();   // wsum is rewritten by the next row block
+    }
+    if (tid == 0) ntrue[p] = run;
+}
+
+int verify_args(const char* fn, const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                const int* d_tent, const int* d_ntent, int tcap) {
+    const char* msg = nullptr;
+    if (!d_lafs1 || !d_lafs2 || !d_tent || !d_ntent) msg = "NULL LAFs or tentatives";
+    else if (S1 < 1 || S2 < 1 || cap1 < 1 || cap2 < 1 || P < 1) msg = "S1, S2, cap1, cap2 and P must be >= 1";
+    else if (!d_pairs && (S1 != S2 || P != S1)) msg = "d_pairs == NULL (pair p = (p, p)) needs S1 == S2 == P";
+    else if (tcap < 1 || tcap > MAX_TCAP) msg = "tcap must be in 1..4194240";
+    if (!msg) return AG_OK;
+    set_error("%s: %s", fn, msg);
+    return AG_ERR_INVALID;
+}
+
+}  // namespace ag
+
+using namespace ag;
+
+extern "C" {
+
+int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                         const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
+                         float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
+    int rc = verify_args("ag_homography_ransac", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc) return rc;
+    AG_REQUIRE(d_H && d_inl && d_ninl, "NULL output");
+    AG_REQUIRE(inl_th > 0.f && isfinite(inl_th), "inl_th must be finite and > 0");
+    AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
+    AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
+    const double th = inl_th;
+    ransac_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
+                                                      log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_H, d_inl, d_ninl, d_iters);
+    AG_CHECK_LAUNCH("ransac_kernel");
+    return AG_OK;
+}
+
+int ag_gt_correspondences_pairs(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                                const int* d_tent, const int* d_ntent, int tcap, const float* d_H1to2, float dist_threshold,
+                                float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream) {
+    int rc = verify_args("ag_gt_correspondences_pairs", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc) return rc;
+    AG_REQUIRE(d_H1to2 && d_min_dist && d_idx2 && d_true && d_ntrue, "NULL homography or output");
+    AG_REQUIRE(dist_threshold >= 0.f, "dist_threshold must be >= 0 (and not NaN)");
+    gt_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, d_H1to2, dist_threshold,
+                                                  d_min_dist, d_idx2, d_true, d_ntrue);
+    AG_CHECK_LAUNCH("gt_kernel");
+    return AG_OK;
+}
+
+}  // extern "C"

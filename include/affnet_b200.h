@@ -301,6 +301,39 @@ int ag_match_pairs(const float* d_desc1, const int* d_count1, int S1, int cap1, 
                    int dim, const int* d_pairs, int P, float ratio, void* d_ws, size_t ws_bytes, int* d_idx2, float* d_min, float* d_second,
                    unsigned char* d_keep, int* d_tent, int* d_ntent, void* stream);
 
+/* Geometric verification of the batched matcher's tentatives (new; the reference verifies one pair at a time on the CPU).  Both take
+ * ag_match_pairs' outputs as they are: LAFs of set 1 d_lafs1 [S1,cap1,2,3] and set 2 d_lafs2 [S2,cap2,2,3] (pixel LAFs of the pipeline),
+ * d_pairs [P,2] (NULL: pair p = (p, p), then S1 == S2 == P), d_tent [P,tcap,2] and d_ntent [P].  Tentative t of pair p = (i, j) joins the
+ * centre lafs1[i, tent[p,t,0], :, 2] with lafs2[j, tent[p,t,1], :, 2].  Everything is read on the device; one launch whatever P is, no
+ * allocation, no synchronisation (CUDA-graph capturable), no workspace.
+ * A pair with ntent outside 0..tcap, an image index out of range or a tentative row outside 0..cap-1 gets -1 in its count (d_ninl /
+ * d_ntrue) and nothing else of it is written.  Rows at or beyond ntent[p] are not written.
+ * AG_ERR_INVALID, before any CUDA call: NULL inputs or outputs, S / cap / P < 1, d_pairs == NULL with S1 != S2 or P != S1, tcap outside
+ * 1..4194240, and the parameter ranges given below.
+ *
+ * ag_homography_ransac: homography RANSAC per pair (the notebook's ransac_validate, findHomography(src, dst, 2.0, 0.99, 50000)),
+ * deterministic for a given seed and independent of P and of the pair's position in the list.  Hypothesis h draws 4 distinct indices
+ * from splitmix64(splitmix64((h << 32) | draw) ^ seed) (at most 64 draws), rejects samples with a collinear triplet in either image or a
+ * triplet orientation that differs between the images for some but not all triplets, and solves H = M2 adj(M1) in fp64 (M maps the
+ * projective basis onto the 4 points).  Inlier: h20 x + h21 y + h22 > 0 and |H x1 - x2|^2 <= inl_th^2 in fp64.  Best: most inliers,
+ * ties to the lowest h.  Hypotheses are evaluated in chunks of 256; after each chunk the search stops once the number evaluated reaches
+ * min(N, max_iters), N = ceil(log(1 - confidence) / log(1 - (best/n)^4)).  Then up to 3 rounds of normalised-DLT least squares on the
+ * inliers, each kept only if the inlier count does not drop.
+ *   d_H [P,3,3] (H[2][2] = 1), d_inl [P,tcap] u8, d_ninl [P], d_iters [P] (hypotheses evaluated; may be NULL).  n < 4 tentatives or no
+ *   hypothesis with an inlier: ninl = 0, H = 0, mask rows < n = 0.
+ *   AG_ERR_INVALID also for inl_th not finite and > 0, confidence outside (0, 1), max_iters < 1.
+ * ag_gt_correspondences_pairs: get_GT_correspondence_indexes (ReprojectionStuff.py:126-137) per pair with d_H1to2 [P,3,3]: the image-2
+ * centres of all the pair's tentatives are mapped through H^-1 into image 1, and tentative t is true when ANY of them lies within
+ * dist_threshold of its image-1 centre, by the fp32 distance sqrt(|(|p|^2 + |a|^2) - 2 a.p + 1e-12|) (nearest: the lowest index among the
+ * minima, NaN ignored).  d_min_dist, d_idx2 [P,tcap]; d_true [P,tcap] the true t in ascending order, d_ntrue [P] their number.
+ *   AG_ERR_INVALID also for dist_threshold < 0 or NaN. */
+int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                         const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
+                         float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
+int ag_gt_correspondences_pairs(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                                const int* d_tent, const int* d_ntent, int tcap, const float* d_H1to2, float dist_threshold,
+                                float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Batched end-to-end pipeline (new; the reference processes one image at a time):
  * pyramid -> detect -> select(1.5K) -> sample -> AffNet -> filter(K) -> [sample -> OriNet -> rotate]
