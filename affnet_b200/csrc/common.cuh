@@ -91,9 +91,11 @@ __device__ __forceinline__ void bitonic_sort_desc(unsigned long long* key, int* 
 
 // Bilinear tap with zeros outside the image (F.grid_sample, padding_mode='zeros').  Explicit rounding steps so that the
 // standalone sampler and the sampler fused into the first CNN layer produce identical bits.
+// The integer corner is converted from the floor clamped to [-2, w] x [-2, h]: every tap outside the image stays outside, and a
+// sample point beyond the int32 range cannot saturate to INT_MAX, whose x0 + 1 would wrap into the "inside" test.
 __device__ __forceinline__ float bilinear_zero(const float* __restrict__ img, int h, int w, float px, float py) {
     const float fx0 = floorf(px), fy0 = floorf(py);
-    const int x0 = (int)fx0, y0 = (int)fy0;
+    const int x0 = (int)fminf(fmaxf(fx0, -2.f), (float)w), y0 = (int)fminf(fmaxf(fy0, -2.f), (float)h);
     const float ax = __fsub_rn(px, fx0), ay = __fsub_rn(py, fy0);
     const float bx = __fsub_rn(1.f, ax), by = __fsub_rn(1.f, ay);
     const bool xin0 = (x0 >= 0) & (x0 < w), xin1 = (x0 + 1 >= 0) & (x0 + 1 < w);
@@ -109,7 +111,7 @@ __device__ __forceinline__ float bilinear_zero(const float* __restrict__ img, in
 // The same tap in two phases (issue the four loads early, combine later); bit-identical to bilinear_zero.
 __device__ __forceinline__ void bilinear_taps(const float* __restrict__ img, int h, int w, float px, float py, float (&t)[4], float& ax, float& ay) {
     const float fx0 = floorf(px), fy0 = floorf(py);
-    const int x0 = (int)fx0, y0 = (int)fy0;
+    const int x0 = (int)fminf(fmaxf(fx0, -2.f), (float)w), y0 = (int)fminf(fmaxf(fy0, -2.f), (float)h);   // as bilinear_zero
     ax = __fsub_rn(px, fx0); ay = __fsub_rn(py, fy0);
     const bool xin0 = (x0 >= 0) & (x0 < w), xin1 = (x0 + 1 >= 0) & (x0 + 1 < w);
     const bool yin0 = (y0 >= 0) & (y0 < h), yin1 = (y0 + 1 >= 0) & (y0 + 1 < h);

@@ -186,7 +186,10 @@ __global__ void __launch_bounds__(NT) blur_kernel(const float* __restrict__ in, 
     __syncthreads();
     // 3. vertical pass: 4 rows x 4 columns per thread
     const int h2 = (h + 1) >> 1, w2 = (w + 1) >> 1;
-    const bool vec_ok = (w & 3) == 0;
+    // 128-bit stores need gx + 3 < w (w % 4 == 0) and a 16-byte-aligned level: ag_pyramid_plan packs the levels back to back at B*h*w
+    // floats, so a level after an octave with odd h*w starts 1-3 floats past a 16-byte boundary.  With w % 4 == 0, b*h*w is a
+    // multiple of 4, so the base address alone decides.  The scalar branch stores the same values.
+    const bool vec_ok = (w & 3) == 0 && (reinterpret_cast<size_t>(out) & 15) == 0;
     {
         const int q = threadIdx.x & 15, rb = threadIdx.x >> 4;     // column quad 0..15, row block 0..15 (4 rows each)
         float4 acc[4];
@@ -213,7 +216,7 @@ __global__ void __launch_bounds__(NT) blur_kernel(const float* __restrict__ in, 
             float* orow = out + (size_t)b * h * w + (size_t)gy * w + gx;
             const float vals[4] = {acc[r].x, acc[r].y, acc[r].z, acc[r].w};
             if (vec_ok) {
-                *reinterpret_cast<float4*>(orow) = acc[r];           // w % 4 == 0 -> gx + 3 < w and 16-byte aligned
+                *reinterpret_cast<float4*>(orow) = acc[r];
             } else {
 #pragma unroll
                 for (int e = 0; e < 4; e++)
@@ -444,6 +447,13 @@ int ag_pyramid_build(const ag_pyramid_plan_t* p, const float* d_img, float* d_py
     AG_REQUIRE(p && d_img && d_pyr, "NULL argument");
     cudaStream_t st = (cudaStream_t)stream;
     const int nl = p->n_levels, seed_level = nl - 2;  // level `nlevels` seeds the next octave (:46-47)
+    // a schedule with a blur the kernel cannot run (more than 2*kMaxRadius+1 taps) is refused before anything is written
+    for (int o = 0; o < p->n_octaves; o++)
+        for (int l = (o == 0 && p->blur_sigma[0][0] > 0.0) ? 0 : 1; l < nl; l++) {
+            BlurTaps t;
+            int rc = make_taps(p->blur_sigma[o][l], &t);
+            if (rc != AG_OK) return rc;
+        }
     // Measured (r02, 16 x 1024x768): the one-launch-per-octave kernel is bit-identical but SLOWER than the per-level launches (octave 0: 0.80
     // vs 0.26 ms, whole pyramid 1.35 vs 0.68 ms): both are bound by instruction issue, and streaming rows gives the vertical pass one
     // 128-bit shared-memory load per 4 FMAs where blur_kernel's 4x4 register block gets 16.  It stays selectable for A/B runs

@@ -260,12 +260,12 @@ def multi_scale_detector(pyr, sigmas, num_features, mrSize, th=0.0, return_level
 # ----------------------------------------------------------------------------------------------
 
 
-def extract_patches(img, LAFs, PS=32):
+def extract_patches(img, LAFs, PS=32, out_dtype=torch.float32):
     """Closed form of affine_grid + grid_sample (bilinear, zeros, align_corners=False).
 
     out[n,0,i,j] = bilinear(img, p - 0.5), p = A_px (x_j, y_i)^T + t_px, x_j = (2j+1)/PS - 1,
     A_px = LAF[:, :, :2]*min(h,w), t_px = (LAF_x*w, LAF_y*h)   (LAF.py:313-324, 364-372).
-    img float32 [1,1,h,w]; LAFs float32 [n,2,3] normalised.  Evaluated in float64, returned fp32.
+    img float32 [1,1,h,w]; LAFs float32 [n,2,3] normalised.  Evaluated in float64, returned as out_dtype (fp32 by default).
     """
     h, w = img.size(2), img.size(3)
     n = LAFs.size(0)
@@ -286,7 +286,7 @@ def extract_patches(img, LAFs, PS=32):
 
     out = (tap(y0, x0) * (1 - fx) * (1 - fy) + tap(y0, x0 + 1) * fx * (1 - fy)
            + tap(y0 + 1, x0) * (1 - fx) * fy + tap(y0 + 1, x0 + 1) * fx * fy)
-    return out.float().view(n, 1, PS, PS)
+    return out.to(out_dtype).view(n, 1, PS, PS)
 
 
 def extract_patches_from_pyramid(pyr, pyr_idxs, level_idxs, LAFs, PS=32):
