@@ -179,17 +179,22 @@ void sift_windows(int PS, int k, float* gk, float* pk);
 int sift_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl, const int* d_count,
              int cap, int PS, int k, int s, const float* gk, const float* pk, float clipval, float* d_out, void* stream);
 
-// 2x2 products of the Baumberg chain in torch.bmm's fp32 operation order (row-by-column, two products added left to right); used by
-// mat2_compose_kernel / lafs_left_multiply_kernel (geometry.cu) and baumberg_pyr_kernel (handcrafted.cu).
+// 2x2 products in torch.bmm's fp32 CPU arithmetic: each entry rounds both products and then adds them, fl(fl(a*b) + fl(c*d)) (no fused
+// multiply-add: it differs in about a quarter of the entries), into an accumulator that starts at +0 (two -0 products give +0).  Used by the Baumberg chain (mat2_compose_kernel /
+// lafs_left_multiply_kernel, baumberg_pyr_kernel in handcrafted.cu) and by the shape filter's compose and the orientation compose
+// (geometry.cu); tests/geometry_restated.py states the same arithmetic.
+__device__ __forceinline__ float dot2_rn(float a, float b, float c, float d) {
+    return __fadd_rn(__fadd_rn(0.f, __fmul_rn(a, b)), __fmul_rn(c, d));
+}
 // out = A * B   (base_A <- A base_A, SparseImgRepresenter.py:133)
 __device__ __forceinline__ void mat2_mul(const float (&a)[4], const float (&b)[4], float (&o)[4]) {
-    o[0] = __fmaf_rn(a[1], b[2], __fmul_rn(a[0], b[0])); o[1] = __fmaf_rn(a[1], b[3], __fmul_rn(a[0], b[1]));
-    o[2] = __fmaf_rn(a[3], b[2], __fmul_rn(a[2], b[0])); o[3] = __fmaf_rn(a[3], b[3], __fmul_rn(a[2], b[1]));
+    o[0] = dot2_rn(a[0], b[0], a[1], b[2]); o[1] = dot2_rn(a[0], b[1], a[1], b[3]);
+    o[2] = dot2_rn(a[2], b[0], a[3], b[2]); o[3] = dot2_rn(a[2], b[1], a[3], b[3]);
 }
 // out = [A * L[:, :2] | L[:, 2]]   (the working LAF of the next Baumberg iteration, SparseImgRepresenter.py:134-135)
 __device__ __forceinline__ void laf_left_mul(const float (&a)[4], const float (&l)[6], float (&o)[6]) {
-    o[0] = __fmaf_rn(a[1], l[3], __fmul_rn(a[0], l[0])); o[1] = __fmaf_rn(a[1], l[4], __fmul_rn(a[0], l[1])); o[2] = l[2];
-    o[3] = __fmaf_rn(a[3], l[3], __fmul_rn(a[2], l[0])); o[4] = __fmaf_rn(a[3], l[4], __fmul_rn(a[2], l[1])); o[5] = l[5];
+    o[0] = dot2_rn(a[0], l[0], a[1], l[3]); o[1] = dot2_rn(a[0], l[1], a[1], l[4]); o[2] = l[2];
+    o[3] = dot2_rn(a[2], l[0], a[3], l[3]); o[4] = dot2_rn(a[2], l[1], a[3], l[4]); o[5] = l[5];
 }
 
 }  // namespace ag

@@ -46,17 +46,22 @@ __device__ __forceinline__ bool shape_ok(const float* A, const float* NL) {
 #pragma unroll
     for (int c = 0; c < 4; c++) {
         const float x = (c & 2) ? 1.f : -1.f, y = (c & 1) ? 1.f : -1.f;
-        const float ox = fmaf(NL[0], x, fmaf(NL[1], y, NL[2]));
-        const float oy = fmaf(NL[3], x, fmaf(NL[4], y, NL[5]));
+        // (h0*x + h1*y) + h2, as the reference's matmul sums it (h1*y + h2 first can put a corner on the other side of 0 or 1)
+        const float ox = __fadd_rn(__fadd_rn(__fmul_rn(NL[0], x), __fmul_rn(NL[1], y)), NL[2]);
+        const float oy = __fadd_rn(__fadd_rn(__fmul_rn(NL[3], x), __fmul_rn(NL[4], y)), NL[5]);
         ok = ok && !(ox > 1.0f || ox < 0.0f || oy > 1.0f || oy < 0.0f);
     }
     return ok;
 }
 
 __device__ __forceinline__ void compose_laf(const float* A, const float* L, float* NL) {
-    // new_LAF = [bmm(A, LAF[:, :, 0:2]), LAF[:, :, 2:]]   SparseImgRepresenter.py:138
-    NL[0] = fmaf(A[0], L[0], A[1] * L[3]); NL[1] = fmaf(A[0], L[1], A[1] * L[4]); NL[2] = L[2];
-    NL[3] = fmaf(A[2], L[0], A[3] * L[3]); NL[4] = fmaf(A[2], L[1], A[3] * L[4]); NL[5] = L[5];
+    // new_LAF = [bmm(A, LAF[:, :, 0:2]), LAF[:, :, 2:]]   SparseImgRepresenter.py:138 (laf_left_mul: both products rounded, as bmm)
+    const float a[4] = {A[0], A[1], A[2], A[3]};
+    const float l[6] = {L[0], L[1], L[2], L[3], L[4], L[5]};
+    float o[6];
+    laf_left_mul(a, l, o);
+#pragma unroll
+    for (int q = 0; q < 6; q++) NL[q] = o[q];
 }
 
 __global__ void __launch_bounds__(GNT) shape_filter_kernel(const ShapeParams P) {
@@ -90,7 +95,8 @@ __global__ void __launch_bounds__(GNT) shape_filter_kernel(const ShapeParams P) 
             float NL[6];
             compose_laf(A + i * 4, L + i * 6, NL);
             const bool ok = shape_ok(A + i * 4, NL);
-            const unsigned hi = sorted ? float_to_ordered(ok ? R[i] : 0.f) : (ok ? 1u : 0u);
+            // sorted: the key is resp * mask (rejected rows as zeros, ahead of negative survivors), -0 made +0 so that it ties by index
+            const unsigned hi = sorted ? float_to_ordered(__fadd_rn(__fmul_rn(R[i], ok ? 1.f : 0.f), 0.f)) : (ok ? 1u : 0u);
             k = ((unsigned long long)hi << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)i);
         }
         s_key[i] = k;
@@ -102,7 +108,8 @@ __global__ void __launch_bounds__(GNT) shape_filter_kernel(const ShapeParams P) 
         const size_t o = (size_t)b * P.out_cap + r;
         float NL[6];
         compose_laf(A + i * 4, L + i * 6, NL);
-        P.resp_out[o] = R[i];
+        // sorted: topk's value, resp * mask (a rejected row that makes the cut comes out as the reference's zero); else resp
+        P.resp_out[o] = sorted ? __fmul_rn(R[i], shape_ok(A + i * 4, NL) ? 1.f : 0.f) : R[i];
 #pragma unroll
         for (int q = 0; q < 6; q++) P.lafs_out[o * 6 + q] = NL[q];
         P.oct_out[o] = P.oct[(size_t)b * P.cap + i];
@@ -116,9 +123,10 @@ __global__ void lafs_rotate_kernel(float* __restrict__ lafs, const float* __rest
     if (i >= n) return;
     float* L = lafs + (size_t)i * 6;
     const float* r = R + (size_t)i * 4;
-    const float l00 = L[0], l01 = L[1], l10 = L[3], l11 = L[4];
-    L[0] = fmaf(l00, r[0], l01 * r[2]); L[1] = fmaf(l00, r[1], l01 * r[3]);
-    L[3] = fmaf(l10, r[0], l11 * r[2]); L[4] = fmaf(l10, r[1], l11 * r[3]);
+    const float l[4] = {L[0], L[1], L[3], L[4]}, rr[4] = {r[0], r[1], r[2], r[3]};
+    float o[4];
+    mat2_mul(l, rr, o);   // bmm(LAF[:, :, :2], R), SparseImgRepresenter.py:175
+    L[0] = o[0]; L[1] = o[1]; L[3] = o[2]; L[4] = o[3];
 }
 
 __global__ void lafs_scale_kernel(const float* __restrict__ in, float* __restrict__ out, int n, float ac, float xc, float yc) {
@@ -136,7 +144,7 @@ __global__ void lafs_to_ell_kernel(const float* __restrict__ lafs, float* __rest
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float* L = lafs + (size_t)i * 6;
-    const float scale = sqrtf(L[0] * L[4] - L[1] * L[3] + 1e-10f);
+    const float scale = sqrtf(__fadd_rn(__fsub_rn(__fmul_rn(L[0], L[4]), __fmul_rn(L[1], L[3])), 1e-10f));   // not contracted
     const float a00 = L[0] / scale, a01 = L[1] / scale, a10 = L[3] / scale, a11 = L[4] / scale;
     // Su = A A^T
     const float s00 = a00 * a00 + a01 * a01, s01 = a00 * a10 + a01 * a11, s11 = a10 * a10 + a11 * a11;

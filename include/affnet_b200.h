@@ -222,8 +222,12 @@ int ag_net_forward_pyr(const ag_net_t* net, const ag_pyramid_plan_t* plan, const
  * ------------------------------------------------------------------------------------------ */
 /* Per image b (B images, `cap` rows each, d_count_in[b] valid):  new_LAF = [A*LAF_A, t]; keep where
  * 1/6 < |l1/(l2+1e-8)| < 6 and the LAF does not touch the boundary; if survivors > num_features keep the
- * top num_features by response (desc; ties by index) else all survivors in order.
- * Outputs are compacted: d_resp_out/d_lafs_out/d_oct_out/d_lvl_out [B,out_cap..], d_count_out [B]. */
+ * top num_features by resp * keep (desc; ties by index, -0 equal to +0) else all survivors in order.  In the first case the response
+ * written is resp * keep, so a rejected row that makes the cut (when survivors have negative responses) comes out as 0, as
+ * torch.topk returns it in the reference.  All arithmetic is the reference's fp32 CPU arithmetic, without fused multiply-adds
+ * (tests/test_gpu_geometry.py pins it bit for bit).
+ * Outputs are compacted: d_resp_out/d_lafs_out/d_oct_out/d_lvl_out [B,out_cap..], d_count_out [B]; only the first d_count_out[b] rows
+ * of image b are written, and d_count_out[b] = -1 where d_count_in[b] < 0.  cap above 16384 returns AG_ERR_CAPACITY and writes nothing. */
 int ag_affine_shape_filter(const float* d_A, const float* d_resp, const float* d_lafs, const int* d_oct,
                            const int* d_lvl, const int* d_count_in, int B, int cap, int num_features, int out_cap,
                            float* d_resp_out, float* d_lafs_out, int* d_oct_out, int* d_lvl_out, int* d_count_out,
