@@ -71,54 +71,41 @@ class ScaleSpaceAffinePatchExtractor(nn.Module):
             ws = L.DetectWs()
             L.check(lib.ag_detect_ws_carve(C.byref(plan), cap, L.ptr(ws_buf), C.byref(ws)))
             L.check(lib.ag_detect(C.byref(plan), L.ptr(self._pyr_buf), float(self.th), int(self.mrSize), C.byref(ws), L.stream_ptr()))
-            n_slots = ws.n_level_slots
             if num_features > 0:
                 out_cap = num_features
-                resp = torch.empty(out_cap, dtype=torch.float32, device=dev)
-                lafs = torch.empty(out_cap, 2, 3, dtype=torch.float32, device=dev)
-                oct_ = torch.empty(out_cap, dtype=torch.int32, device=dev)
-                lvl = torch.empty(out_cap, dtype=torch.int32, device=dev)
-                cnt = torch.empty(1, dtype=torch.int32, device=dev)
+                resp, lafs, oct_, lvl, cnt = self._select_outputs(out_cap, dev)
                 L.check(lib.ag_select_keypoints(C.byref(plan), C.byref(ws), num_features, float(a_scale), out_cap, L.ptr(resp),
                                                 L.ptr(lafs), L.ptr(oct_), L.ptr(lvl), L.ptr(cnt), L.stream_ptr()))
-            # one host round trip: candidate count (overflow check) + selected count
-            hdr = self._wrap_i32(ws.d_cand_count, 1 + 2 * n_slots, ws_buf)
-            host = torch.cat([hdr, cnt]).cpu() if num_features > 0 else hdr.cpu()
+                # one host round trip: candidate count (overflow check) + selected count
+                host = torch.cat([self._wrap_i32(ws.d_cand_count, 1, ws_buf), cnt]).cpu()
+            else:
+                host = self._wrap_i32(ws.d_cand_count, 1, ws_buf).cpu()
             n_cand = int(host[0])
             if n_cand > cap:
                 cap = n_cand + 1024
                 continue
-            if num_features > 0:
-                n = int(host[-1])
-                return resp[:n], lafs[:n], oct_[:n], lvl[:n]
-            return self._select_all(ws, ws_buf, host, n_cand, a_scale)
+            if num_features <= 0:
+                # th mode: every candidate of the accepted levels in (octave, level, raster) order; the candidate count bounds them
+                resp, lafs, oct_, lvl, cnt = self._select_outputs(max(n_cand, 1), dev)
+                scratch = torch.empty(lib.ag_select_all_workspace_bytes(C.byref(plan), cap), dtype=torch.uint8, device=dev)
+                L.check(lib.ag_select_all_keypoints(C.byref(plan), C.byref(ws), float(a_scale), max(n_cand, 1), L.ptr(scratch),
+                                                    scratch.numel(), L.ptr(resp), L.ptr(lafs), L.ptr(oct_), L.ptr(lvl), L.ptr(cnt),
+                                                    L.stream_ptr()))
+                host = cnt.cpu()
+            n = int(host[-1])
+            return resp[:n], lafs[:n], oct_[:n], lvl[:n]
+
+    @staticmethod
+    def _select_outputs(n, dev):
+        return (torch.empty(n, dtype=torch.float32, device=dev), torch.empty(n, 2, 3, dtype=torch.float32, device=dev),
+                torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+                torch.empty(1, dtype=torch.int32, device=dev))
 
     @staticmethod
     def _wrap_i32(addr, n, owner):
         """View `n` int32 at device address `addr` inside `owner` (a uint8 tensor)."""
         off = addr - owner.data_ptr()
         return owner[off:off + 4 * n].view(torch.int32)
-
-    def _select_all(self, ws, ws_buf, host, n_cand, a_scale):
-        """num_features <= 0 (th mode): every candidate of the accepted levels in (octave, level, raster) order.
-        Plain tensor plumbing over the candidate list the detect kernel produced."""
-        n_slots, cap = ws.n_level_slots, ws.cand_cap
-        pos = host[1:1 + n_slots]
-        f32 = lambda addr, n: ws_buf[addr - ws_buf.data_ptr():addr - ws_buf.data_ptr() + 4 * n].view(torch.float32)  # noqa: E731
-        val = f32(ws.d_cand_val, cap)[:n_cand]
-        seq = self._wrap_i32(ws.d_cand_seq, cap, ws_buf)[:n_cand].to(torch.int64) & 0xFFFFFFFF
-        scyx = f32(ws.d_cand_scyx, cap * 3).view(cap, 3)[:n_cand]
-        slot = seq >> 27
-        live = seq != 0xFFFFFFFF                                    # dropped by the resolve pass
-        accept = live & (pos > 1).to(val.device)[slot.clamp(max=n_slots - 1)]
-        order = torch.argsort(torch.where(accept, seq, torch.full_like(seq, 1 << 40)))[:int(accept.sum())]
-        val, scyx, slot = val[order], scyx[order], slot[order]
-        n_det = self._plan.n_levels - 2
-        lafs = torch.zeros(val.numel(), 2, 3, dtype=torch.float32, device=val.device)
-        lafs[:, 0, 0] = lafs[:, 1, 1] = scyx[:, 0] * a_scale
-        lafs[:, 0, 2] = scyx[:, 2]
-        lafs[:, 1, 2] = scyx[:, 1]
-        return val.clone(), lafs, (slot // n_det).to(torch.int32), (slot % n_det).to(torch.int32)
 
     def multiScaleDetector(self, x, num_features=0):
         """SparseImgRepresenter.py:53-111 -> (responses, LAFs normalised (A not yet scaled by mrSize), pyr_idxs, level_idxs)."""
@@ -173,7 +160,13 @@ class ScaleSpaceAffinePatchExtractor(nn.Module):
         lvl_o = torch.empty(n, dtype=torch.int32, device=dev)
         cnt_in = torch.tensor([n], dtype=torch.int32, device=dev)
         cnt_o = torch.empty(1, dtype=torch.int32, device=dev)
-        if n > 0:
+        if n > 0 and num_features <= 0:
+            # every survivor in order (:151-156), at any n
+            L.check(L.lib().ag_affine_shape_filter_all(L.ptr(base_A), L.ptr(final_resp), L.ptr(LAFs), L.ptr(oct_), L.ptr(lvl), L.ptr(cnt_in),
+                                                       1, n, L.ptr(resp_o), L.ptr(lafs_o), L.ptr(oct_o), L.ptr(lvl_o), L.ptr(cnt_o),
+                                                       L.stream_ptr()))
+            m = int(cnt_o.item())
+        elif n > 0:
             L.check(L.lib().ag_affine_shape_filter(L.ptr(base_A), L.ptr(final_resp), L.ptr(LAFs), L.ptr(oct_), L.ptr(lvl), L.ptr(cnt_in),
                                                    1, n, int(num_features), n, L.ptr(resp_o), L.ptr(lafs_o), L.ptr(oct_o), L.ptr(lvl_o),
                                                    L.ptr(cnt_o), L.stream_ptr()))

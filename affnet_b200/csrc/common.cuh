@@ -69,6 +69,32 @@ __host__ __device__ inline uint32_t float_to_ordered(float f) {
 
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
+// Exclusive prefix sum of one int per thread over a block of NT threads (a multiple of 32, at most 1024); `total` receives the block's
+// sum.  s_warp holds NT / 32 ints of shared memory.  Starts and ends with a barrier, so it may be called in a loop on the same s_warp.
+template <int NT>
+__device__ __forceinline__ int block_exclusive_scan(int v, int* s_warp, int& total) {
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    int incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    __syncthreads();
+    if (lane == 31) s_warp[wid] = incl;
+    __syncthreads();
+    int before = 0, sum = 0;
+#pragma unroll
+    for (int w = 0; w < NT / 32; w++) {
+        const int t = s_warp[w];
+        before += (w < wid) ? t : 0;
+        sum += t;
+    }
+    total = sum;
+    __syncthreads();
+    return before + incl - v;
+}
+
 // Block-wide bitonic sort (descending) of n = 2^k 64-bit keys in shared memory, optionally with an int payload.  Every thread owns whole
 // compare-exchange PAIRS (pair p -> elements i = p with a 0 bit inserted at log2(j), i | j), so no thread idles on the "ixj > i" half:
 // half the loop trips of the textbook form.

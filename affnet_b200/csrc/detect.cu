@@ -970,6 +970,19 @@ struct SelectParams {
     int* count;
 };
 
+// One selected keypoint, output row o: its response, the normalised LAF [[a s, 0, x], [0, a s, y]] with a = a_scale (mrSize *
+// LAFs[:, :, 0:2], SparseImgRepresenter.py:198), octave and level index of its detection slot
+__device__ __forceinline__ void write_keypoint(float a_scale, float val, const float* scyx, int slot, int n_det, size_t o, float* resp,
+                                               float* lafs, int* oct, int* lvl) {
+    const float sc = __fmul_rn(a_scale, scyx[0]);
+    resp[o] = val;
+    float* L = lafs + o * 6;
+    L[0] = sc; L[1] = 0.f; L[2] = scyx[2];
+    L[3] = 0.f; L[4] = sc; L[5] = scyx[1];
+    oct[o] = slot / n_det;
+    lvl[o] = slot % n_det;  // detection level_idx - 1: patches come from the level below (:94)
+}
+
 // A cluster of SEL_CL CTAs per image (thread-block cluster, distributed shared memory): every CTA scans 1/SEL_CL of the candidate list,
 // the per-pass histograms of the radix select are merged by CTA 0 through DSMEM, the selected candidates are appended to CTA 0's sort
 // buffer with DSMEM atomics, and CTA 0 sorts and writes the output.  The radix select stops as soon as the chosen digit's bucket is needed
@@ -1130,18 +1143,143 @@ __global__ void __launch_bounds__(SNT) select_kernel(const SelectParams P) {
     const float* scyx = P.cand_scyx + (size_t)b * P.cand_cap * 3;
     for (int i = threadIdx.x; i < m_out; i += SNT) {
         const int c = s_idx[i];
-        const size_t o = (size_t)b * P.out_cap + i;
-        const float sc = __fmul_rn(P.a_scale, scyx[c * 3 + 0]);  // mrSize * LAFs[:, :, 0:2]   SparseImgRepresenter.py:198
-        P.resp[o] = val[c];
-        float* L = P.lafs + o * 6;
-        L[0] = sc; L[1] = 0.f; L[2] = scyx[c * 3 + 2];
-        L[3] = 0.f; L[4] = sc; L[5] = scyx[c * 3 + 1];
-        const int slot = (int)(seq[c] >> SEQ_PIX_BITS);
-        P.oct[o] = slot / P.n_det;
-        P.lvl[o] = slot % P.n_det;  // detection level_idx - 1: patches come from the level below (:94)
+        write_keypoint(P.a_scale, val[c], scyx + (size_t)c * 3, (int)(seq[c] >> SEQ_PIX_BITS), P.n_det, (size_t)b * P.out_cap + i, P.resp, P.lafs,
+                       P.oct, P.lvl);
     }
     // a candidate list that overflowed its capacity is reported as count = -1 (downstream kernels then process no rows)
     if (threadIdx.x == 0) P.count[b] = (P.cand_count[b] > P.cand_cap) ? -1 : m_out;
+}
+
+// ---- ordered keep-all selection at any count (threshold mode: num_features <= 0, every candidate of the accepted levels) ----------
+// The answer is every live candidate of an accepted slot in ascending seq = (slot, raster pixel) order.  A bitmap over the pixels of every
+// detection level, concatenated in slot order, holds one bit per live candidate (set with atomicOr: the result does not depend on the
+// order); the row of a candidate is then the number of set bits before its own: the exclusive prefix of the per-word popcounts plus the
+// popcount of its word below its bit.  Four launches and a memset, none of which sorts: O(pixels / 32 + candidates), no count limit.
+constexpr int SA_NT = 256;
+constexpr int SA_WPT = 8;                   // bitmap words per thread in the prefix kernels
+constexpr int SA_CHUNK = SA_NT * SA_WPT;    // bitmap words per CTA in the prefix kernels
+constexpr int SA_MAX_GRID = 1024;           // CTAs per image of the candidate loops (grid-stride beyond)
+
+struct SelectAllParams {
+    const float* cand_val;
+    const uint32_t* cand_seq;
+    const float* cand_scyx;
+    const int* cand_count;
+    const int* level_pos;
+    int cand_cap, n_slots, n_det, out_cap;
+    int nw, nc;                     // bitmap words / prefix chunks per image
+    int word_base[32];              // first bitmap word of each slot
+    float a_scale;
+    uint32_t* bits;                 // [B, nw]
+    int* word_prefix;               // [B, nw] set bits of the image before word w
+    int* chunk_sum;                 // [B, nc]
+    int* total;                     // [B]
+    float* resp;
+    float* lafs;
+    int* oct;
+    int* lvl;
+    int* count;
+};
+
+__device__ __forceinline__ unsigned accepted_slots(const int* level_pos, int b, int n_slots) {
+    // warp 0: bit s set when slot s has more than one positive response (HandCraftedModules.py:253)
+    const bool a = (int)threadIdx.x < n_slots && level_pos[b * n_slots + threadIdx.x] > 1;
+    return __ballot_sync(0xffffffffu, a);
+}
+
+__device__ __forceinline__ bool live_candidate(uint32_t sq, unsigned accept) {
+    return sq != 0xFFFFFFFFu && ((accept >> (sq >> SEQ_PIX_BITS)) & 1u);   // dropped by resolve_kernel / level not accepted
+}
+
+__global__ void __launch_bounds__(SA_NT) select_all_mark_kernel(const SelectAllParams P) {
+    __shared__ unsigned s_accept;
+    const int b = blockIdx.y;
+    const int n = P.cand_count[b];
+    if (n > P.cand_cap) return;   // overflowed: reported as -1 by the scatter, nothing marked
+    if (threadIdx.x < 32) {
+        const unsigned a = accepted_slots(P.level_pos, b, P.n_slots);
+        if (threadIdx.x == 0) s_accept = a;
+    }
+    __syncthreads();
+    const unsigned accept = s_accept;
+    const uint32_t* seq = P.cand_seq + (size_t)b * P.cand_cap;
+    uint32_t* bits = P.bits + (size_t)b * P.nw;
+    for (int i = blockIdx.x * SA_NT + threadIdx.x; i < n; i += gridDim.x * SA_NT) {
+        const uint32_t sq = seq[i];
+        if (!live_candidate(sq, accept)) continue;
+        const uint32_t pix = sq & ((1u << SEQ_PIX_BITS) - 1u);
+        atomicOr(&bits[P.word_base[sq >> SEQ_PIX_BITS] + (int)(pix >> 5)], 1u << (pix & 31u));
+    }
+}
+
+__global__ void __launch_bounds__(SA_NT) select_all_chunk_kernel(const SelectAllParams P) {
+    __shared__ int s_warp[SA_NT / 32];
+    const int b = blockIdx.y, c = blockIdx.x;
+    const uint32_t* bits = P.bits + (size_t)b * P.nw;
+    int s = 0;
+#pragma unroll
+    for (int k = 0; k < SA_WPT; k++) {
+        const int w = c * SA_CHUNK + k * SA_NT + threadIdx.x;
+        if (w < P.nw) s += __popc(bits[w]);
+    }
+    int total;
+    block_exclusive_scan<SA_NT>(s, s_warp, total);
+    if (threadIdx.x == 0) P.chunk_sum[(size_t)b * P.nc + c] = total;
+}
+
+__global__ void __launch_bounds__(SA_NT) select_all_prefix_kernel(const SelectAllParams P) {
+    __shared__ int s_warp[SA_NT / 32];
+    const int b = blockIdx.y, c = blockIdx.x;
+    const int* cs = P.chunk_sum + (size_t)b * P.nc;
+    int before = 0;
+    for (int j = threadIdx.x; j < c; j += SA_NT) before += cs[j];
+    int base;
+    block_exclusive_scan<SA_NT>(before, s_warp, base);   // base: set bits in the chunks before this one
+    const uint32_t* bits = P.bits + (size_t)b * P.nw;
+    int* wp = P.word_prefix + (size_t)b * P.nw;
+    const int w0 = c * SA_CHUNK + threadIdx.x * SA_WPT;
+    int pc[SA_WPT], s = 0;
+#pragma unroll
+    for (int k = 0; k < SA_WPT; k++) {
+        pc[k] = (w0 + k < P.nw) ? __popc(bits[w0 + k]) : 0;
+        s += pc[k];
+    }
+    int chunk;
+    int run = base + block_exclusive_scan<SA_NT>(s, s_warp, chunk);
+#pragma unroll
+    for (int k = 0; k < SA_WPT; k++) {
+        if (w0 + k < P.nw) wp[w0 + k] = run;
+        run += pc[k];
+    }
+    if (c == P.nc - 1 && threadIdx.x == 0) P.total[b] = base + chunk;
+}
+
+__global__ void __launch_bounds__(SA_NT) select_all_scatter_kernel(const SelectAllParams P) {
+    __shared__ unsigned s_accept;
+    const int b = blockIdx.y;
+    const int n = P.cand_count[b], total = P.total[b];
+    const bool overflow = n > P.cand_cap || total > P.out_cap;
+    if (blockIdx.x == 0 && threadIdx.x == 0) P.count[b] = overflow ? -1 : total;
+    if (overflow) return;   // nothing of the image is written
+    if (threadIdx.x < 32) {
+        const unsigned a = accepted_slots(P.level_pos, b, P.n_slots);
+        if (threadIdx.x == 0) s_accept = a;
+    }
+    __syncthreads();
+    const unsigned accept = s_accept;
+    const size_t cb = (size_t)b * P.cand_cap;
+    const uint32_t* bits = P.bits + (size_t)b * P.nw;
+    const int* wp = P.word_prefix + (size_t)b * P.nw;
+    for (int i = blockIdx.x * SA_NT + threadIdx.x; i < n; i += gridDim.x * SA_NT) {
+        const uint32_t sq = P.cand_seq[cb + i];
+        if (!live_candidate(sq, accept)) continue;
+        const int slot = (int)(sq >> SEQ_PIX_BITS);
+        const uint32_t pix = sq & ((1u << SEQ_PIX_BITS) - 1u);
+        const int w = P.word_base[slot] + (int)(pix >> 5);
+        const int row = wp[w] + __popc(bits[w] & ((1u << (pix & 31u)) - 1u));
+        write_keypoint(P.a_scale, P.cand_val[cb + i], P.cand_scyx + (cb + i) * 3, slot, P.n_det, (size_t)b * P.out_cap + row, P.resp, P.lafs,
+                       P.oct, P.lvl);
+    }
 }
 
 }  // namespace ag
@@ -1380,6 +1518,65 @@ int ag_select_keypoints(const ag_pyramid_plan_t* p, const ag_detect_ws_t* ws, in
     int rcl = check_cuda(cudaLaunchKernelEx(&cfg, select_kernel, S), "select_kernel launch");
     if (rcl != AG_OK) return rcl;
     AG_CHECK_LAUNCH("select_kernel");
+    return AG_OK;
+}
+
+// Scratch of ag_select_all_keypoints: bitmap and word prefixes over every detection level's pixels, chunk sums, per-image totals.
+static void select_all_layout(const ag_pyramid_plan_t* p, int word_base[32], int* nw, int* nc) {
+    const int n_det = p->n_levels - 2;
+    long long w = 0;
+    for (int s = 0; s < p->n_octaves * n_det && s < 32; s++) {
+        word_base[s] = (int)w;
+        const int o = s / n_det;
+        w += ((long long)p->h[o] * p->w[o] + 31) / 32;
+    }
+    *nw = (int)w;
+    *nc = (int)((w + SA_CHUNK - 1) / SA_CHUNK);
+}
+
+size_t ag_select_all_workspace_bytes(const ag_pyramid_plan_t* p, int cand_cap) {
+    if (!p || cand_cap <= 0 || p->B < 1 || p->n_levels < 3 || p->n_octaves * (p->n_levels - 2) > 32) return 0;
+    int wb[32], nw, nc;
+    select_all_layout(p, wb, &nw, &nc);
+    const size_t B = p->B;
+    return 2 * align_up(B * nw * sizeof(uint32_t), 256) + align_up(B * nc * sizeof(int), 256) + align_up(B * sizeof(int), 256);
+}
+
+int ag_select_all_keypoints(const ag_pyramid_plan_t* p, const ag_detect_ws_t* ws, float a_scale, int out_cap, void* d_scratch,
+                            size_t scratch_bytes, float* d_resp, float* d_lafs, int* d_oct, int* d_lvl, int* d_count, void* stream) {
+    AG_REQUIRE(p && ws && d_scratch && d_resp && d_lafs && d_oct && d_lvl && d_count, "NULL argument");
+    AG_REQUIRE(out_cap >= 1, "out_cap must be positive");
+    AG_REQUIRE(ws->B == p->B && ws->n_level_slots == p->n_octaves * (p->n_levels - 2) && ws->n_level_slots <= 32, "workspace / plan mismatch");
+    const size_t need = ag_select_all_workspace_bytes(p, ws->cand_cap);
+    if (scratch_bytes < need) {
+        set_error("ag_select_all_keypoints: scratch of %zu bytes needed, %zu given", need, scratch_bytes);
+        return AG_ERR_CAPACITY;
+    }
+    SelectAllParams S;
+    memset(&S, 0, sizeof(S));
+    select_all_layout(p, S.word_base, &S.nw, &S.nc);
+    S.cand_val = ws->d_cand_val; S.cand_seq = ws->d_cand_seq; S.cand_scyx = ws->d_cand_scyx;
+    S.cand_count = ws->d_cand_count; S.level_pos = ws->d_level_pos;
+    S.cand_cap = ws->cand_cap; S.n_slots = ws->n_level_slots; S.n_det = p->n_levels - 2; S.out_cap = out_cap; S.a_scale = a_scale;
+    const size_t B = p->B;
+    unsigned char* c = (unsigned char*)d_scratch;
+    S.bits = (uint32_t*)c; c += align_up(B * S.nw * sizeof(uint32_t), 256);
+    S.word_prefix = (int*)c; c += align_up(B * S.nw * sizeof(int), 256);
+    S.chunk_sum = (int*)c; c += align_up(B * S.nc * sizeof(int), 256);
+    S.total = (int*)c;
+    S.resp = d_resp; S.lafs = d_lafs; S.oct = d_oct; S.lvl = d_lvl; S.count = d_count;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = check_cuda(cudaMemsetAsync(S.bits, 0, B * S.nw * sizeof(uint32_t), st), "memset select bitmap");
+    if (rc != AG_OK) return rc;
+    const int grid = cdiv(ws->cand_cap, SA_NT) < SA_MAX_GRID ? cdiv(ws->cand_cap, SA_NT) : SA_MAX_GRID;
+    select_all_mark_kernel<<<dim3(grid, p->B), SA_NT, 0, st>>>(S);
+    AG_CHECK_LAUNCH("select_all_mark_kernel");
+    select_all_chunk_kernel<<<dim3(S.nc, p->B), SA_NT, 0, st>>>(S);
+    AG_CHECK_LAUNCH("select_all_chunk_kernel");
+    select_all_prefix_kernel<<<dim3(S.nc, p->B), SA_NT, 0, st>>>(S);
+    AG_CHECK_LAUNCH("select_all_prefix_kernel");
+    select_all_scatter_kernel<<<dim3(grid, p->B), SA_NT, 0, st>>>(S);
+    AG_CHECK_LAUNCH("select_all_scatter_kernel");
     return AG_OK;
 }
 

@@ -118,6 +118,52 @@ __global__ void __launch_bounds__(GNT) shape_filter_kernel(const ShapeParams P) 
     if (threadIdx.x == 0) P.count_out[b] = (P.count_in[b] < 0) ? -1 : m;   // -1 = upstream capacity overflow, propagated
 }
 
+// getAffineShape's num_features <= 0 branch (SparseImgRepresenter.py:151-156): every survivor in index order with its response unchanged,
+// at any cap.  One CTA per image walks the rows in chunks of GNT * FA_RPT; a block scan of the survivor flags gives each survivor its output
+// row.  Same compose_laf / shape_ok as shape_filter_kernel, so the rows equal its num_features = 0 answer bit for bit.
+constexpr int FA_RPT = 4;   // consecutive rows per thread and chunk
+
+__global__ void __launch_bounds__(GNT) shape_filter_all_kernel(const ShapeParams P) {
+    __shared__ int s_warp[GNT / 32];
+    const int b = blockIdx.x;
+    const int cin = P.count_in[b];
+    const int n = max(0, min(cin, P.cap));
+    const size_t rb = (size_t)b * P.cap;
+    const float* A = P.A + rb * 4;
+    const float* L = P.lafs + rb * 6;
+    int base = 0;
+    for (int r0 = 0; r0 < n; r0 += GNT * FA_RPT) {
+        const int i0 = r0 + threadIdx.x * FA_RPT;
+        float NL[FA_RPT][6];
+        bool ok[FA_RPT];
+        int c = 0;
+#pragma unroll
+        for (int k = 0; k < FA_RPT; k++) {
+            const int i = i0 + k;
+            ok[k] = false;
+            if (i < n) {
+                compose_laf(A + (size_t)i * 4, L + (size_t)i * 6, NL[k]);
+                ok[k] = shape_ok(A + (size_t)i * 4, NL[k]);
+            }
+            c += ok[k] ? 1 : 0;
+        }
+        int total;
+        int dst = base + block_exclusive_scan<GNT>(c, s_warp, total);
+#pragma unroll
+        for (int k = 0; k < FA_RPT; k++) {
+            if (!ok[k]) continue;
+            const size_t i = rb + i0 + k, o = rb + dst++;
+            P.resp_out[o] = P.resp[i];
+#pragma unroll
+            for (int q = 0; q < 6; q++) P.lafs_out[o * 6 + q] = NL[k][q];
+            P.oct_out[o] = P.oct[i];
+            P.lvl_out[o] = P.lvl[i];
+        }
+        base += total;
+    }
+    if (threadIdx.x == 0) P.count_out[b] = (cin < 0) ? -1 : base;   // -1 = upstream capacity overflow, propagated
+}
+
 __global__ void lafs_rotate_kernel(float* __restrict__ lafs, const float* __restrict__ R, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -217,6 +263,21 @@ int ag_affine_shape_filter(const float* d_A, const float* d_resp, const float* d
     P.resp_out = d_resp_out; P.lafs_out = d_lafs_out; P.oct_out = d_oct_out; P.lvl_out = d_lvl_out; P.count_out = d_count_out;
     shape_filter_kernel<<<B, GNT, smem, (cudaStream_t)stream>>>(P);
     AG_CHECK_LAUNCH("shape_filter_kernel");
+    return AG_OK;
+}
+
+int ag_affine_shape_filter_all(const float* d_A, const float* d_resp, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                               const int* d_count_in, int B, int cap, float* d_resp_out, float* d_lafs_out, int* d_oct_out, int* d_lvl_out,
+                               int* d_count_out, void* stream) {
+    AG_REQUIRE(d_A && d_resp && d_lafs && d_oct && d_lvl && d_count_in && d_resp_out && d_lafs_out && d_oct_out &&
+                   d_lvl_out && d_count_out, "NULL argument");
+    AG_REQUIRE(B >= 1 && cap >= 1, "bad sizes");
+    ShapeParams P;
+    P.A = d_A; P.resp = d_resp; P.lafs = d_lafs; P.oct = d_oct; P.lvl = d_lvl; P.count_in = d_count_in;
+    P.cap = cap; P.num_features = 0; P.out_cap = cap; P.sort_cap = 0;
+    P.resp_out = d_resp_out; P.lafs_out = d_lafs_out; P.oct_out = d_oct_out; P.lvl_out = d_lvl_out; P.count_out = d_count_out;
+    shape_filter_all_kernel<<<B, GNT, 0, (cudaStream_t)stream>>>(P);
+    AG_CHECK_LAUNCH("shape_filter_all_kernel");
     return AG_OK;
 }
 

@@ -21,17 +21,19 @@ struct ag_pipeline {
     const ag_net_t* aff;
     const ag_net_t* ori;
     const ag_net_t* hard;
-    int M;          // prefilter keypoints per image = int(1.5 K) with a shape step, K without
+    int M;          // prefilter keypoints per image = int(1.5 K) with a shape step, K without; C in threshold mode
     int cand_cap;
+    bool th_mode;   // ag_pipeline_create_th: detector threshold th, keep-all selection and shape filter
+    float th;
     // workspace layout (byte offsets)
     size_t off_pyr, off_det, off_resp1, off_lafs1, off_oct1, off_lvl1, off_cnt1, off_patches, off_A, off_lafs2, off_oct2,
-        off_lvl2, off_nlafs, off_oct3, off_lvl3, off_net, net_bytes, off_A2, off_base2, off_lafsw, total;
+        off_lvl2, off_nlafs, off_oct3, off_lvl3, off_net, net_bytes, off_A2, off_base2, off_lafsw, off_sel, sel_bytes, total;
     int launches;
 };
 
 using namespace ag;
 
-// ag_pipeline_create, ag_pipeline_create_ex and ag_pipeline_create_desc: `fn` names the entry point the caller called in the error texts
+// ag_pipeline_create, ag_pipeline_create_ex, ag_pipeline_create_desc and ag_pipeline_create_th: `fn` names the entry point the caller called in the error texts
 #define PIPE_REQUIRE(cond, msg)                         \
     do {                                                \
         if (!(cond)) {                                  \
@@ -42,8 +44,9 @@ using namespace ag;
 
 static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est,
                            const ag_pipeline_descriptor_t* desc, const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet,
-                           ag_pipeline_t** out) {
+                           bool th_mode, float th, ag_pipeline_t** out) {
     PIPE_REQUIRE(cfg && est && desc && out, "NULL argument");
+    PIPE_REQUIRE(isfinite(th), "th must be finite");
     PIPE_REQUIRE(desc->kind == AG_DESC_HARDNET || desc->kind == AG_DESC_SIFT, "unknown descriptor kind");
     const bool sift = desc->kind == AG_DESC_SIFT;
     PIPE_REQUIRE(sift || hardnet, "NULL argument: AG_DESC_HARDNET needs a HardNet");
@@ -69,14 +72,15 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
     p->hard = sift ? nullptr : hardnet;
     int rc = ag_pyramid_plan(cfg->B, cfg->H, cfg->W, cfg->nlevels, cfg->init_sigma, cfg->border, &p->plan);
     if (rc != AG_OK) { delete p; return rc; }
-    // the selection kernels sort in shared memory (ag_select_keypoints / ag_affine_shape_filter): fail here, not at run time
-    if (shape && (int)(1.5 * cfg->num_features) > 16384) {
+    // the top-K selection kernels sort in shared memory (ag_select_keypoints / ag_affine_shape_filter): fail here, not at run time.
+    // Threshold mode keeps everything without a sort and has no such limit.
+    if (!th_mode && shape && (int)(1.5 * cfg->num_features) > 16384) {
         set_error("%s: num_features %d needs a prefilter of int(1.5 K) = %d keypoints; the shared-memory selection holds 16384 (K <= 10923)",
                   fn, cfg->num_features, (int)(1.5 * cfg->num_features));
         delete p;
         return AG_ERR_CAPACITY;
     }
-    if (!shape && cfg->num_features > 16384) {
+    if (!th_mode && !shape && cfg->num_features > 16384) {
         set_error("%s: num_features %d without a shape estimator: the shared-memory selection holds 16384 (K <= 16384)", fn,
                   cfg->num_features);
         delete p;
@@ -101,7 +105,10 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
         p->sift_pk.resize((size_t)sift_k * sift_k);
         sift_windows(desc->ps, sift_k, p->sift_gk.data(), p->sift_pk.data());
     }
-    p->M = shape ? (int)(1.5 * cfg->num_features) : cfg->num_features;  // SparseImgRepresenter.py:192-194
+    p->th_mode = th_mode;
+    p->th = th_mode ? th : 0.f;
+    // SparseImgRepresenter.py:192-194; threshold mode keeps every candidate, so the prefilter is the capacity C itself
+    p->M = (shape && !th_mode) ? (int)(1.5 * cfg->num_features) : cfg->num_features;
     p->cand_cap = cfg->cand_cap > 0 ? cfg->cand_cap : (cfg->H * cfg->W) / 8;
     if (p->cand_cap < p->M) p->cand_cap = p->M;
     const size_t B = cfg->B, M = shape ? p->M : 0, K = cfg->num_features;
@@ -136,6 +143,8 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
     p->off_A2 = take(aff_chain ? sizeof(float) * B * M * 4 : 0);
     p->off_base2 = take(aff_chain ? sizeof(float) * B * M * 4 : 0);
     p->off_lafsw = take(aff_chain ? sizeof(float) * B * M * 6 : 0);
+    p->sel_bytes = th_mode ? ag_select_all_workspace_bytes(&p->plan, p->cand_cap) : 0;
+    p->off_sel = take(p->sel_bytes);
     p->total = o;
     p->launches = 0;
     *out = p;
@@ -152,17 +161,22 @@ int ag_pipeline_create(const ag_pipeline_config_t* cfg, const ag_net_t* affnet, 
     AG_REQUIRE(cfg && affnet && hardnet && out, "NULL argument");
     AG_REQUIRE(!cfg->do_ori || orinet, "do_ori needs an OriNet");
     const ag_pipeline_estimators_t est = {AG_SHAPE_AFFNET, 1, 0, cfg->do_ori ? AG_ORI_ORINET : AG_ORI_NONE, 0};
-    return pipeline_create(__func__, cfg, &est, &HARDNET_DESC, affnet, orinet, hardnet, out);
+    return pipeline_create(__func__, cfg, &est, &HARDNET_DESC, affnet, orinet, hardnet, false, 0.f, out);
 }
 
 int ag_pipeline_create_ex(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_net_t* affnet,
                           const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
-    return pipeline_create(__func__, cfg, est, &HARDNET_DESC, affnet, orinet, hardnet, out);
+    return pipeline_create(__func__, cfg, est, &HARDNET_DESC, affnet, orinet, hardnet, false, 0.f, out);
 }
 
 int ag_pipeline_create_desc(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
                             const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
-    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, out);
+    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, false, 0.f, out);
+}
+
+int ag_pipeline_create_th(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
+                          float th, const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
+    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, true, th, out);
 }
 
 void ag_pipeline_destroy(ag_pipeline_t* p) { delete p; }
@@ -192,13 +206,24 @@ int ag_pipeline_run(ag_pipeline_t* p, const float* d_img, void* d_ws, size_t ws_
     ag_detect_ws_t det;
     if ((rc = ag_detect_ws_carve(&p->plan, p->cand_cap, ws + p->off_det, &det))) return rc;
     if ((rc = ag_pyramid_build(&p->plan, d_img, pyr, stream))) return rc;
-    if ((rc = ag_detect(&p->plan, pyr, 0.f, (int)c.mrSize, &det, stream))) return rc;
+    if ((rc = ag_detect(&p->plan, pyr, p->th, (int)c.mrSize, &det, stream))) return rc;
     const ag_pipeline_estimators_t& e = p->est;
+    void* sel = ws + p->off_sel;
     if (e.shape == AG_SHAPE_NONE) {
         // num_Baum_iters = 0: K keypoints straight from the detector, no shape filter (SparseImgRepresenter.py:192-200)
-        if ((rc = ag_select_keypoints(&p->plan, &det, K, (float)c.mrSize, K, d_resp, lafs2, oct2, lvl2, d_count, stream))) return rc;
+        if (p->th_mode) {
+            if ((rc = ag_select_all_keypoints(&p->plan, &det, (float)c.mrSize, K, sel, p->sel_bytes, d_resp, lafs2, oct2, lvl2, d_count, stream)))
+                return rc;
+        } else if ((rc = ag_select_keypoints(&p->plan, &det, K, (float)c.mrSize, K, d_resp, lafs2, oct2, lvl2, d_count, stream))) {
+            return rc;
+        }
     } else {
-        if ((rc = ag_select_keypoints(&p->plan, &det, M, (float)c.mrSize, M, resp1, lafs1, oct1, lvl1, cnt1, stream))) return rc;
+        if (p->th_mode) {
+            if ((rc = ag_select_all_keypoints(&p->plan, &det, (float)c.mrSize, M, sel, p->sel_bytes, resp1, lafs1, oct1, lvl1, cnt1, stream)))
+                return rc;
+        } else if ((rc = ag_select_keypoints(&p->plan, &det, M, (float)c.mrSize, M, resp1, lafs1, oct1, lvl1, cnt1, stream))) {
+            return rc;
+        }
         // affine shape: base_A of getAffineShape's loop (SparseImgRepresenter.py:127-141) into A
         if (e.shape == AG_SHAPE_BAUMBERG) {
             if ((rc = baumberg_pyr(&p->plan, pyr, lafs1, oct1, lvl1, cnt1, M, e.shape_ps, e.num_baum_iters, p->shape_gk.data(), A, stream)))
@@ -227,7 +252,12 @@ int ag_pipeline_run(ag_pipeline_t* p, const float* d_img, void* d_ws, size_t ws_
                 if (it != it_n - 1 && (rc = ag_lafs_left_multiply(base, lafs1, lafsw, n, stream))) return rc;
             }
         }
-        if ((rc = ag_affine_shape_filter(A, resp1, lafs1, oct1, lvl1, cnt1, B, M, K, K, d_resp, lafs2, oct2, lvl2, d_count, stream))) return rc;
+        if (p->th_mode) {
+            // num_features <= 0: every survivor in order (SparseImgRepresenter.py:151-156); M = K = C
+            if ((rc = ag_affine_shape_filter_all(A, resp1, lafs1, oct1, lvl1, cnt1, B, M, d_resp, lafs2, oct2, lvl2, d_count, stream))) return rc;
+        } else if ((rc = ag_affine_shape_filter(A, resp1, lafs1, oct1, lvl1, cnt1, B, M, K, K, d_resp, lafs2, oct2, lvl2, d_count, stream))) {
+            return rc;
+        }
     }
     if (e.ori == AG_ORI_ORINET) {
         if ((rc = ag_net_forward_pyr(p->ori, &p->plan, pyr, lafs2, oct2, lvl2, d_count, K, A, netws, p->net_bytes, stream))) return rc;

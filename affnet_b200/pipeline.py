@@ -47,12 +47,16 @@ def descriptor(HardNet):
 
 class DetectDescribePipeline:
     def __init__(self, B, H, W, AffNet, HardNet, OriNet=None, num_features=2000, border=5, mrSize=5.192, nlevels=3,
-                 init_sigma=1.6, do_ori=True, cand_cap=0, device="cuda", outputs=None, num_Baum_iters=1):
+                 init_sigma=1.6, do_ori=True, cand_cap=0, device="cuda", outputs=None, num_Baum_iters=1, th=None):
         """outputs: optional list of (lafs [B,K,2,3], desc [B,K,128], count [B] int32) CUDA tensors, one tuple per output slot, that the
         kernels write into directly (e.g. DescriptorExchange.outputs(): the blocks an all-gather sends); default: one private slot.
         AffNet / OriNet / do_ori / num_Baum_iters select the estimators as ScaleSpaceAffinePatchExtractor does (see `estimators`):
         e.g. AffNet=AffineShapeEstimator(19), num_Baum_iters=16 is the HesAff baseline, num_Baum_iters=0 the plain detector.
-        HardNet may be a SIFTNet: the descriptors are then SIFTNet's at its patch size and clipval, and no checkpoint is needed."""
+        HardNet may be a SIFTNet: the descriptors are then SIFTNet's at its patch size and clipval, and no checkpoint is needed.
+        th: the reference's threshold mode (ScaleSpaceAffinePatchExtractor(th=th): -1 in hesaffnet.py, 28.41 its HessianAffine default):
+        every keypoint above th is kept in (octave, level, raster) order, with no top-K, and num_features is the per-image capacity C of
+        the outputs [B,C,..]; an image with more keypoints than C gets count -1 (see check())."""
+        self.th = None if th is None else float(th)
         self.cfg = L.PipelineConfig(B, H, W, num_features, nlevels, border, float(init_sigma), float(mrSize), 1 if do_ori else 0, cand_cap)
         self.est, aff, ori = estimators(AffNet, OriNet, do_ori, num_Baum_iters)
         self.desc_cfg, hard = descriptor(HardNet)
@@ -89,7 +93,11 @@ class DetectDescribePipeline:
             L.lib().ag_pipeline_destroy(self._h)
             self._h = None
         h = C.c_void_p()
-        L.check(L.lib().ag_pipeline_create_desc(C.byref(self.cfg), C.byref(self.est), C.byref(self.desc_cfg), hs[0], hs[1], hs[2], C.byref(h)))
+        if self.th is None:
+            L.check(L.lib().ag_pipeline_create_desc(C.byref(self.cfg), C.byref(self.est), C.byref(self.desc_cfg), hs[0], hs[1], hs[2], C.byref(h)))
+        else:
+            L.check(L.lib().ag_pipeline_create_th(C.byref(self.cfg), C.byref(self.est), C.byref(self.desc_cfg), self.th, hs[0], hs[1], hs[2],
+                                                  C.byref(h)))
         self._h, self._net_handles, self._graph = h, hs, None
 
     def _nets_current(self):
@@ -119,9 +127,12 @@ class DetectDescribePipeline:
         return lafs, resp, desc, count
 
     def check(self):
-        """Synchronises and raises if any image overflowed the candidate capacity (count == -1)."""
+        """Synchronises and raises if any image overflowed a capacity (count == -1)."""
         if any(bool((c < 0).any().item()) for (_, _, _, c) in self._slots):
-            raise L.AffnetB200Error("candidate capacity exceeded: construct the pipeline with a larger cand_cap")
+            if self.th is None:
+                raise L.AffnetB200Error("candidate capacity exceeded: construct the pipeline with a larger cand_cap")
+            raise L.AffnetB200Error("capacity exceeded in threshold mode: an image has more candidates than cand_cap or more keypoints above "
+                                    "th than num_features = %d; construct the pipeline with a larger cand_cap or num_features" % self.K)
         return self
 
     def capture(self):

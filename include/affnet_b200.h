@@ -130,6 +130,20 @@ int ag_select_keypoints(const ag_pyramid_plan_t* plan, const ag_detect_ws_t* ws,
                         int out_cap, float* d_resp, float* d_lafs, int* d_oct, int* d_lvl, int* d_count,
                         void* stream);
 
+/* Ordered keep-all selection at any count (threshold mode, SparseImgRepresenter.py:104-110 with num = -1): for each image, every candidate of
+ * the accepted levels (more than one positive response) in (octave, level, raster) order, the A part of the LAF scaled by a_scale.  The
+ * rows equal ag_select_keypoints(num_features <= 0, out_cap >= their number) bit for bit, and there is no 16384 limit: a bitmap over the
+ * detection levels' pixels and per-word popcount prefixes give each candidate its row, without a sort.
+ * d_count[b] = -1 when image b's candidate list overflowed ws->cand_cap or when it has more than out_cap keypoints; nothing of such an
+ * image is written.  Rows at or beyond d_count[b] are never written.
+ * d_scratch: ag_select_all_workspace_bytes(plan, ws->cand_cap) bytes, 256-B aligned, any content (about B * 8 bytes per 32 pixels of
+ * every detection level: the size is set by the pyramid, cand_cap only has to be positive).  A memset and four launches, deterministic,
+ * no host synchronisation (CUDA-graph capturable).  AG_ERR_CAPACITY for a smaller scratch, before any CUDA call. */
+size_t ag_select_all_workspace_bytes(const ag_pyramid_plan_t* plan, int cand_cap);
+int ag_select_all_keypoints(const ag_pyramid_plan_t* plan, const ag_detect_ws_t* ws, float a_scale, int out_cap,
+                            void* d_scratch, size_t scratch_bytes, float* d_resp, float* d_lafs, int* d_oct, int* d_lvl,
+                            int* d_count, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Affine bilinear sampler          replaces extract_patches / generate_patch_grid_from_normalized_LAFs
  *                                  (LAF.py:313-372) and extract_patches_from_pyramid_with_inv_index
@@ -232,6 +246,13 @@ int ag_affine_shape_filter(const float* d_A, const float* d_resp, const float* d
                            const int* d_lvl, const int* d_count_in, int B, int cap, int num_features, int out_cap,
                            float* d_resp_out, float* d_lafs_out, int* d_oct_out, int* d_lvl_out, int* d_count_out,
                            void* stream);
+/* Keep-all shape filter at any cap (getAffineShape's num_features <= 0 branch, SparseImgRepresenter.py:151-156): every survivor of image b
+ * in index order with its response unchanged, written to rows 0 .. d_count_out[b]-1 of [B,cap..] outputs.  Bit-identical to
+ * ag_affine_shape_filter(num_features = 0, out_cap = cap) wherever that accepts the call (same device arithmetic), with no cap limit and
+ * no workspace.  d_count_out[b] = -1 where d_count_in[b] < 0; a count above cap is read as cap.  One launch. */
+int ag_affine_shape_filter_all(const float* d_A, const float* d_resp, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                               const int* d_count_in, int B, int cap, float* d_resp_out, float* d_lafs_out, int* d_oct_out,
+                               int* d_lvl_out, int* d_count_out, void* stream);
 
 /* LAF_A <- LAF_A * R  then (optionally) denormalise to pixels of a WxH image.  d_lafs [n,2,3] in/out. */
 int ag_lafs_apply_rotation(float* d_lafs, const float* d_R, int n, void* stream);
@@ -406,6 +427,16 @@ typedef struct {
 } ag_pipeline_descriptor_t;
 int ag_pipeline_create_desc(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
                             const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
+/* Threshold mode (ScaleSpaceAffinePatchExtractor(th = th), SparseImgRepresenter.py:33-37; the reference's hesaffnet.py runs th = -1, its
+ * HessianAffine default is 28.41): the detector subtracts th from the Hessian response, every candidate of the accepted levels is kept
+ * in (octave, level, raster) order (ag_select_all_keypoints), and with a shape step every survivor of the shape filter in that order
+ * (ag_affine_shape_filter_all): there is no top-K.  cfg->num_features is the per-image keypoint capacity C (>= 1, no 16384 limit): the
+ * prefilter and the outputs hold C rows, and an image with more than C accepted candidates gets count -1, as a candidate-list overflow
+ * does.  Estimators and descriptor as ag_pipeline_create_desc.  The workspace is that formula with M = K = C plus the selection's scratch:
+ * the net share grows by about 256 KB per HardNet row, so B x C decides the cost (2 x 32768 rows: about 16 GB).
+ * AG_ERR_INVALID (before any CUDA call) for th NaN or infinite and for everything ag_pipeline_create_desc refuses except its K limits. */
+int ag_pipeline_create_th(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
+                          float th, const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
 void ag_pipeline_destroy(ag_pipeline_t* p);
 size_t ag_pipeline_workspace_bytes(const ag_pipeline_t* p);
 const ag_pyramid_plan_t* ag_pipeline_plan(const ag_pipeline_t* p);
