@@ -17,11 +17,13 @@ __device__ __forceinline__ float warp_sum_f(float v) {
 }
 
 // OrientationDetector.forward on the PS x PS patch `p` (shared memory) of one warp; s_w [PS*PS], s_b [PS*PS], s_h [40] are the warp's
-// scratch.  Returns the angle on every lane.
+// scratch.  Returns the angle on every lane.  A non-finite weight (a NaN or infinite pixel, or gx^2 + gy^2 overflowing) gives bin 0, the
+// angle pi: the reference multiplies it by the 0 of every other bin's mask, so every smoothed bin is NaN and torch's max returns index 0.
 __device__ __forceinline__ float orientation_hist_warp(const float* p, int PS, const float* gk, float* s_w, unsigned char* s_b, float* s_h,
                                                        int lane) {
     const int NP = PS * PS;
     const float PI_F = 3.14159265358979323846f;
+    bool nonfinite = false;
     for (int i = lane; i < NP; i += 32) {
         float gx, gy;
         grad_at(p, PS, i / PS, i % PS, 0.5f, -0.5f, gx, gy);   // weights (0.5, 0, -0.5): 0.5*x[j-1] - 0.5*x[j+1]
@@ -32,8 +34,11 @@ __device__ __forceinline__ float orientation_hist_warp(const float* p, int PS, c
         const float wo1 = __fsub_rn(o_big, bo0);
         bo0 = fmodf(bo0, 36.0f);
         s_b[i] = (unsigned char)(int)bo0;
-        s_w[i] = __fmul_rn(__fsub_rn(1.0f, wo1), mag);   // only the lower-bin weight is accumulated (as the reference does)
+        const float w = __fmul_rn(__fsub_rn(1.0f, wo1), mag);   // only the lower-bin weight is accumulated (as the reference does)
+        s_w[i] = w;
+        nonfinite |= !isfinite(w);
     }
+    nonfinite = __any_sync(0xffffffffu, nonfinite);
     __syncwarp();
     // deterministic histogram: lane b sums bin b (and b+32) over all pixels in raster order
     for (int b = lane; b < 36; b += 32) {
@@ -56,10 +61,15 @@ __device__ __forceinline__ float orientation_hist_warp(const float* p, int PS, c
         const int oi = __shfl_xor_sync(0xffffffffu, bidx, o);
         if (ov > best || (ov == best && oi < bidx)) { best = ov; bidx = oi; }
     }
+    if (nonfinite) bidx = 0;
     return -__fsub_rn(__fdiv_rn(__fmul_rn(2.0f * PI_F, (float)bidx), 36.0f), PI_F);
 }
 
 // AffineShapeEstimator.forward on the PS x PS patch `p` (shared memory) of one warp -> up-is-up rectified A, on every lane.
+// Every fp32 operation is rounded on its own, in the left-to-right order of the reference's torch expressions (no fused multiply-adds),
+// so the result is a function of the patch alone: tests/handcrafted_restated.py states the same arithmetic.  The moments are summed
+// per lane over i = lane, lane + 32, ... and then by the xor butterfly of warp_sum_f.  A flat patch, a ramp along one axis or a
+// non-finite pixel gives NaN in all four entries, as in the reference (A[0,1] is 0 * det there).
 __device__ __forceinline__ void baumberg_warp(const float* p, int PS, const float* gk, int lane, float (&A)[4]) {
     const int NP = PS * PS;
     float a = 0.f, b = 0.f, c = 0.f;
@@ -67,30 +77,35 @@ __device__ __forceinline__ void baumberg_warp(const float* p, int PS, const floa
         float gx, gy;
         grad_at(p, PS, i / PS, i % PS, -1.0f, 1.0f, gx, gy);   // weights (-1, 0, 1)
         const float g = gk[i];
-        a += gx * gx * g; b += gx * gy * g; c += gy * gy * g;
+        a = __fadd_rn(a, __fmul_rn(__fmul_rn(gx, gx), g));
+        b = __fadd_rn(b, __fmul_rn(__fmul_rn(gx, gy), g));
+        c = __fadd_rn(c, __fmul_rn(__fmul_rn(gy, gy), g));
     }
-    a = warp_sum_f(a) / (float)NP; b = warp_sum_f(b) / (float)NP; c = warp_sum_f(c) / (float)NP;
+    a = __fdiv_rn(warp_sum_f(a), (float)NP); b = __fdiv_rn(warp_sum_f(b), (float)NP); c = __fdiv_rn(warp_sum_f(c), (float)NP);
     // invSqrt (HandCraftedModules.py:94-117)
     const float eps = 1e-12f;
     const float mask = (b != 0.f) ? 1.f : 0.f;
-    const float r1 = mask * (c - a) / (2.f * b + eps);
-    const float sgn = (r1 > 0.f) ? 1.f : ((r1 < 0.f) ? -1.f : 0.f);
-    const float t1 = sgn / (fabsf(r1) + sqrtf(1.f + r1 * r1));
-    float r = 1.0f / sqrtf(1.f + t1 * t1);
-    float t = t1 * r;
-    r = r * mask + 1.0f * (1.0f - mask);
-    t = t * mask;
-    float x = 1.f / sqrtf(r * r * a - 2.0f * r * t * b + t * t * c);
-    float z = 1.f / sqrtf(t * t * a + 2.0f * r * t * b + r * r * c);
-    const float d = sqrtf(x * z);
-    x = x / d; z = z / d;
-    const float na = r * r * x + t * t * z, nb = -r * t * x + t * r * z, nc = t * t * x + r * r * z;
+    const float r1 = __fdiv_rn(__fmul_rn(mask, __fsub_rn(c, a)), __fadd_rn(__fmul_rn(2.f, b), eps));
+    const float sgn = (r1 > 0.f) ? 1.f : ((r1 < 0.f) ? -1.f : 0.f);   // torch.sign: 0 for +-0 and NaN
+    const float t1 = __fdiv_rn(sgn, __fadd_rn(fabsf(r1), __fsqrt_rn(__fadd_rn(1.f, __fmul_rn(r1, r1)))));
+    float r = __fdiv_rn(1.f, __fsqrt_rn(__fadd_rn(1.f, __fmul_rn(t1, t1))));
+    float t = __fmul_rn(t1, r);
+    r = __fadd_rn(__fmul_rn(r, mask), __fsub_rn(1.f, mask));   // r * mask + 1.0 * (1.0 - mask); 1.0 * y == y
+    t = __fmul_rn(t, mask);
+    const float rr = __fmul_rn(r, r), tt = __fmul_rn(t, t), rt2 = __fmul_rn(__fmul_rn(2.f, r), t);
+    float x = __fdiv_rn(1.f, __fsqrt_rn(__fadd_rn(__fsub_rn(__fmul_rn(rr, a), __fmul_rn(rt2, b)), __fmul_rn(tt, c))));
+    float z = __fdiv_rn(1.f, __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(tt, a), __fmul_rn(rt2, b)), __fmul_rn(rr, c))));
+    const float d = __fsqrt_rn(__fmul_rn(x, z));
+    x = __fdiv_rn(x, d); z = __fdiv_rn(z, d);
+    const float na = __fadd_rn(__fmul_rn(rr, x), __fmul_rn(tt, z));
+    const float nb = __fadd_rn(__fmul_rn(__fmul_rn(-r, t), x), __fmul_rn(__fmul_rn(t, r), z));
+    const float nc = __fadd_rn(__fmul_rn(tt, x), __fmul_rn(rr, z));
     // abc2A + rectifyAffineTransformationUpIsUp (LAF.py:285-291)
     const float a00 = na, a01 = nb, a10 = nb, a11 = nc;
-    const float det = sqrtf(fabsf(a00 * a11 - a10 * a01 + 1e-10f));
-    const float b2a2 = sqrtf(a01 * a01 + a00 * a00);
-    A[0] = b2a2 / det; A[1] = 0.f;
-    A[2] = (a11 * a01 + a10 * a00) / (b2a2 * det); A[3] = det / b2a2;
+    const float det = __fsqrt_rn(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(a00, a11), __fmul_rn(a10, a01)), 1e-10f)));
+    const float b2a2 = __fsqrt_rn(__fadd_rn(__fmul_rn(a01, a01), __fmul_rn(a00, a00)));
+    A[0] = __fdiv_rn(b2a2, det); A[1] = __fmul_rn(0.f, det);
+    A[2] = __fdiv_rn(__fadd_rn(__fmul_rn(a11, a01), __fmul_rn(a10, a00)), __fmul_rn(b2a2, det)); A[3] = __fdiv_rn(det, b2a2);
 }
 
 __global__ void __launch_bounds__(HC_WARPS * 32) orientation_hist_kernel(const float* __restrict__ patches, int n, int PS, const float* __restrict__ gk,
@@ -259,6 +274,16 @@ int baumberg_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float*
     return launch_hc_pyr(false, plan, d_pyr, d_lafs, d_oct, d_lvl, d_count, cap, PS, iters, gk, d_A, (cudaStream_t)stream);
 }
 
+// The device libm calls of the estimators, one element per thread, compiled with this file's flags (ag_debug_libm).
+__global__ void libm_probe_kernel(const float* __restrict__ y, const float* __restrict__ x, int n, float* __restrict__ at,
+                                  float* __restrict__ co, float* __restrict__ si) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    at[i] = atan2f(y[i], x[i]);
+    co[i] = cosf(x[i]);
+    si[i] = sinf(x[i]);
+}
+
 }  // namespace ag
 
 using namespace ag;
@@ -301,6 +326,24 @@ int ag_baumberg_shape(const float* d_patches, int n, int PS, const float* d_gk, 
     baumberg_kernel<<<cdiv(n, HC_WARPS), HC_WARPS * 32, 0, (cudaStream_t)stream>>>(d_patches, n, PS, d_gk, d_A);
     AG_CHECK_LAUNCH("baumberg_kernel");
     return AG_OK;
+}
+
+int ag_debug_libm(const float* d_y, const float* d_x, int n, float* d_atan2, float* d_cos, float* d_sin, void* stream) {
+    AG_REQUIRE(d_y && d_x && d_atan2 && d_cos && d_sin, "NULL argument");
+    if (n <= 0) return AG_OK;
+    libm_probe_kernel<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(d_y, d_x, n, d_atan2, d_cos, d_sin);
+    AG_CHECK_LAUNCH("libm_probe_kernel");
+    return AG_OK;
+}
+
+int ag_debug_orientation_hist_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                                  const int* d_count, int cap, int PS, const float* h_gk, float* d_R, void* stream) {
+    return launch_hc_pyr(true, plan, d_pyr, d_lafs, d_oct, d_lvl, d_count, cap, PS, 1, h_gk, d_R, (cudaStream_t)stream);
+}
+
+int ag_debug_baumberg_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                          const int* d_count, int cap, int PS, int iters, const float* h_gk, float* d_A, void* stream) {
+    return launch_hc_pyr(false, plan, d_pyr, d_lafs, d_oct, d_lvl, d_count, cap, PS, iters, h_gk, d_A, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -37,7 +37,9 @@ __device__ __forceinline__ float block_sum_128(float v, float* s_red) {
     return (s_red[0] + s_red[1]) + (s_red[2] + s_red[3]);   // a fixed order: every thread gets the same bits
 }
 
-// SIFTNet.forward on the PS x PS patch `p` (shared memory, complete on entry) -> out[0..127] in [bin][cy][cx] order.
+// SIFTNet.forward on the PS x PS patch `p` (shared memory, complete on entry) -> out[0..127] in [bin][cy][cx] order.  A non-finite bin
+// weight (a NaN or infinite pixel, or gx^2 + gy^2 overflowing) at a pixel the pooling reads makes all 128 outputs NaN, as in the
+// reference: it multiplies that weight by the 0 of every other bin's mask, and the NaN reaches every output through the L2 norms.
 __device__ __forceinline__ void sift_block(const SiftParams& P, float* p, float* out) {
     const int PS = P.PS, NP = PS * PS;
     float* s_w0 = p + NP;
@@ -45,19 +47,24 @@ __device__ __forceinline__ void sift_block(const SiftParams& P, float* p, float*
     float* s_red = s_w1 + NP;
     unsigned char* s_b = (unsigned char*)(s_red + 4);
     const float TWO_PI_F = 6.28318530717958647692f;
+    const int pooled = 3 * P.s + P.k;   // the four windows of a row / column cover [0, 3 s + k)
+    int nonfinite = 0;
     for (int t = threadIdx.x; t < NP; t += SIFT_THREADS) {
         float gx, gy;
-        grad_at(p, PS, t / PS, t % PS, -1.0f, 1.0f, gx, gy);   // weights (-1, 0, 1), replicate padding
+        const int ti = t / PS, tj = t % PS;
+        grad_at(p, PS, ti, tj, -1.0f, 1.0f, gx, gy);   // weights (-1, 0, 1), replicate padding
         const float mag = __fmul_rn(__fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), 1e-10f)), P.gk[t]);
         const float ori = atan2f(gy, __fadd_rn(gx, 1e-8f));
         const float o_big = __fmul_rn(__fdiv_rn(__fadd_rn(ori, TWO_PI_F), TWO_PI_F), 8.0f);
         const float bo0 = floorf(o_big);
         const float wo1 = __fsub_rn(o_big, bo0);
         s_b[t] = (unsigned char)((int)bo0 & 7);                 // floor(o) % 8; the upper bin is (bo0 + 1) % 8
-        s_w0[t] = __fmul_rn(__fsub_rn(1.0f, wo1), mag);
-        s_w1[t] = __fmul_rn(wo1, mag);
+        const float w0 = __fmul_rn(__fsub_rn(1.0f, wo1), mag), w1 = __fmul_rn(wo1, mag);
+        s_w0[t] = w0;
+        s_w1[t] = w1;
+        nonfinite |= (ti < pooled) & (tj < pooled) & !(isfinite(w0) & isfinite(w1));
     }
-    __syncthreads();
+    nonfinite = __syncthreads_or(nonfinite);
     // the k x k pooling of angle bin `bin` over the window of cell (cy, cx), stride s, no padding
     const int bin = threadIdx.x & 7, cell = threadIdx.x >> 3, cy = cell >> 2, cx = cell & 3;
     const int k = P.k, base = cy * P.s * PS + cx * P.s;
@@ -74,7 +81,7 @@ __device__ __forceinline__ void sift_block(const SiftParams& P, float* p, float*
     float x = __fdiv_rn(acc, __fsqrt_rn(__fadd_rn(fabsf(block_sum_128(__fmul_rn(acc, acc), s_red)), 1e-10f)));
     x = fminf(fmaxf(x, 0.f), P.clip);
     x = __fdiv_rn(x, __fsqrt_rn(__fadd_rn(fabsf(block_sum_128(__fmul_rn(x, x), s_red)), 1e-10f)));
-    out[bin * 16 + cell] = x;
+    out[bin * 16 + cell] = nonfinite ? __int_as_float(0x7fffffff) : x;
 }
 
 __global__ void __launch_bounds__(SIFT_THREADS) sift_kernel(const __grid_constant__ SiftParams P) {

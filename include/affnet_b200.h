@@ -199,6 +199,18 @@ int ag_debug_pyramid_mode(int fused);
 /* Developer diagnostic: run the second-generation trunk on materialised patches [n,32,32] up to conv layer `upto` (2..5) and decode
  * that layer's activations (fp16 hi [+ lo] planes in the engine's HBM layout) to fp32 [n,C,H,H].  d_ws: ag_net_workspace_bytes(). */
 int ag_debug_tcx_layer(const ag_net_t* net, const float* d_patches, int n, int upto, float* d_out, void* d_ws, size_t ws_bytes, void* stream);
+/* Developer diagnostic: the device libm calls of the hand-crafted estimators, compiled with their flags, one element per thread:
+ * d_atan2[i] = atan2f(d_y[i], d_x[i]), d_cos[i] = cosf(d_x[i]), d_sin[i] = sinf(d_x[i]) for i < n.  Lets a test restate the estimators
+ * bit for bit (tests/handcrafted_restated.py); not used by the pipeline. */
+int ag_debug_libm(const float* d_y, const float* d_x, int n, float* d_atan2, float* d_cos, float* d_sin, void* stream);
+/* Developer diagnostic: the batched pipeline's fused hand-crafted estimators called directly (same layout as ag_extract_patches_pyr;
+ * d_count [B] required; h_gk [PS,PS] in host memory, 3 <= PS <= 41).  Rows at or beyond d_count[b] are not written.
+ *   ag_debug_orientation_hist_pyr  d_R [B,cap,2,2] = [[cos, sin], [-sin, cos]] of the gradient-histogram angle of each sampled patch
+ *   ag_debug_baumberg_pyr          d_A [B,cap,2,2] = base_A after `iters` >= 1 Baumberg iterations (SparseImgRepresenter.py:127-141) */
+int ag_debug_orientation_hist_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                                  const int* d_count, int cap, int PS, const float* h_gk, float* d_R, void* stream);
+int ag_debug_baumberg_pyr(const ag_pyramid_plan_t* plan, const float* d_pyr, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                          const int* d_count, int cap, int PS, int iters, const float* h_gk, float* d_A, void* stream);
 /* Scratch bytes for a forward over n patches. */
 size_t ag_net_workspace_bytes(int kind, int n);
 

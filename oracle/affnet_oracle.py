@@ -328,11 +328,12 @@ def _trunk(x, sd, cfg):
 
 
 def rectify_up_is_up(A):
-    """LAF.py:285-291."""
+    """LAF.py:285-291 (A[0,1] is 0 * det there: NaN when det is not finite)."""
     det = torch.sqrt(torch.abs(A[:, 0, 0] * A[:, 1, 1] - A[:, 1, 0] * A[:, 0, 1] + 1e-10))
     b2a2 = torch.sqrt(A[:, 0, 1] * A[:, 0, 1] + A[:, 0, 0] * A[:, 0, 0])
     out = torch.zeros_like(A)
     out[:, 0, 0] = b2a2 / det
+    out[:, 0, 1] = 0 * det
     out[:, 1, 0] = (A[:, 1, 1] * A[:, 0, 1] + A[:, 1, 0] * A[:, 0, 0]) / (b2a2 * det)
     out[:, 1, 1] = det / b2a2
     return out
