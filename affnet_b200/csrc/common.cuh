@@ -222,5 +222,14 @@ __device__ __forceinline__ void laf_left_mul(const float (&a)[4], const float (&
     o[0] = dot2_rn(a[0], l[0], a[1], l[3]); o[1] = dot2_rn(a[0], l[1], a[1], l[4]); o[2] = l[2];
     o[3] = dot2_rn(a[2], l[0], a[3], l[3]); o[4] = dot2_rn(a[2], l[1], a[3], l[4]); o[5] = l[5];
 }
+// rectifyAffineTransformationUpIsUp (LAF.py:285-291) of [[a00, a01], [a10, a11]] -> A[4], each torch operation one fp32 operation in
+// the expression's left-to-right order (no contraction); A[0,1] = 0 * det as in the reference (NaN when det is).  Shared by the
+// Baumberg estimator and the AffNet heads, and restated by tests/handcrafted_restated.py and tests/nets_restated.py.
+__device__ __forceinline__ void rectify_up_is_up(float a00, float a01, float a10, float a11, float* A) {
+    const float det = __fsqrt_rn(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(a00, a11), __fmul_rn(a10, a01)), 1e-10f)));
+    const float b2a2 = __fsqrt_rn(__fadd_rn(__fmul_rn(a01, a01), __fmul_rn(a00, a00)));
+    A[0] = __fdiv_rn(b2a2, det); A[1] = __fmul_rn(0.f, det);
+    A[2] = __fdiv_rn(__fadd_rn(__fmul_rn(a11, a01), __fmul_rn(a10, a00)), __fmul_rn(b2a2, det)); A[3] = __fdiv_rn(det, b2a2);
+}
 
 }  // namespace ag

@@ -101,11 +101,7 @@ __device__ __forceinline__ void baumberg_warp(const float* p, int PS, const floa
     const float nb = __fadd_rn(__fmul_rn(__fmul_rn(-r, t), x), __fmul_rn(__fmul_rn(t, r), z));
     const float nc = __fadd_rn(__fmul_rn(tt, x), __fmul_rn(rr, z));
     // abc2A + rectifyAffineTransformationUpIsUp (LAF.py:285-291)
-    const float a00 = na, a01 = nb, a10 = nb, a11 = nc;
-    const float det = __fsqrt_rn(fabsf(__fadd_rn(__fsub_rn(__fmul_rn(a00, a11), __fmul_rn(a10, a01)), 1e-10f)));
-    const float b2a2 = __fsqrt_rn(__fadd_rn(__fmul_rn(a01, a01), __fmul_rn(a00, a00)));
-    A[0] = __fdiv_rn(b2a2, det); A[1] = __fmul_rn(0.f, det);
-    A[2] = __fdiv_rn(__fadd_rn(__fmul_rn(a11, a01), __fmul_rn(a10, a00)), __fmul_rn(b2a2, det)); A[3] = __fdiv_rn(det, b2a2);
+    rectify_up_is_up(na, nb, nb, nc, A);
 }
 
 __global__ void __launch_bounds__(HC_WARPS * 32) orientation_hist_kernel(const float* __restrict__ patches, int n, int PS, const float* __restrict__ gk,

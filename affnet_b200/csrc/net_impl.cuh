@@ -29,6 +29,7 @@ struct ag_net {
     __half* d_headh;   // head for the tensor-core GEMM, k = (pixel*C/8 + c/8)*8 + c%8: HardNet fp16 [8192/8][128][8]; AffNet / OriNet [4096/8][32 hi | 32 lo][8]
     float* d_head_w;   // AffNet [3][4096], OriNet w_eff[4096][18] (per-position shifted copies), HardNet [8192][128]
     float* d_head_b;   // AffNet bias[3], OriNet bias[2], HardNet {scale[128], shift[128]}
+    float* d_head_bx;  // HardNet fp16 tensor-core head: {scale[128] / the power-of-two scale of d_headh, shift[128]}
     float w_inv_scale[6];   // tensor-core layers: 1 / (power-of-two scale of d_wh[l]); [0] = layer 1 (scaled in the kernel)
     float head_inv_scale;   // AffNet / OriNet tensor-core head: 1 / (power-of-two scale of d_headh)
     float* d_all;      // fp32 allocation

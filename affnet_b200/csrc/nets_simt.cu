@@ -167,12 +167,8 @@ __global__ void affnet_head_kernel(const float* __restrict__ feat, const float* 
     }
     s0 = warp_sum(s0); s1 = warp_sum(s1); s2 = warp_sum(s2);
     if (lane == 0) {
-        const float a00 = 1.0f + tanhf(s0 + bias[0]), a01 = 0.f, a10 = tanhf(s1 + bias[1]), a11 = 1.0f + tanhf(s2 + bias[2]);
-        const float det = sqrtf(fabsf(a00 * a11 - a10 * a01 + 1e-10f));
-        const float b2a2 = sqrtf(a01 * a01 + a00 * a00);
-        float* o = out + (size_t)pi * 4;
-        o[0] = b2a2 / det; o[1] = 0.f;
-        o[2] = (a11 * a01 + a10 * a00) / (b2a2 * det); o[3] = det / b2a2;
+        const float a00 = 1.0f + tanhf(s0 + bias[0]), a10 = tanhf(s1 + bias[1]), a11 = 1.0f + tanhf(s2 + bias[2]);
+        rectify_up_is_up(a00, 0.f, a10, a11, out + (size_t)pi * 4);
     }
 }
 
@@ -433,7 +429,7 @@ int ag_net_create(int kind, const float* h_blob, size_t n_floats, ag_net_t** out
                         memcpy(&packed_bf[headbf_off + (((size_t)(pix * 16 + cg)) * 128 + o) * 8 + e], &bv, 2);
                     }
     }
-    size_t headh_off = 0;
+    size_t headh_off = 0, hbx_off = 0;
     float head_scale = 1.0f;
     if (kind == AG_NET_HARDNET) {
         while (packed_h.size() % 8) packed_h.push_back(__float2half_rn(0.f));
@@ -441,11 +437,18 @@ int ag_net_create(int kind, const float* h_blob, size_t n_floats, ag_net_t** out
         packed_h.resize(packed_h.size() + (size_t)8192 * 128);
         __half* dst = packed_h.data() + headh_off;
         const float* hw = packed.data() + hw_off;  // [k = c*64 + p][cout]
+        // times a power of two, as every conv layer: a BatchNorm follows this conv, so a checkpoint's head weights can have any scale, and
+        // below 2^-14 fp16 would keep them as subnormals (head weights near 1e-5 lose 3e-3 of their value, 7e-4 of a descriptor).  The
+        // exact inverse is folded into the BatchNorm scale that tc_head_kernel multiplies by.
+        const float hs = pow2_scale(hw, (size_t)8192 * 128);
         for (int pix = 0; pix < 64; pix++)
             for (int cg = 0; cg < 16; cg++)
                 for (int o = 0; o < 128; o++)
                     for (int e = 0; e < 8; e++)
-                        dst[(((size_t)(pix * 16 + cg)) * 128 + o) * 8 + e] = __float2half_rn(hw[((size_t)(cg * 8 + e) * 64 + pix) * 128 + o]);
+                        dst[(((size_t)(pix * 16 + cg)) * 128 + o) * 8 + e] = __float2half_rn(hs * hw[((size_t)(cg * 8 + e) * 64 + pix) * 128 + o]);
+        hbx_off = packed.size();
+        for (int o = 0; o < 128; o++) packed.push_back(packed[hb_off + o] * (1.0f / hs));
+        for (int o = 0; o < 128; o++) packed.push_back(packed[hb_off + 128 + o]);
     }
     if (kind != AG_NET_HARDNET) {   // AffNet (3 outputs) / OriNet (18 shifted outputs): [4096/8][32 hi rows | 32 lo rows][8]
         const int no = (kind == AG_NET_AFFNET) ? 3 : 18;
@@ -504,6 +507,7 @@ int ag_net_create(int kind, const float* h_blob, size_t n_floats, ag_net_t** out
     net->d_w1 = net->d_w[0];
     net->d_head_w = net->d_all + hw_off;
     net->d_head_b = net->d_all + hb_off;
+    net->d_head_bx = net->d_all + hbx_off;
     *out = net;
     return AG_OK;
 }

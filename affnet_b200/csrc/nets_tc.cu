@@ -108,7 +108,7 @@ int tc_hardnet_head(const ag_net* net, const void* headbuf, int n, int group, co
         if (rc != AG_OK) return rc;
     }
     if (bf16) tc_head_kernel<1><<<(n + 127) / 128, 288, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh_bf, net->d_head_b, out, n, group, count);
-    else tc_head_kernel<0><<<(n + 127) / 128, 288, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh, net->d_head_b, out, n, group, count);
+    else tc_head_kernel<0><<<(n + 127) / 128, 288, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh, net->d_head_bx, out, n, group, count);
     AG_CHECK_LAUNCH("tc_head_kernel");
     return AG_OK;
 }

@@ -92,18 +92,28 @@ static int launch_first(void* out, const __half* w, const float* b, float inv_sc
     return AG_OK;
 }
 
-// debug / test helper: an activation buffer in one of the HBM layouts -> fp32 [n][C][H][H] (hi + lo planes added)
-__global__ void tcx_decode_kernel(const __half* __restrict__ buf, int layout, int C, int osa, int H, int n, float* __restrict__ out) {
+// debug / test helper: an activation buffer in one of the HBM layouts (L_HEAD included) -> fp32 [n][C][H][H] (hi + lo planes added;
+// bf: 16-bit bf16 values)
+__global__ void tcx_decode_kernel(const __half* __restrict__ buf, int layout, int C, int osa, int H, int n, int bf, float* __restrict__ out) {
     const size_t total = (size_t)n * C * H * H;
+    auto val = [&](size_t k) -> float { return bf ? __uint_as_float((uint32_t)__half_as_ushort(buf[k]) << 16) : __half2float(buf[k]); };
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const int x = (int)(i % H), y = (int)((i / H) % H), c = (int)((i / ((size_t)H * H)) % C), pi = (int)(i / ((size_t)H * H * C));
-        const int slots = layout_slots(layout);
-        const size_t unit_halfs = (size_t)(C / 8) * slots * 8 * (osa ? 2 : 1);
-        const int unit = layout_pair(layout) ? (pi >> 1) : pi;
-        const int slot = layout_slot(layout, y, x, pi & 1);
-        const __half* ub = buf + (size_t)unit * unit_halfs;
-        float v = __half2float(ub[((size_t)(c / 8) * slots + slot) * 8 + (c & 7)]);
-        if (osa) v += __half2float(ub[((size_t)(C / 8 + c / 8) * slots + slot) * 8 + (c & 7)]);
+        size_t hi, lo;
+        if (layout == L_HEAD) {   // [patch/128][pixel*C/8 + c/8][patch%128][8], the residual plane behind all tiles
+            const size_t tile = (size_t)H * H * (C / 8) * 128 * 8;
+            hi = (size_t)(pi >> 7) * tile + ((((size_t)(y * H + x) * (C / 8) + c / 8) * 128 + (pi & 127)) * 8 + (c & 7));
+            lo = hi + (size_t)((n + 127) >> 7) * tile;
+        } else {
+            const int slots = layout_slots(layout);
+            const size_t unit_halfs = (size_t)(C / 8) * slots * 8 * (osa ? 2 : 1);
+            const int unit = layout_pair(layout) ? (pi >> 1) : pi;
+            const int slot = layout_slot(layout, y, x, pi & 1);
+            hi = (size_t)unit * unit_halfs + ((size_t)(c / 8) * slots + slot) * 8 + (c & 7);
+            lo = hi + (size_t)(C / 8) * slots * 8;
+        }
+        float v = val(hi);
+        if (osa) v += val(lo);
         out[i] = v;
     }
 }
@@ -237,28 +247,32 @@ using namespace ag;
 
 extern "C" {
 
-// Developer diagnostic (tests/test_gpu_tcx.py): run the second-generation trunk of `net` on materialised patches [n,32,32] up to conv
-// layer `upto` (2..5) and decode that layer's output (fp16 hi [+ lo] planes in its HBM layout) to fp32 [n][C][H][H].
+// Developer diagnostic (tests/test_gpu_tcx.py, tests/test_gpu_net_bounds.py): run the second-generation trunk of `net` with the
+// handle's engine (ENGINE_TC2_BF16: the bf16 HardNet trunk; any other engine: the fp16 one) on materialised patches [n,32,32] up to conv
+// layer `upto` (2..6) and decode that layer's output (fp16 / bf16 hi [+ lo] planes in its HBM layout; layer 6: the head operand) to
+// fp32 [n][C][H][H].  d_ws: ag_net_workspace_bytes().
 int ag_debug_tcx_layer(const ag_net_t* net, const float* d_patches, int n, int upto, float* d_out, void* d_ws, size_t ws_bytes, void* stream) {
     AG_REQUIRE(net && d_patches && d_out && d_ws, "NULL argument");
-    AG_REQUIRE(upto >= 2 && upto <= 5 && n >= 1, "layer out of range");
+    AG_REQUIRE(upto >= 2 && upto <= 6 && n >= 1, "layer out of range");
     const size_t act = align_up(tcx_act_bytes(n), 256);
-    AG_REQUIRE(ws_bytes >= 2 * act, "workspace too small");
+    AG_REQUIRE(ws_bytes >= ag_net_workspace_bytes(net->kind, n), "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     char* base = (char*)d_ws;
     const tc::FirstSrc src = tc_src_patches(d_patches);
     const bool hard = net->kind == AG_NET_HARDNET;
-    int rc = hard ? tcx_trunk_hardnet(net, src, n, n, nullptr, base, base + act, nullptr, st, upto)
-                  : tcx_trunk_affori(net, src, n, n, nullptr, base, base + act, nullptr, st, upto);
+    const int bf = hard && net->engine == AG_ENGINE_TC2_BF16;
+    int rc = hard ? tcx_trunk_hardnet(net, src, n, n, nullptr, base, base + act, base + 2 * act, st, upto, bf)
+                  : tcx_trunk_affori(net, src, n, n, nullptr, base, base + act, base + 2 * act, st, upto);
     if (rc) return rc;
-    // layer l (2..5) writes: 2 -> bufB (L_S2_16, 32x32), 3 -> bufA (L_S1_16, 16x16), 4 -> bufB (L_S2_8P, 16x16), 5 -> bufA (L_S1_8P, 8x8)
-    const int lay = upto == 2 ? tcx::L_S2_16 : upto == 3 ? tcx::L_S1_16 : upto == 4 ? tcx::L_S2_8P : tcx::L_S1_8P;
+    // layer l writes: 2 -> bufB (L_S2_16, 32x32), 3 -> bufA (L_S1_16, 16x16), 4 -> bufB (L_S2_8P, 16x16), 5 -> bufA (L_S1_8P, 8x8),
+    // 6 -> the head operand behind both buffers (L_HEAD, 8x8)
+    const int lay = upto == 2 ? tcx::L_S2_16 : upto == 3 ? tcx::L_S1_16 : upto == 4 ? tcx::L_S2_8P : upto == 5 ? tcx::L_S1_8P : tcx::L_HEAD;
     const int H = upto == 2 ? 32 : (upto <= 4 ? 16 : 8);
     const int Cb = hard ? 32 : 16;
     const int C = upto == 2 ? Cb : (upto <= 4 ? 2 * Cb : 4 * Cb);
-    const void* buf = (upto == 2 || upto == 4) ? base + act : base;
+    const void* buf = upto == 6 ? base + 2 * act : (upto == 2 || upto == 4) ? base + act : base;
     const int osa = hard ? 0 : 1;
-    tcx::tcx_decode_kernel<<<296, 256, 0, st>>>((const __half*)buf, lay, C, osa, H, n, d_out);
+    tcx::tcx_decode_kernel<<<296, 256, 0, st>>>((const __half*)buf, lay, C, osa, H, n, bf, d_out);
     AG_CHECK_LAUNCH("tcx_decode_kernel");
     return AG_OK;
 }

@@ -195,15 +195,9 @@ __global__ void __launch_bounds__(288, 1) tc_headx_kernel(const __half* __restri
             if (!ok) continue;
             if (KIND == 0) {
                 const float s0 = acc[0] * inv_scale, s1 = acc[1] * inv_scale, s2 = acc[2 % NO] * inv_scale;
-                const float a00 = 1.0f + tanhf(s0 + bias[0]), a01 = 0.f, a10 = tanhf(s1 + bias[1]), a11 = 1.0f + tanhf(s2 + bias[2]);
+                const float a00 = 1.0f + tanhf(s0 + bias[0]), a10 = tanhf(s1 + bias[1]), a11 = 1.0f + tanhf(s2 + bias[2]);
                 if (raw_out) { raw_out[(size_t)pi * 3] = a00; raw_out[(size_t)pi * 3 + 1] = a10; raw_out[(size_t)pi * 3 + 2] = a11; }   // convertJIT/AffNetJIT.pt: xy + [1, 0, 1]
-                if (out) {
-                    const float det = sqrtf(fabsf(a00 * a11 - a10 * a01 + 1e-10f));
-                    const float b2a2 = sqrtf(a01 * a01 + a00 * a00);
-                    float* o = out + (size_t)pi * 4;
-                    o[0] = b2a2 / det; o[1] = 0.f;
-                    o[2] = (a11 * a01 + a10 * a00) / (b2a2 * det); o[3] = det / b2a2;
-                }
+                if (out) rectify_up_is_up(a00, 0.f, a10, a11, out + (size_t)pi * 4);
             } else {
                 float m0 = 0.f, m1 = 0.f;
 #pragma unroll

@@ -196,8 +196,9 @@ int ag_net_get_engine(const ag_net_t* net);
 /* Developer switch: 1 = ag_pyramid_build runs one launch per octave (pyramid_fused.cuh: bit-identical, measured slower), 0 = one
  * launch per level (default).  Returns the previous mode. */
 int ag_debug_pyramid_mode(int fused);
-/* Developer diagnostic: run the second-generation trunk on materialised patches [n,32,32] up to conv layer `upto` (2..5) and decode
- * that layer's activations (fp16 hi [+ lo] planes in the engine's HBM layout) to fp32 [n,C,H,H].  d_ws: ag_net_workspace_bytes(). */
+/* Developer diagnostic: run the second-generation trunk with the handle's engine (ENGINE_TC2_BF16: bf16 operands, HardNet; otherwise
+ * fp16) on materialised patches [n,32,32] up to conv layer `upto` (2..6) and decode that layer's activations (hi [+ lo] planes in the
+ * engine's HBM layout; layer 6: the 8x8 head's operand) to fp32 [n,C,H,H].  d_ws: ag_net_workspace_bytes(). */
 int ag_debug_tcx_layer(const ag_net_t* net, const float* d_patches, int n, int upto, float* d_out, void* d_ws, size_t ws_bytes, void* stream);
 /* Developer diagnostic: the device libm calls of the hand-crafted estimators, compiled with their flags, one element per thread:
  * d_atan2[i] = atan2f(d_y[i], d_x[i]), d_cos[i] = cosf(d_x[i]), d_sin[i] = sinf(d_x[i]) for i < n.  Lets a test restate the estimators
