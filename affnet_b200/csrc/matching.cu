@@ -260,6 +260,7 @@ extern "C" {
 
 int ag_distance_matrix(const float* d_a, int n1, const float* d_b, int n2, int dim, float* d_out, void* stream) {
     AG_REQUIRE(d_a && d_b && d_out && n1 >= 1 && n2 >= 1 && dim >= 1, "bad arguments");
+    AG_REQUIRE(cdiv(n1, MT) <= 65535, "n1 above 4194240 rows");   // the row tiles are grid.y
     dist_matrix_kernel<<<dim3(cdiv(n2, MT), cdiv(n1, MT)), 256, 0, (cudaStream_t)stream>>>(d_a, n1, d_b, n2, dim, d_out);
     AG_CHECK_LAUNCH("dist_matrix_kernel");
     return AG_OK;

@@ -140,8 +140,9 @@ def block_sum(contrib):
     return s
 
 
-def refit(pts, mask):
-    """Normalised DLT on the rows of `mask` -> H [9] or None."""
+def refit(pts, mask, trace=None):
+    """Normalised DLT on the rows of `mask` -> H [9] or None.  A list `trace` receives the normal matrix before (A0) and after (A) the
+    Jacobi sweeps, V, the chosen column mi, the mask and H (None when not finite)."""
     m = mask[:, None]
     x1, y1, x2, y2 = [np.where(mask, pts[:, k], 0.0) for k in range(4)]
     st = block_sum(np.stack([x1, y1, x1 * x1, y1 * y1, x2, y2, x2 * x2, y2 * y2], axis=1))
@@ -166,6 +167,7 @@ def refit(pts, mask):
             A[k, l] = A[l, k] = nm[e]
             e += 1
     V = np.eye(9)
+    A0 = A.copy()
     for _ in range(JACOBI_SWEEPS):
         for p in range(8):
             for q in range(p + 1, 9):
@@ -190,11 +192,15 @@ def refit(pts, mask):
     T1 = np.array([s1, 0.0, -(s1 * c1x), 0.0, s1, -(s1 * c1y), 0.0, 0.0, 1.0])
     T2i = np.array([1.0 / s2, 0.0, c2x, 0.0, 1.0 / s2, c2y, 0.0, 0.0, 1.0])
     H, ok = normalise_h(mul3(mul3(T2i, Hn), T1))
+    if trace is not None:
+        trace.append(dict(A0=A0, A=A.copy(), V=V.copy(), mi=mi, mask=mask.copy(), H=H if ok else None))
     return H if ok else None
 
 
-def ransac(pts, inl_th=2.0, confidence=0.99, max_iters=50000, seed=0):
-    """pts [n,4] float32 (x1, y1, x2, y2) -> (H [3,3] float32, mask [n] bool, ninl, iters) as ag_homography_ransac computes them."""
+def ransac(pts, inl_th=2.0, confidence=0.99, max_iters=50000, seed=0, trace=None):
+    """pts [n,4] float32 (x1, y1, x2, y2) -> (H [3,3] float32, mask [n] bool, ninl, iters) as ag_homography_ransac computes them.
+    A dict `trace` receives the best minimal hypothesis (H0), the inlier count of every refit round in order (counts: the first is
+    the hypothesis', a lower later one ended the rounds) and refit()'s trace of each round (refits)."""
     pts = np.asarray(pts, dtype=np.float32).astype(np.float64)
     n = len(pts)
     th = float(np.float32(inl_th))
@@ -225,13 +231,18 @@ def ransac(pts, inl_th=2.0, confidence=0.99, max_iters=50000, seed=0):
     H = best_H
     mask = inliers(H, pts, th2)[0]
     cnt = int(mask.sum())
+    refits = [] if trace is not None else None
+    if trace is not None:
+        trace.update(H0=H.copy(), counts=[cnt], refits=refits)
     for _ in range(REFIT_ROUNDS):
         if cnt < 4:
             break
-        Hr = refit(pts, mask)
+        Hr = refit(pts, mask, refits)
         if Hr is None:
             break
         mr = inliers(Hr, pts, th2)[0]
+        if trace is not None:
+            trace["counts"].append(int(mr.sum()))
         if int(mr.sum()) < cnt:
             break
         H, mask, cnt = Hr, mr, int(mr.sum())

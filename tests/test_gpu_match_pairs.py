@@ -1,10 +1,11 @@
-"""GPU tests (-m gpu) of the batched SNN matcher (ag_match_pairs, Losses.match_snn_pairs).  The expected values are computed without the
-matcher's kernels: ag_distance_matrix (distance_matrix_vector) on the count-sliced descriptors of each pair, then the torch reductions of
-snn_rule.snn_expected.  Every output is prefilled with a sentinel, so rows the matcher must not write are checked as well."""
+"""GPU tests (-m gpu) of the batched SNN matcher (ag_match_pairs, Losses.match_snn_pairs).  The expected values are computed without any
+library kernel: the exact restatement of the distances (matching_restated.distances_blocked, float64 tensor operations on the device) on
+the count-sliced descriptors of each pair, then the torch reductions of snn_rule.snn_expected.  Every output is prefilled with a sentinel, so rows the matcher must not write are checked as well."""
 import pytest
 import torch
 
 from helpers import SENTINEL, gold, gray_from_rgb, load_weights, synthetic_image
+from matching_restated import distances_blocked
 from snn_rule import snn_expected
 
 pytestmark = pytest.mark.gpu
@@ -55,7 +56,6 @@ def check_against_expected(o, d1, c1, d2, c2, pairs, ratio=0.8, tag=""):
     """Valid pairs: idx2, min, second and keep bit-identical to snn_expected, tent[:ntent] = (arange[keep], idx2[keep]), rows beyond n1 and
     tentative rows beyond ntent untouched.  Pairs with an index out of range or a count outside 0..cap: ntent -1; with an empty image: 0;
     nothing else written.  Returns the per-pair tentative counts."""
-    from affnet_b200.Losses import distance_matrix_vector
     S1, cap1 = d1.shape[:2]
     S2, cap2 = d2.shape[:2]
     cnt1 = [cap1] * S1 if c1 is None else c1.tolist()
@@ -71,7 +71,7 @@ def check_against_expected(o, d1, c1, d2, c2, pairs, ratio=0.8, tag=""):
             n1 = 0
         else:
             n2 = cnt2[j]
-            idx2, mn, sec, keep, tent = snn_expected(distance_matrix_vector(d1[i, :n1], d2[j, :n2]), ratio)
+            idx2, mn, sec, keep, tent = snn_expected(distances_blocked(d1[i, :n1], d2[j, :n2], DEV, rows=4096), ratio)
             assert torch.equal(o["idx2"][p, :n1].long(), idx2), what
             assert torch.equal(o["min"][p, :n1], mn), what
             assert torch.equal(o["second"][p, :n1], sec), what
@@ -161,8 +161,7 @@ def test_constructed_cases(L, D):
     assert idx2[5] == 0 and o["min"][0, 5].item() == float("inf")
     if D > 1:
         assert idx2[0] == 3 and idx2[1] == 3 and idx2[10] == 50 and idx2[11] == 51 and 20 not in idx2
-        from affnet_b200.Losses import distance_matrix_vector
-        dm = distance_matrix_vector(d1[0], d2[0])
+        dm = distances_blocked(d1[0], d2[0], DEV)
         unmasked = torch.where(torch.isnan(dm[10]), float("inf"), dm[10]).sort().values[1]
         assert o["second"][0, 10].item() != unmasked.item()
     # the same rows twice, as set 1 and set 2 of one tensor (self matching)

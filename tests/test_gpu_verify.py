@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import affnet_oracle as O
+import matching_restated as MR
 import oracle_ransac as R
 from helpers import SENTINEL, gold, gray_from_rgb, load_weights, synthetic_image
 from verify_cases import corner_error, correspondences, project, random_homography
@@ -92,23 +93,16 @@ def build_sets(cases, seed=0):
 
 
 def check_ransac_pair(o, p, pts, tag, th=2.0, max_iters=50000):
-    """Pair p of the GPU outputs against the restatement: ninl and iters exactly, masks except near-threshold points, H to 1e-4."""
+    """Pair p of the GPU outputs against the restatement: ninl, iters, the whole inlier mask and the bits of H equal."""
     H, m, n, it = R.ransac(pts, th, 0.99, max_iters, 0)
     k = len(pts)
     assert int(o["ninl"][p]) == n and int(o["iters"][p]) == it, (tag, int(o["ninl"][p]), n, int(o["iters"][p]), it)
-    gm = o["inl"][p, :k].numpy()
-    assert set(np.unique(gm).tolist()) <= {0, 1}, tag
+    assert np.array_equal(o["inl"][p, :k].numpy(), m.astype(np.uint8)), (tag, int((o["inl"][p, :k].numpy() != m).sum()))
+    assert np.array_equal(o["H"][p].numpy().view(np.int32), H.view(np.int32)), (tag, o["H"][p], H)
     if n > 0:
-        Hd = H.astype(np.float64).reshape(9)
-        x, y = pts[:, 0].astype(np.float64), pts[:, 1].astype(np.float64)
-        w = Hd[6] * x + Hd[7] * y + Hd[8]
-        err = ((Hd[0] * x + Hd[1] * y + Hd[2]) / w - pts[:, 2]) ** 2 + ((Hd[3] * x + Hd[4] * y + Hd[5]) / w - pts[:, 3]) ** 2
-        border = np.abs(err - th * th) <= 1e-6 * th * th
-        assert np.array_equal(gm.astype(bool)[~border], m[~border]), tag
-        assert np.linalg.norm(o["H"][p].numpy() - H) <= 1e-4 * np.linalg.norm(H), (tag, o["H"][p], H)
         assert float(o["H"][p, 2, 2]) == 1.0
     else:
-        assert not gm.any() and not o["H"][p].any(), tag
+        assert not o["H"][p].any(), tag
     assert bool((o["inl"][p, k:] == INL_SENTINEL).all()), (tag, "mask rows beyond ntent written")
     return n, it
 
@@ -190,20 +184,37 @@ def gt_oracle(pts, Hm, th):
 
 
 def check_gt_pair(o, p, pts, Hm, th, tag):
-    """The kept set equals the oracle's except rows within 0.1 px of the threshold; min_dist within 0.05 px, or min_dist^2 within 1 px^2.
-    The reference's formula subtracts fp32 terms of up to ~3e6 px^2 (ulp 0.25), so its value carries rounding noise of ~1 px^2 that
-    depends on the order of the operations: ~0.08 px at the 6 px threshold, more at small distances."""
+    """min_dist, idx2 and the true rows bit for bit against the restatement (tests/matching_restated.py).  Against the oracle: both
+    min_dist^2 within the bound derived from their fp32 chains of the float64 minimum (tests/matching_restated.gt_sq64), and the same
+    decision wherever the float64 margin to the threshold exceeds both bounds.  (The reference's formula subtracts fp32 terms of up to
+    ~3e6 px^2, so its rounding noise is ~1 px^2 and depends on the order of the operations: no fixed fp32 result to match.)"""
     n = len(pts)
-    keep, mn = gt_oracle(pts, Hm, th)
+    Hf = np.asarray(Hm, np.float32)
+    mn, idx2, true = MR.gt_check(pts, Hf, th, DEV)
     ntrue = int(o["ntrue"][p])
-    got = o["true"][p, :ntrue].numpy()
-    assert np.all(np.diff(got) > 0), tag
-    gm = o["min"][p, :n].numpy().astype(np.float64)
-    near = np.abs(mn - th) <= 0.1
-    assert set(got[~near[got]].tolist()) == set(keep[~near[keep]].tolist()), tag
-    ok = (np.abs(gm - mn) <= 0.05) | (np.abs(gm * gm - mn.astype(np.float64) ** 2) <= 1.0)
-    assert ok.all(), (tag, np.flatnonzero(~ok)[:5], gm[~ok][:5], mn[~ok][:5])
+    assert ntrue == true.numel() and torch.equal(o["true"][p, :ntrue].long(), true), tag
+    gm = o["min"][p, :n]
+    assert torch.equal(gm.view(torch.int32), mn.view(torch.int32)) and torch.equal(o["idx2"][p, :n].long(), idx2), tag
     assert bool((o["true"][p, ntrue:] == -7).all()) and bool((o["min"][p, n:] == SENTINEL).all()), (tag, "rows beyond ntent written")
+    keep, omn = gt_oracle(pts, Hm, th)
+    if n == 0:
+        return ntrue, 0
+    D2, bk = MR.gt_sq64(pts, Hf)
+    _, br = MR.gt_sq64(pts, Hf, fp32_inverse=True)
+    j = np.argmin(D2, 1)
+    r = np.arange(n)
+    d2, bk, br = D2[r, j], bk[r, j], br[r, j]
+    g2, o2 = gm.numpy().astype(np.float64) ** 2, omn.astype(np.float64) ** 2
+    assert np.all(np.abs(g2 - d2) <= bk) and np.all(np.abs(o2 - d2) <= br), tag
+    th2 = float(np.float32(th)) ** 2
+    sure = np.abs(d2 - th2) > np.maximum(bk, br)
+    ok = np.zeros(n, bool)
+    ok[keep] = True
+    got = np.zeros(n, bool)
+    got[true.numpy()] = True
+    assert np.array_equal(got[sure], ok[sure]) and np.array_equal(got[sure], (d2 <= th2)[sure]), tag
+    print("\nGT %-16s: worst |min_dist^2 - D^2| %.3f of the bound (oracle %.3f); %d of %d rows clear of the threshold" % (
+        tag, float(np.max(np.abs(g2 - d2) / bk)), float(np.max(np.abs(o2 - d2) / br)), int(sure.sum()), n), end="")
     return ntrue, len(keep)
 
 
@@ -252,7 +263,8 @@ def warp(img, Hm):
 def test_synthetic_warped_pairs(L, nets):
     """8 seeded 768x1024 images, each with its own warp (rotation <= 20 deg, scale 0.8-1.1, perspective ~1e-4), as one B = 16 pipeline
     batch (AffNet + histogram orientation, K = 2000): at least 95 % of the tentatives are GT-true at 6 px, every estimate lies within the
-    2 px inlier threshold of the true homography at all its inliers, and maps the frame's corners within 2 px.  On an H100 the corner
+    2 px inlier threshold of the true homography at all its inliers, and maps the frame's corners within 2 px.  RANSAC's and the GT
+    check's outputs equal their restatements bit for bit.  On an H100 the corner
     errors were 0.08 to 1.37 px: where the warp moves a corner out of view there are no keypoints, and the estimate is extrapolated."""
     from affnet_b200.Losses import match_snn_pairs
     from affnet_b200.pipeline import DetectDescribePipeline
@@ -270,7 +282,7 @@ def test_synthetic_warped_pairs(L, nets):
     tent, ntent, _, _ = match_snn_pairs(desc, cnt, pairs=pairs)
     H, inl, ninl, iters = find_homography_pairs(lafs, tent, ntent, pairs=pairs)
     Ht = torch.from_numpy(np.stack(Hs).astype(np.float32)).to(DEV)
-    true, ntrue, _, _ = gt_correspondences_pairs(lafs, tent, ntent, Ht, pairs=pairs)
+    true, ntrue, gmn, gidx = gt_correspondences_pairs(lafs, tent, ntent, Ht, pairs=pairs)
     pipe.check()
     nt, nti, nin, it = ntent.tolist(), ntrue.tolist(), ninl.tolist(), iters.tolist()
     print()
@@ -282,11 +294,17 @@ def test_synthetic_warped_pairs(L, nets):
         print("warped pair %d: %4d tentatives, %4d GT-true (>= %.0f), %4d inliers, %5d iterations, largest error at the inliers %.3f px (<= 2), "
               "corner error %.3f px (< 2)" % (k, nt[k], nti[k], 0.95 * nt[k], nin[k], it[k], at_inl, err))
         assert nt[k] > 100 and nti[k] >= 0.95 * nt[k] and at_inl <= 2.0 and err < 2.0, k
-        # the restatement on the same tentatives gives the same counts
+        # the restatements on the same tentatives give the same outputs, bit for bit
         t = tent[k, :nt[k]].long()
         pts = torch.cat([lafs[2 * k, t[:, 0], :, 2], lafs[2 * k + 1, t[:, 1], :, 2]], 1).cpu().numpy()
-        _, _, n_r, it_r = R.ransac(pts)
+        H_r, m_r, n_r, it_r = R.ransac(pts)
         assert (n_r, it_r) == (nin[k], it[k]), k
+        assert np.array_equal(inl[k, :nt[k]].cpu().numpy(), m_r.astype(np.uint8)), k
+        assert np.array_equal(H[k].cpu().numpy().view(np.int32), H_r.view(np.int32)), k
+        mn_r, idx2_r, true_r = MR.gt_check(pts, Hs[k].astype(np.float32), 6.0, DEV)
+        assert nti[k] == true_r.numel() and torch.equal(true[k, :nti[k]].cpu().long(), true_r), k
+        assert torch.equal(gmn[k, :nt[k]].cpu().view(torch.int32), mn_r.view(torch.int32)), k
+        assert torch.equal(gidx[k, :nt[k]].cpu().long(), idx2_r), k
 
 
 def test_graf_1_to_6(L, nets):

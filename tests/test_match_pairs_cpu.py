@@ -66,6 +66,18 @@ def test_refusals_and_texts(L):
     assert lib.ag_last_error() == b"ag_match_snn: workspace too small"
 
 
+def test_distance_matrix_refusals(L):
+    """ag_distance_matrix refuses before any CUDA call (the pointers are never dereferenced), n1 above 65535 row tiles included."""
+    lib = L.lib()
+    f = C.c_void_p(256)
+    for args in ((None, 5, f, 5, 8, f), (f, 0, f, 5, 8, f), (f, 5, f, 0, 8, f), (f, 5, f, 5, 0, f), (f, 5, f, 5, 8, None)):
+        assert lib.ag_distance_matrix(*args, None) == -1 and lib.ag_last_error().decode().startswith("ag_distance_matrix")
+    assert lib.ag_distance_matrix(f, 4194241, f, 5, 8, f, None) == -1
+    assert lib.ag_last_error().decode() == "ag_distance_matrix: n1 above 4194240 rows"
+    assert lib.ag_distance_matrix(f, 4194240, None, 5, 8, f, None) == -1    # the largest n1 passes that check (the NULL is refused)
+    assert "bad arguments" in lib.ag_last_error().decode()
+
+
 def test_wrapper_refusals(L):
     from affnet_b200.Losses import match_snn_pairs
     d = torch.zeros(2, 5, 8)
