@@ -248,6 +248,86 @@ def detector_level_stats(octave, sigmas, mrSize, th=0.0):
     return out
 
 
+def mixed_batch(h, w, seed):
+    """Two textured images around a constant one (which has no keypoint)."""
+    return torch.cat([synthetic_image(h, w, seed), torch.full((1, 1, h, w), 77.0), synthetic_image(h, w, seed + 1)])
+
+
+def plan_sigmas(plan):
+    return [[plan.sigma[o][l] for l in range(plan.n_levels)] for o in range(plan.n_octaves)]
+
+
+def flat_pyramid(plan, pyrs, device="cuda"):
+    """pyrs[b][o][l] ([1,1,h_o,w_o] or [h_o,w_o]) -> the plan's device buffer: image b of level (o, l) at level_offset[o][l] + b*h_o*w_o."""
+    buf = torch.zeros(plan.total_floats, dtype=torch.float32)
+    for b, pyr in enumerate(pyrs):
+        for o in range(plan.n_octaves):
+            n = plan.h[o] * plan.w[o]
+            for l in range(plan.n_levels):
+                off = plan.level_offset[o][l] + b * n
+                buf[off:off + n] = pyr[o][l].reshape(-1)
+    return buf.to(device)
+
+
+def gpu_pyramids(L, imgs, nlevels=3, border=5):
+    """The GPU blur's pyramid of imgs [B,1,H,W] -> (plan, device buffer, per-image CPU copies pyrs[b][o][l] [1,1,h,w])."""
+    from affnet_b200.HandCraftedModules import ScalePyramid
+    plan, buf = ScalePyramid(nlevels, 1.6, border).build(imgs.to("cuda").contiguous())
+    views, _, _ = ScalePyramid.views(plan, buf)
+    pyrs = [[[lv[b:b + 1].cpu() for lv in octave] for octave in views] for b in range(plan.B)]
+    return plan, buf, pyrs
+
+
+class Detector:
+    """ag_detect once over a workspace of `cap` candidates per image; select() calls ag_select_keypoints and select_all()
+    ag_select_all_keypoints into sentinel-filled outputs."""
+
+    def __init__(self, L, plan, buf, th=0.0, mr=5.192, cap=None):
+        import ctypes as C
+        self.C, self.L, self.lib, self.plan = C, L, L.lib(), plan
+        self.cap = cap or max(plan.H * plan.W // 4, 4096)
+        self.ws_buf = torch.full((self.lib.ag_detect_ws_bytes(C.byref(plan), self.cap),), 0xFF, dtype=torch.uint8, device="cuda")
+        self.ws = L.DetectWs()
+        L.check(self.lib.ag_detect_ws_carve(C.byref(plan), self.cap, L.ptr(self.ws_buf), C.byref(self.ws)))
+        L.check(self.lib.ag_detect(C.byref(plan), L.ptr(buf), float(th), int(mr), C.byref(self.ws), L.stream_ptr()))
+
+    def cand_counts(self):
+        off = self.ws.d_cand_count - self.ws_buf.data_ptr()
+        return self.ws_buf[off:off + 4 * self.plan.B].view(torch.int32).cpu()
+
+    def _outputs(self, cap):
+        B, isent = self.plan.B, int(SENTINEL)
+        return (torch.full((B, cap), SENTINEL, device="cuda"), torch.full((B, cap, 2, 3), SENTINEL, device="cuda"),
+                torch.full((B, cap), isent, dtype=torch.int32, device="cuda"), torch.full((B, cap), isent, dtype=torch.int32, device="cuda"),
+                torch.full((B,), isent, dtype=torch.int32, device="cuda"))
+
+    def select(self, nf, out_cap=None, a_scale=1.0):
+        """-> (rc, (resp [B,out_cap], lafs [B,out_cap,2,3], oct, lvl, count [B])) on the CPU."""
+        C, L = self.C, self.L
+        cap = out_cap or nf
+        out = self._outputs(cap)
+        rc = self.lib.ag_select_keypoints(C.byref(self.plan), C.byref(self.ws), int(nf), float(a_scale), cap, *[L.ptr(t) for t in out],
+                                          L.stream_ptr())
+        torch.cuda.synchronize()
+        return rc, tuple(t.cpu() for t in out)
+
+    def checked_select(self, nf, out_cap=None, a_scale=1.0):
+        rc, out = self.select(nf, out_cap, a_scale)
+        self.L.check(rc)
+        return out
+
+    def select_all(self, out_cap, a_scale=1.0):
+        """ag_select_all_keypoints (every candidate of the accepted levels, seq order) -> the outputs of select()."""
+        C, L = self.C, self.L
+        nbytes = self.lib.ag_select_all_workspace_bytes(C.byref(self.plan), self.cap)
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+        out = self._outputs(out_cap)
+        L.check(self.lib.ag_select_all_keypoints(C.byref(self.plan), C.byref(self.ws), float(a_scale), out_cap, L.ptr(scratch), nbytes,
+                                                 *[L.ptr(t) for t in out], L.stream_ptr()))
+        torch.cuda.synchronize()
+        return tuple(t.cpu() for t in out)
+
+
 class OracleCandidates:
     """Every keypoint the oracle emits for one image before its global top-k (num_features <= 0: per-level raster order, octave after
     octave, level after level), with each one's seq; select(nf) applies the selection rule the C ABI documents: the top nf by (response

@@ -9,7 +9,9 @@ import pytest
 import torch
 
 import affnet_oracle as O
-from helpers import TOL, gold, gray_from_rgb, laf_rel_errors, load_weights, match_keypoints, orientation_boundary_shares, parity_report
+from detect_restated import Restated, bits, bound_ratio, softargmax32, softargmax64
+from helpers import (TOL, OracleCandidates, gold, gray_from_rgb, laf_rel_errors, load_weights, match_keypoints, orientation_boundary_shares,
+                     parity_report)
 
 pytestmark = pytest.mark.gpu
 
@@ -162,7 +164,10 @@ def test_nms_level_identical_given_response_maps(L):
             else:
                 assert n == r_o.numel()
                 assert torch.equal(resp[:n].cpu(), r_o)            # raster order, identical values (incl. negatives)
-                assert (lafs[:n].cpu() - A_o).abs().max() < 1e-6
+                maps3 = torch.stack([torch.from_numpy(np.ascontiguousarray(a)) for a in (low, cur, high)])
+                assert torch.equal(bits(lafs[:n].cpu()), bits(softargmax32(maps3, scales, idx_o, "taps")))   # detect_level_kernel's order
+                L64, B64 = softargmax64(maps3, scales, idx_o)
+                assert bound_ratio(A_o, L64, B64) <= 1.0
         if r_o is not None:
             assert np.array_equal(om_out.cpu().numpy(), om_o)
             # raw candidate list: same pixel set
@@ -177,13 +182,17 @@ def test_detector_identical_given_oracle_pyramid(L):
     pyr, sig, pix = O.scale_pyramid(img)
     plan = L.make_plan(1, img.size(2), img.size(3), 3, 1.6, 5)
     buf = pyr_to_flat(L, pyr, plan)
+    c = OracleCandidates(pyr, sig, 5.192)
+    R = Restated(pyr, sig, c.seq, "rows")
     for nf in (450, 200, 4000):
         r_o, L_o, p_o, l_o = O.multi_scale_detector(pyr, sig, nf, 5.192)
         r, la, oc, lv, _, _ = run_detect(L, plan, buf, nf, 1.0)
         assert r.numel() == r_o.numel()
         assert torch.equal(r, r_o)
         assert torch.equal(oc.float(), p_o) and torch.equal(lv.float(), l_o)
-        assert (la - L_o).abs().max() < 1e-6
+        idx = torch.from_numpy(np.ascontiguousarray(c.order(nf)[0])).long()
+        assert torch.equal(bits(la), bits(R.lafs32[idx]))                 # detect_rows_kernel's order
+        assert bound_ratio(la, R.lafs64[idx], R.bound[idx]) <= 1.0
 
 
 def test_detector_threshold_mode_returns_all(L):
@@ -196,7 +205,10 @@ def test_detector_threshold_mode_returns_all(L):
     pyr_g = [[t.cpu() for t in o] for o in det.scale_pyr]
     r_o, L_o, p_o, l_o = O.multi_scale_detector(pyr_g, sig, -1, 5.192, th=5.0)
     assert r.numel() == r_o.numel() and torch.equal(r.cpu(), r_o)
-    assert torch.equal(oc.cpu(), p_o) and (la.cpu() - L_o).abs().max() < 1e-6
+    c = OracleCandidates(pyr_g, sig, 5.192, th=5.0)
+    R = Restated(pyr_g, sig, c.seq, "rows", th=5.0)                      # every candidate, in seq order
+    assert torch.equal(oc.cpu(), p_o) and torch.equal(bits(la.cpu()), bits(R.lafs32))
+    assert bound_ratio(L_o, R.lafs64, R.bound) <= 1.0
 
 
 def test_sampler_vs_oracle(L):

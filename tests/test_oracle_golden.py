@@ -5,6 +5,8 @@ import pytest
 import torch
 
 import affnet_oracle as O
+import detect_cases as DC
+from detect_restated import Restated, bound_ratio, softargmax64
 from helpers import gold, load_weights, gray_from_rgb, match_keypoints
 
 W = load_weights()
@@ -44,7 +46,13 @@ def test_detector_stage_bit_exact_vs_reference_golden():
     resp, LAFs, pidx, lidx = O.multi_scale_detector(pyr, sig, int(1.5 * K), 5.192)
     assert torch.equal(resp, T(z["det_resp"]))                     # identical index set and order
     assert torch.equal(pidx, T(z["det_pidx"])) and torch.equal(lidx, T(z["det_lidx"]))
-    assert (LAFs - T(z["det_LAFs"])).abs().max() < 1e-6            # soft-argmax conv order: 6e-8
+    # the soft-argmax sums in F.conv2d's order, which differs between the reference's run and the oracle's: both lie within the
+    # float64 soft-argmax's bound for any summation order (tests/detect_restated.py)
+    for name, pyr_g, sig_g, seq, ref, ora, maps in DC.golden_rows():
+        R = Restated(pyr_g, sig_g, seq, None, maps=maps)
+        assert bound_ratio(ref, R.lafs64, R.bound) <= 1.0 and bound_ratio(ora, R.lafs64, R.bound) <= 1.0, name
+        if name.startswith("graf_crop"):
+            assert torch.equal(ora, LAFs)
 
 
 def test_nms_octave_map_q4():
@@ -55,7 +63,9 @@ def test_nms_octave_map_q4():
         assert torch.equal(r, T(z[tag + "_resp"]))
         assert (r < 0).any() or nf > 0                             # Q4: re-detected pixels go negative
         assert np.array_equal(om, z[tag + "_omap"])                # uint8 wrap reproduced
-        assert (A - T(z[tag + "_LAFs"])).abs().max() < 1e-6
+        maps3 = torch.cat([low, cur, high], 1)[0]
+        L64, B64 = softargmax64(maps3, list(z["scales"]), idxs)
+        assert bound_ratio(A, L64, B64) <= 1.0 and bound_ratio(T(z[tag + "_LAFs"]), L64, B64) <= 1.0
 
 
 def test_sampler_and_affnet_stage():
