@@ -41,9 +41,6 @@ class ScaleSpaceAffinePatchExtractor(nn.Module):
             self.th = 0
         if RespNet is not None:
             raise NotImplementedError("custom RespNet: only the fused Hessian response is implemented")
-        if th is None and int(1.5 * num_features if num_Baum_iters > 0 else num_features) > 16384:
-            raise L.AffnetB200Error("num_features=%d: the device-side selection sorts at most 16384 keypoints in shared memory "
-                                    "(num_features <= 10923 with a shape estimator, <= 16384 without)" % num_features)
         # SparseImgRepresenter.py:42-49: the hand-crafted estimators are the defaults
         self.OriNet = OriNet if OriNet is not None else OrientationDetector(patch_size=19)
         self.AffNet = AffNet if AffNet is not None else AffineShapeEstimator(patch_size=19)
@@ -74,8 +71,11 @@ class ScaleSpaceAffinePatchExtractor(nn.Module):
             if num_features > 0:
                 out_cap = num_features
                 resp, lafs, oct_, lvl, cnt = self._select_outputs(out_cap, dev)
-                L.check(lib.ag_select_keypoints(C.byref(plan), C.byref(ws), num_features, float(a_scale), out_cap, L.ptr(resp),
-                                                L.ptr(lafs), L.ptr(oct_), L.ptr(lvl), L.ptr(cnt), L.stream_ptr()))
+                # any count: the shared-memory sort up to 16384 keypoints, the global-memory one above (no scratch below)
+                scratch = self._scratch(lib.ag_select_topk_workspace_bytes(C.byref(plan), cap, out_cap), dev)
+                L.check(lib.ag_select_topk_keypoints(C.byref(plan), C.byref(ws), num_features, float(a_scale), out_cap, L.ptr(scratch),
+                                                     0 if scratch is None else scratch.numel(), L.ptr(resp), L.ptr(lafs), L.ptr(oct_),
+                                                     L.ptr(lvl), L.ptr(cnt), L.stream_ptr()))
                 # one host round trip: candidate count (overflow check) + selected count
                 host = torch.cat([self._wrap_i32(ws.d_cand_count, 1, ws_buf), cnt]).cpu()
             else:
@@ -100,6 +100,11 @@ class ScaleSpaceAffinePatchExtractor(nn.Module):
         return (torch.empty(n, dtype=torch.float32, device=dev), torch.empty(n, 2, 3, dtype=torch.float32, device=dev),
                 torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
                 torch.empty(1, dtype=torch.int32, device=dev))
+
+    @staticmethod
+    def _scratch(nbytes, dev):
+        """Scratch of a top-K entry point, or None when it needs none."""
+        return torch.empty(nbytes, dtype=torch.uint8, device=dev) if nbytes else None
 
     @staticmethod
     def _wrap_i32(addr, n, owner):
@@ -167,9 +172,10 @@ class ScaleSpaceAffinePatchExtractor(nn.Module):
                                                        L.stream_ptr()))
             m = int(cnt_o.item())
         elif n > 0:
-            L.check(L.lib().ag_affine_shape_filter(L.ptr(base_A), L.ptr(final_resp), L.ptr(LAFs), L.ptr(oct_), L.ptr(lvl), L.ptr(cnt_in),
-                                                   1, n, int(num_features), n, L.ptr(resp_o), L.ptr(lafs_o), L.ptr(oct_o), L.ptr(lvl_o),
-                                                   L.ptr(cnt_o), L.stream_ptr()))
+            scratch = self._scratch(lib.ag_affine_shape_filter_topk_workspace_bytes(1, n), dev)
+            L.check(lib.ag_affine_shape_filter_topk(L.ptr(base_A), L.ptr(final_resp), L.ptr(LAFs), L.ptr(oct_), L.ptr(lvl), L.ptr(cnt_in),
+                                                    1, n, int(num_features), n, L.ptr(scratch), 0 if scratch is None else scratch.numel(),
+                                                    L.ptr(resp_o), L.ptr(lafs_o), L.ptr(oct_o), L.ptr(lvl_o), L.ptr(cnt_o), L.stream_ptr()))
             m = int(cnt_o.item())
         else:
             m = 0

@@ -83,6 +83,8 @@ PROTOTYPES = {
     "ag_select_keypoints": (i32, [C.POINTER(PyramidPlan), C.POINTER(DetectWs), i32, f32, i32, vp, vp, vp, vp, vp, vp]),
     "ag_select_all_workspace_bytes": (sz, [C.POINTER(PyramidPlan), i32]),
     "ag_select_all_keypoints": (i32, [C.POINTER(PyramidPlan), C.POINTER(DetectWs), f32, i32, vp, sz, vp, vp, vp, vp, vp, vp]),
+    "ag_select_topk_workspace_bytes": (sz, [C.POINTER(PyramidPlan), i32, i32]),
+    "ag_select_topk_keypoints": (i32, [C.POINTER(PyramidPlan), C.POINTER(DetectWs), i32, f32, i32, vp, sz, vp, vp, vp, vp, vp, vp]),
     "ag_extract_patches": (i32, [vp, i32, i32, i32, i32, vp, i32, i32, vp, vp]),
     "ag_extract_patches_pyr": (i32, [C.POINTER(PyramidPlan), vp, vp, vp, vp, vp, i32, i32, vp, vp]),
     "ag_pyramid_level_for_lafs": (i32, [C.POINTER(PyramidPlan), vp, i32, i32, vp, vp, vp]),
@@ -107,6 +109,8 @@ PROTOTYPES = {
     "ag_net_forward_pyr": (i32, [vp, C.POINTER(PyramidPlan), vp, vp, vp, vp, vp, i32, vp, vp, sz, vp]),
     "ag_affine_shape_filter": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
     "ag_affine_shape_filter_all": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]),
+    "ag_affine_shape_filter_topk_workspace_bytes": (sz, [i32, i32]),
+    "ag_affine_shape_filter_topk": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp, sz, vp, vp, vp, vp, vp, vp]),
     "ag_lafs_apply_rotation": (i32, [vp, vp, i32, vp]),
     "ag_lafs_scale": (i32, [vp, vp, i32, f32, f32, f32, vp]),
     "ag_lafs_to_ell": (i32, [vp, i32, vp, vp]),
@@ -129,6 +133,8 @@ PROTOTYPES = {
                                       C.POINTER(vp)]),
     "ag_pipeline_create_th": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), C.POINTER(PipelineDescriptor), f32, vp, vp, vp,
                                     C.POINTER(vp)]),
+    "ag_pipeline_create_topk": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), C.POINTER(PipelineDescriptor), vp, vp, vp,
+                                      C.POINTER(vp)]),
     "ag_pipeline_destroy": (None, [vp]),
     "ag_pipeline_workspace_bytes": (sz, [vp]),
     "ag_pipeline_plan": (C.POINTER(PyramidPlan), [vp]),

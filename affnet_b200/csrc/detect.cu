@@ -16,6 +16,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "topk.cuh"
 
 namespace ag {
 
@@ -990,20 +991,6 @@ __device__ __forceinline__ void write_keypoint(float a_scale, float val, const f
 // 0.88 ms for one 4K image.)
 constexpr int SEL_CL = 8;
 
-__device__ __forceinline__ uint32_t dsmem_addr(const void* p, int rank) {
-    uint32_t a = (uint32_t)__cvta_generic_to_shared(p), r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ int dsmem_ld_i32(uint32_t a) { int v; asm volatile("ld.shared::cluster.s32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
-__device__ __forceinline__ unsigned long long dsmem_ld_u64(uint32_t a) { unsigned long long v; asm volatile("ld.shared::cluster.u64 %0, [%1];" : "=l"(v) : "r"(a) : "memory"); return v; }
-__device__ __forceinline__ void dsmem_st_i32(uint32_t a, int v) { asm volatile("st.shared::cluster.s32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-__device__ __forceinline__ void dsmem_st_u64(uint32_t a, unsigned long long v) { asm volatile("st.shared::cluster.u64 [%0], %1;" ::"r"(a), "l"(v) : "memory"); }
-__device__ __forceinline__ int dsmem_atomic_add(uint32_t a, int v) { int o; asm volatile("atom.shared::cluster.add.s32 %0, [%1], %2;" : "=r"(o) : "r"(a), "r"(v) : "memory"); return o; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
 __global__ void __launch_bounds__(SNT) select_kernel(const SelectParams P) {
     extern __shared__ unsigned char smem_raw[];
     unsigned long long* s_key = reinterpret_cast<unsigned long long*>(smem_raw);                                    // used by cluster rank 0
@@ -1148,6 +1135,75 @@ __global__ void __launch_bounds__(SNT) select_kernel(const SelectParams P) {
     }
     // a candidate list that overflowed its capacity is reported as count = -1 (downstream kernels then process no rows)
     if (threadIdx.x == 0) P.count[b] = (P.cand_count[b] > P.cand_cap) ? -1 : m_out;
+}
+
+// ---- top-K selection at any count (ag_select_topk_keypoints above TOPK_SMEM_MAX keys) -------------------------------------------------
+// select_kernel's selection parameters and keys, fed to the global-memory top-m primitive (topk.cuh), then the same write_keypoint.
+struct SelTopkSrc {
+    const float* cand_val;
+    const uint32_t* cand_seq;
+    const int* cand_count;
+    const int* level_pos;
+    const int* level_emit;
+    int cand_cap, n_slots, num_features, out_cap;
+
+    __device__ TopkSetup setup(int b) const {
+        const int nf = num_features;
+        unsigned acc = 0;
+        long long total = 0;
+        bool trimmed = false;
+        for (int s = 0; s < n_slots; s++) {
+            const int pos = level_pos[b * n_slots + s], emit = level_emit[b * n_slots + s];
+            if (pos > 1) {  // HandCraftedModules.py:253
+                acc |= 1u << s;
+                if (nf > 0 && nf < pos) { total += nf; trimmed = true; }  // per-level topk :259
+                else total += emit;
+            }
+        }
+        const bool sorted = (nf > 0) && (total > nf || trimmed);  // SparseImgRepresenter.py:104
+        const int n = min(cand_count[b], cand_cap);
+        long long m = sorted ? nf : total;
+        if (m > out_cap) m = out_cap;
+        if (m > n) m = n;
+        TopkSetup t;
+        t.n = n; t.m = (int)m; t.sorted = sorted; t.radix = sorted || m < total; t.fail = cand_count[b] > cand_cap; t.ctx = acc;
+        return t;
+    }
+    __device__ unsigned long long key(int b, int i, const TopkSetup& t) const {
+        const size_t o = (size_t)b * cand_cap + i;
+        const uint32_t sq = cand_seq[o];
+        if (!((t.ctx >> (sq >> SEQ_PIX_BITS)) & 1u)) return 0ull;
+        const unsigned long long lo = (unsigned long long)(0xFFFFFFFFu - sq);
+        return t.sorted ? (((unsigned long long)float_to_ordered(cand_val[o]) << 32) | lo) : (lo + 1ull);
+    }
+};
+
+struct SelTopkWrite {
+    const float* cand_val;
+    const uint32_t* cand_seq;
+    const float* cand_scyx;
+    const int* idx;          // sorted candidate rows [B, rows]
+    const TopkImage* img;
+    int cand_cap, n_det, out_cap, rows;
+    float a_scale;
+    float* resp;
+    float* lafs;
+    int* oct;
+    int* lvl;
+    int* count;
+};
+
+constexpr int STW_NT = 256;
+
+__global__ void __launch_bounds__(STW_NT) select_topk_write_kernel(const SelTopkWrite P) {
+    const int b = blockIdx.y, r = blockIdx.x * STW_NT + threadIdx.x;
+    const int cnt = P.img[b].count;   // -1: candidate overflow, nothing of the image is written
+    if (r == 0) P.count[b] = cnt;
+    if (r >= cnt) return;
+    const int c = P.idx[(size_t)b * P.rows + r];
+    const size_t cb = (size_t)b * P.cand_cap + c;
+    write_keypoint(P.a_scale, P.cand_val[cb], P.cand_scyx + cb * 3, (int)(P.cand_seq[cb] >> SEQ_PIX_BITS), P.n_det, (size_t)b * P.out_cap + r,
+                   P.resp, P.lafs, P.oct, P.lvl);
 }
 
 // ---- ordered keep-all selection at any count (threshold mode: num_features <= 0, every candidate of the accepted levels) ----------
@@ -1577,6 +1633,45 @@ int ag_select_all_keypoints(const ag_pyramid_plan_t* p, const ag_detect_ws_t* ws
     AG_CHECK_LAUNCH("select_all_prefix_kernel");
     select_all_scatter_kernel<<<dim3(grid, p->B), SA_NT, 0, st>>>(S);
     AG_CHECK_LAUNCH("select_all_scatter_kernel");
+    return AG_OK;
+}
+
+size_t ag_select_topk_workspace_bytes(const ag_pyramid_plan_t* p, int cand_cap, int out_cap) {
+    if (!p || p->B < 1 || cand_cap <= 0 || out_cap <= TOPK_SMEM_MAX) return 0;
+    return topk_scratch_bytes(p->B, out_cap);
+}
+
+int ag_select_topk_keypoints(const ag_pyramid_plan_t* p, const ag_detect_ws_t* ws, int num_features, float a_scale, int out_cap,
+                             void* d_scratch, size_t scratch_bytes, float* d_resp, float* d_lafs, int* d_oct, int* d_lvl, int* d_count,
+                             void* stream) {
+    AG_REQUIRE(p && ws && d_resp && d_lafs && d_oct && d_lvl && d_count && (d_scratch || scratch_bytes == 0), "NULL argument");
+    AG_REQUIRE(out_cap >= 1, "out_cap must be positive");
+    const int need = (num_features > 0) ? (num_features < out_cap ? num_features : out_cap) : out_cap;
+    if (need <= TOPK_SMEM_MAX)   // the shared-memory kernel holds it: bit-identical by construction
+        return ag_select_keypoints(p, ws, num_features, a_scale, out_cap, d_resp, d_lafs, d_oct, d_lvl, d_count, stream);
+    AG_REQUIRE(ws->B == p->B && ws->n_level_slots == p->n_octaves * (p->n_levels - 2) && ws->n_level_slots <= 32, "workspace / plan mismatch");
+    const size_t nb = ag_select_topk_workspace_bytes(p, ws->cand_cap, out_cap);
+    if (scratch_bytes < nb) {
+        set_error("ag_select_topk_keypoints: scratch of %zu bytes needed, %zu given", nb, scratch_bytes);
+        return AG_ERR_CAPACITY;
+    }
+    TopkBufs T;
+    topk_carve((unsigned char*)d_scratch, p->B, out_cap, T);
+    SelTopkSrc S;
+    S.cand_val = ws->d_cand_val; S.cand_seq = ws->d_cand_seq; S.cand_count = ws->d_cand_count;
+    S.level_pos = ws->d_level_pos; S.level_emit = ws->d_level_emit;
+    S.cand_cap = ws->cand_cap; S.n_slots = ws->n_level_slots; S.num_features = num_features; S.out_cap = out_cap;
+    cudaStream_t st = (cudaStream_t)stream;
+    int fin = 0;
+    int rc = topk_run(S, T, p->B, need, st, &fin);
+    if (rc != AG_OK) return rc;
+    SelTopkWrite Wr;
+    Wr.cand_val = ws->d_cand_val; Wr.cand_seq = ws->d_cand_seq; Wr.cand_scyx = ws->d_cand_scyx;
+    Wr.idx = T.idx[fin]; Wr.img = T.img;
+    Wr.cand_cap = ws->cand_cap; Wr.n_det = p->n_levels - 2; Wr.out_cap = out_cap; Wr.rows = T.rows; Wr.a_scale = a_scale;
+    Wr.resp = d_resp; Wr.lafs = d_lafs; Wr.oct = d_oct; Wr.lvl = d_lvl; Wr.count = d_count;
+    select_topk_write_kernel<<<dim3(cdiv(need, STW_NT), p->B), STW_NT, 0, st>>>(Wr);
+    AG_CHECK_LAUNCH("select_topk_write_kernel");
     return AG_OK;
 }
 

@@ -7,6 +7,7 @@
 // Decisions (eigen-ratio test, boundary test) use the reference's fp32 operation order with non-contracted
 // intrinsics so that identical A matrices give the identical survivor set.
 #include "common.cuh"
+#include "topk.cuh"
 
 namespace ag {
 
@@ -164,6 +165,70 @@ __global__ void __launch_bounds__(GNT) shape_filter_all_kernel(const ShapeParams
     if (threadIdx.x == 0) P.count_out[b] = (cin < 0) ? -1 : base;   // -1 = upstream capacity overflow, propagated
 }
 
+// ---- top-K filter at any cap (ag_affine_shape_filter_topk above TOPK_SMEM_MAX rows) -----------------------------------------------------
+// shape_filter_kernel's rule on the global-memory top-m primitive (topk.cuh).  One pass over the rows writes each row's keep flag, its
+// sorted-mode key resp * keep (-0 made +0) and the survivor count; the key source then reads them, and the writer recomputes the row with the
+// same compose_laf / shape_ok.
+constexpr int SK_NT = 256;
+
+__global__ void __launch_bounds__(SK_NT) shape_keys_kernel(const ShapeParams P, uint32_t* __restrict__ ord, unsigned char* __restrict__ keep,
+                                                           int* __restrict__ surv) {
+    const int b = blockIdx.y, i = blockIdx.x * SK_NT + threadIdx.x;
+    const int n = max(0, min(P.count_in[b], P.cap));
+    bool ok = false;
+    if (i < n) {
+        const size_t r = (size_t)b * P.cap + i;
+        float NL[6];
+        compose_laf(P.A + r * 4, P.lafs + r * 6, NL);
+        ok = shape_ok(P.A + r * 4, NL);
+        ord[r] = float_to_ordered(__fadd_rn(__fmul_rn(P.resp[r], ok ? 1.f : 0.f), 0.f));
+        keep[r] = ok ? 1 : 0;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, ok);
+    if ((threadIdx.x & 31) == 0 && bal) atomicAdd(&surv[b], __popc(bal));
+}
+
+struct ShapeTopkSrc {
+    const uint32_t* ord;
+    const unsigned char* keep;
+    const int* surv;
+    const int* count_in;
+    int cap, num_features, out_cap;
+
+    __device__ TopkSetup setup(int b) const {
+        const int S = surv[b];
+        const bool sorted = (num_features > 0) && (S > num_features);  // SparseImgRepresenter.py:151
+        int m = sorted ? num_features : S;
+        if (m > out_cap) m = out_cap;
+        TopkSetup t;
+        t.n = max(0, min(count_in[b], cap)); t.m = m; t.sorted = sorted; t.radix = 1; t.fail = count_in[b] < 0; t.ctx = 0;
+        return t;
+    }
+    // shape_filter_kernel's key: sorted, (resp * keep, row ascending); else (keep, row ascending)
+    __device__ unsigned long long key(int b, int i, const TopkSetup& t) const {
+        const size_t r = (size_t)b * cap + i;
+        const unsigned hi = t.sorted ? ord[r] : (unsigned)keep[r];
+        return ((unsigned long long)hi << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)i);
+    }
+};
+
+__global__ void __launch_bounds__(SK_NT) shape_topk_write_kernel(const ShapeParams P, const int* __restrict__ idx, const TopkImage* __restrict__ img,
+                                                                 int rows) {
+    const int b = blockIdx.y, r = blockIdx.x * SK_NT + threadIdx.x;
+    const TopkImage im = img[b];
+    if (r == 0) P.count_out[b] = im.count;   // -1 = upstream capacity overflow, propagated
+    if (r >= im.count) return;
+    const int i = idx[(size_t)b * rows + r];
+    const size_t ri = (size_t)b * P.cap + i, o = (size_t)b * P.out_cap + r;
+    float NL[6];
+    compose_laf(P.A + ri * 4, P.lafs + ri * 6, NL);
+    P.resp_out[o] = im.sorted ? __fmul_rn(P.resp[ri], shape_ok(P.A + ri * 4, NL) ? 1.f : 0.f) : P.resp[ri];
+#pragma unroll
+    for (int q = 0; q < 6; q++) P.lafs_out[o * 6 + q] = NL[q];
+    P.oct_out[o] = P.oct[ri];
+    P.lvl_out[o] = P.lvl[ri];
+}
+
 __global__ void lafs_rotate_kernel(float* __restrict__ lafs, const float* __restrict__ R, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -278,6 +343,51 @@ int ag_affine_shape_filter_all(const float* d_A, const float* d_resp, const floa
     P.resp_out = d_resp_out; P.lafs_out = d_lafs_out; P.oct_out = d_oct_out; P.lvl_out = d_lvl_out; P.count_out = d_count_out;
     shape_filter_all_kernel<<<B, GNT, 0, (cudaStream_t)stream>>>(P);
     AG_CHECK_LAUNCH("shape_filter_all_kernel");
+    return AG_OK;
+}
+
+size_t ag_affine_shape_filter_topk_workspace_bytes(int B, int cap) {
+    if (B < 1 || cap <= TOPK_SMEM_MAX) return 0;
+    const size_t nb = B, nc = cap;
+    return topk_scratch_bytes(nb, nc) + align_up(nb * nc * sizeof(uint32_t), 256) + align_up(nb * nc, 256) + align_up(nb * sizeof(int), 256);
+}
+
+int ag_affine_shape_filter_topk(const float* d_A, const float* d_resp, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                                const int* d_count_in, int B, int cap, int num_features, int out_cap, void* d_scratch, size_t scratch_bytes,
+                                float* d_resp_out, float* d_lafs_out, int* d_oct_out, int* d_lvl_out, int* d_count_out, void* stream) {
+    AG_REQUIRE(d_A && d_resp && d_lafs && d_oct && d_lvl && d_count_in && d_resp_out && d_lafs_out && d_oct_out && d_lvl_out && d_count_out &&
+                   (d_scratch || scratch_bytes == 0), "NULL argument");
+    AG_REQUIRE(B >= 1 && cap >= 1 && out_cap >= 1, "bad sizes");
+    if (cap <= TOPK_SMEM_MAX)   // the shared-memory kernel holds it: bit-identical by construction
+        return ag_affine_shape_filter(d_A, d_resp, d_lafs, d_oct, d_lvl, d_count_in, B, cap, num_features, out_cap, d_resp_out, d_lafs_out,
+                                      d_oct_out, d_lvl_out, d_count_out, stream);
+    const size_t nb = ag_affine_shape_filter_topk_workspace_bytes(B, cap);
+    if (scratch_bytes < nb) {
+        set_error("ag_affine_shape_filter_topk: scratch of %zu bytes needed, %zu given", nb, scratch_bytes);
+        return AG_ERR_CAPACITY;
+    }
+    TopkBufs T;
+    unsigned char* c = topk_carve((unsigned char*)d_scratch, B, cap, T);
+    uint32_t* ord = (uint32_t*)c; c += align_up((size_t)B * cap * sizeof(uint32_t), 256);
+    unsigned char* keep = c; c += align_up((size_t)B * cap, 256);
+    int* surv = (int*)c;
+    ShapeParams P;
+    P.A = d_A; P.resp = d_resp; P.lafs = d_lafs; P.oct = d_oct; P.lvl = d_lvl; P.count_in = d_count_in;
+    P.cap = cap; P.num_features = num_features; P.out_cap = out_cap; P.sort_cap = 0;
+    P.resp_out = d_resp_out; P.lafs_out = d_lafs_out; P.oct_out = d_oct_out; P.lvl_out = d_lvl_out; P.count_out = d_count_out;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = check_cuda(cudaMemsetAsync(surv, 0, (size_t)B * sizeof(int), st), "memset survivor counts");
+    if (rc != AG_OK) return rc;
+    shape_keys_kernel<<<dim3(cdiv(cap, SK_NT), B), SK_NT, 0, st>>>(P, ord, keep, surv);
+    AG_CHECK_LAUNCH("shape_keys_kernel");
+    ShapeTopkSrc S;
+    S.ord = ord; S.keep = keep; S.surv = surv; S.count_in = d_count_in; S.cap = cap; S.num_features = num_features; S.out_cap = out_cap;
+    int need = out_cap < cap ? out_cap : cap;   // the most rows the rule can select
+    if (num_features > 0 && num_features < need) need = num_features;
+    int fin = 0;
+    if ((rc = topk_run(S, T, B, need, st, &fin)) != AG_OK) return rc;
+    shape_topk_write_kernel<<<dim3(cdiv(need, SK_NT), B), SK_NT, 0, st>>>(P, T.idx[fin], T.img, T.rows);
+    AG_CHECK_LAUNCH("shape_topk_write_kernel");
     return AG_OK;
 }
 

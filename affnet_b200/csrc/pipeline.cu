@@ -24,6 +24,7 @@ struct ag_pipeline {
     int M;          // prefilter keypoints per image = int(1.5 K) with a shape step, K without; C in threshold mode
     int cand_cap;
     bool th_mode;   // ag_pipeline_create_th: detector threshold th, keep-all selection and shape filter
+    bool topk;      // ag_pipeline_create_topk: the top-K steps at any count (ag_select_topk_keypoints, ag_affine_shape_filter_topk)
     float th;
     // workspace layout (byte offsets)
     size_t off_pyr, off_det, off_resp1, off_lafs1, off_oct1, off_lvl1, off_cnt1, off_patches, off_A, off_lafs2, off_oct2,
@@ -33,7 +34,7 @@ struct ag_pipeline {
 
 using namespace ag;
 
-// ag_pipeline_create, ag_pipeline_create_ex, ag_pipeline_create_desc and ag_pipeline_create_th: `fn` names the entry point the caller called in the error texts
+// ag_pipeline_create, ag_pipeline_create_ex, ag_pipeline_create_desc, ag_pipeline_create_th and ag_pipeline_create_topk: `fn` names the entry point the caller called in the error texts
 #define PIPE_REQUIRE(cond, msg)                         \
     do {                                                \
         if (!(cond)) {                                  \
@@ -44,7 +45,7 @@ using namespace ag;
 
 static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est,
                            const ag_pipeline_descriptor_t* desc, const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet,
-                           bool th_mode, float th, ag_pipeline_t** out) {
+                           bool th_mode, float th, bool topk, ag_pipeline_t** out) {
     PIPE_REQUIRE(cfg && est && desc && out, "NULL argument");
     PIPE_REQUIRE(isfinite(th), "th must be finite");
     PIPE_REQUIRE(desc->kind == AG_DESC_HARDNET || desc->kind == AG_DESC_SIFT, "unknown descriptor kind");
@@ -73,14 +74,14 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
     int rc = ag_pyramid_plan(cfg->B, cfg->H, cfg->W, cfg->nlevels, cfg->init_sigma, cfg->border, &p->plan);
     if (rc != AG_OK) { delete p; return rc; }
     // the top-K selection kernels sort in shared memory (ag_select_keypoints / ag_affine_shape_filter): fail here, not at run time.
-    // Threshold mode keeps everything without a sort and has no such limit.
-    if (!th_mode && shape && (int)(1.5 * cfg->num_features) > 16384) {
+    // Threshold mode keeps everything without a sort and has no such limit, and the top-K entry points sort in global memory above it.
+    if (!th_mode && !topk && shape && (int)(1.5 * cfg->num_features) > 16384) {
         set_error("%s: num_features %d needs a prefilter of int(1.5 K) = %d keypoints; the shared-memory selection holds 16384 (K <= 10923)",
                   fn, cfg->num_features, (int)(1.5 * cfg->num_features));
         delete p;
         return AG_ERR_CAPACITY;
     }
-    if (!th_mode && !shape && cfg->num_features > 16384) {
+    if (!th_mode && !topk && !shape && cfg->num_features > 16384) {
         set_error("%s: num_features %d without a shape estimator: the shared-memory selection holds 16384 (K <= 16384)", fn,
                   cfg->num_features);
         delete p;
@@ -106,6 +107,7 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
         sift_windows(desc->ps, sift_k, p->sift_gk.data(), p->sift_pk.data());
     }
     p->th_mode = th_mode;
+    p->topk = topk && !th_mode;
     p->th = th_mode ? th : 0.f;
     // SparseImgRepresenter.py:192-194; threshold mode keeps every candidate, so the prefilter is the capacity C itself
     p->M = (shape && !th_mode) ? (int)(1.5 * cfg->num_features) : cfg->num_features;
@@ -144,6 +146,11 @@ static int pipeline_create(const char* fn, const ag_pipeline_config_t* cfg, cons
     p->off_base2 = take(aff_chain ? sizeof(float) * B * M * 4 : 0);
     p->off_lafsw = take(aff_chain ? sizeof(float) * B * M * 6 : 0);
     p->sel_bytes = th_mode ? ag_select_all_workspace_bytes(&p->plan, p->cand_cap) : 0;
+    if (p->topk) {   // one scratch for both top-K steps, which run one after the other; 0 while both fit the shared-memory kernels
+        const size_t sb = ag_select_topk_workspace_bytes(&p->plan, p->cand_cap, shape ? p->M : cfg->num_features);
+        const size_t fb = shape ? ag_affine_shape_filter_topk_workspace_bytes(cfg->B, p->M) : 0;
+        p->sel_bytes = sb > fb ? sb : fb;
+    }
     p->off_sel = take(p->sel_bytes);
     p->total = o;
     p->launches = 0;
@@ -161,22 +168,27 @@ int ag_pipeline_create(const ag_pipeline_config_t* cfg, const ag_net_t* affnet, 
     AG_REQUIRE(cfg && affnet && hardnet && out, "NULL argument");
     AG_REQUIRE(!cfg->do_ori || orinet, "do_ori needs an OriNet");
     const ag_pipeline_estimators_t est = {AG_SHAPE_AFFNET, 1, 0, cfg->do_ori ? AG_ORI_ORINET : AG_ORI_NONE, 0};
-    return pipeline_create(__func__, cfg, &est, &HARDNET_DESC, affnet, orinet, hardnet, false, 0.f, out);
+    return pipeline_create(__func__, cfg, &est, &HARDNET_DESC, affnet, orinet, hardnet, false, 0.f, false, out);
 }
 
 int ag_pipeline_create_ex(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_net_t* affnet,
                           const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
-    return pipeline_create(__func__, cfg, est, &HARDNET_DESC, affnet, orinet, hardnet, false, 0.f, out);
+    return pipeline_create(__func__, cfg, est, &HARDNET_DESC, affnet, orinet, hardnet, false, 0.f, false, out);
 }
 
 int ag_pipeline_create_desc(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
                             const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
-    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, false, 0.f, out);
+    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, false, 0.f, false, out);
 }
 
 int ag_pipeline_create_th(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
                           float th, const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
-    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, true, th, out);
+    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, true, th, false, out);
+}
+
+int ag_pipeline_create_topk(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
+                            const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out) {
+    return pipeline_create(__func__, cfg, est, desc, affnet, orinet, hardnet, false, 0.f, true, out);
 }
 
 void ag_pipeline_destroy(ag_pipeline_t* p) { delete p; }
@@ -214,12 +226,18 @@ int ag_pipeline_run(ag_pipeline_t* p, const float* d_img, void* d_ws, size_t ws_
         if (p->th_mode) {
             if ((rc = ag_select_all_keypoints(&p->plan, &det, (float)c.mrSize, K, sel, p->sel_bytes, d_resp, lafs2, oct2, lvl2, d_count, stream)))
                 return rc;
+        } else if (p->topk) {
+            if ((rc = ag_select_topk_keypoints(&p->plan, &det, K, (float)c.mrSize, K, sel, p->sel_bytes, d_resp, lafs2, oct2, lvl2, d_count, stream)))
+                return rc;
         } else if ((rc = ag_select_keypoints(&p->plan, &det, K, (float)c.mrSize, K, d_resp, lafs2, oct2, lvl2, d_count, stream))) {
             return rc;
         }
     } else {
         if (p->th_mode) {
             if ((rc = ag_select_all_keypoints(&p->plan, &det, (float)c.mrSize, M, sel, p->sel_bytes, resp1, lafs1, oct1, lvl1, cnt1, stream)))
+                return rc;
+        } else if (p->topk) {
+            if ((rc = ag_select_topk_keypoints(&p->plan, &det, M, (float)c.mrSize, M, sel, p->sel_bytes, resp1, lafs1, oct1, lvl1, cnt1, stream)))
                 return rc;
         } else if ((rc = ag_select_keypoints(&p->plan, &det, M, (float)c.mrSize, M, resp1, lafs1, oct1, lvl1, cnt1, stream))) {
             return rc;
@@ -255,6 +273,10 @@ int ag_pipeline_run(ag_pipeline_t* p, const float* d_img, void* d_ws, size_t ws_
         if (p->th_mode) {
             // num_features <= 0: every survivor in order (SparseImgRepresenter.py:151-156); M = K = C
             if ((rc = ag_affine_shape_filter_all(A, resp1, lafs1, oct1, lvl1, cnt1, B, M, d_resp, lafs2, oct2, lvl2, d_count, stream))) return rc;
+        } else if (p->topk) {
+            if ((rc = ag_affine_shape_filter_topk(A, resp1, lafs1, oct1, lvl1, cnt1, B, M, K, K, sel, p->sel_bytes, d_resp, lafs2, oct2, lvl2, d_count,
+                                                  stream)))
+                return rc;
         } else if ((rc = ag_affine_shape_filter(A, resp1, lafs1, oct1, lvl1, cnt1, B, M, K, K, d_resp, lafs2, oct2, lvl2, d_count, stream))) {
             return rc;
         }

@@ -47,7 +47,7 @@ def descriptor(HardNet):
 
 class DetectDescribePipeline:
     def __init__(self, B, H, W, AffNet, HardNet, OriNet=None, num_features=2000, border=5, mrSize=5.192, nlevels=3,
-                 init_sigma=1.6, do_ori=True, cand_cap=0, device="cuda", outputs=None, num_Baum_iters=1, th=None):
+                 init_sigma=1.6, do_ori=True, cand_cap=0, device="cuda", outputs=None, num_Baum_iters=1, th=None, large_k=False):
         """outputs: optional list of (lafs [B,K,2,3], desc [B,K,128], count [B] int32) CUDA tensors, one tuple per output slot, that the
         kernels write into directly (e.g. DescriptorExchange.outputs(): the blocks an all-gather sends); default: one private slot.
         AffNet / OriNet / do_ori / num_Baum_iters select the estimators as ScaleSpaceAffinePatchExtractor does (see `estimators`):
@@ -55,8 +55,12 @@ class DetectDescribePipeline:
         HardNet may be a SIFTNet: the descriptors are then SIFTNet's at its patch size and clipval, and no checkpoint is needed.
         th: the reference's threshold mode (ScaleSpaceAffinePatchExtractor(th=th): -1 in hesaffnet.py, 28.41 its HessianAffine default):
         every keypoint above th is kept in (octave, level, raster) order, with no top-K, and num_features is the per-image capacity C of
-        the outputs [B,C,..]; an image with more keypoints than C gets count -1 (see check())."""
+        the outputs [B,C,..]; an image with more keypoints than C gets count -1 (see check()).
+        large_k: accept any num_features (ag_pipeline_create_topk).  By default the top-K steps are limited to what they sort in shared
+        memory (num_features <= 10923 with a shape step, <= 16384 without); with large_k the same kernels run up to those sizes, with the
+        same workspace, launches and outputs, and a global-memory sort runs above them.  Ignored in threshold mode, which has no limit."""
         self.th = None if th is None else float(th)
+        self.large_k = bool(large_k)
         self.cfg = L.PipelineConfig(B, H, W, num_features, nlevels, border, float(init_sigma), float(mrSize), 1 if do_ori else 0, cand_cap)
         self.est, aff, ori = estimators(AffNet, OriNet, do_ori, num_Baum_iters)
         self.desc_cfg, hard = descriptor(HardNet)
@@ -93,7 +97,9 @@ class DetectDescribePipeline:
             L.lib().ag_pipeline_destroy(self._h)
             self._h = None
         h = C.c_void_p()
-        if self.th is None:
+        if self.th is None and self.large_k:
+            L.check(L.lib().ag_pipeline_create_topk(C.byref(self.cfg), C.byref(self.est), C.byref(self.desc_cfg), hs[0], hs[1], hs[2], C.byref(h)))
+        elif self.th is None:
             L.check(L.lib().ag_pipeline_create_desc(C.byref(self.cfg), C.byref(self.est), C.byref(self.desc_cfg), hs[0], hs[1], hs[2], C.byref(h)))
         else:
             L.check(L.lib().ag_pipeline_create_th(C.byref(self.cfg), C.byref(self.est), C.byref(self.desc_cfg), self.th, hs[0], hs[1], hs[2],

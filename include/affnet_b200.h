@@ -122,7 +122,7 @@ int ag_detect_level_from_responses(const float* d_low, const float* d_cur, const
  * out_cap bounds the rows written: when it is below the number the rule above selects, the first out_cap rows of that answer
  * are returned in the same order (the out_cap highest by (response desc, seq asc) when sorted, else the out_cap first in
  * (octave, level, raster) order), deterministically.  min(num_features, out_cap) (out_cap when num_features <= 0) may not
- * exceed 16384 (shared-memory sort): larger requests return AG_ERR_CAPACITY and write nothing.
+ * exceed 16384 (shared-memory sort): larger requests return AG_ERR_CAPACITY and write nothing (ag_select_topk_keypoints has no limit).
  * a_scale multiplies the A part of the LAF (mrSize; SparseImgRepresenter.py:198).
  * Outputs [B, out_cap(,..)]: resp, LAFs (normalised), octave idx, level idx (= detection level-1); d_count[b] = -1 if the
  * candidate list of image b overflowed ws->cand_cap (the caller should retry with a larger capacity). */
@@ -143,6 +143,19 @@ size_t ag_select_all_workspace_bytes(const ag_pyramid_plan_t* plan, int cand_cap
 int ag_select_all_keypoints(const ag_pyramid_plan_t* plan, const ag_detect_ws_t* ws, float a_scale, int out_cap,
                             void* d_scratch, size_t scratch_bytes, float* d_resp, float* d_lafs, int* d_oct, int* d_lvl,
                             int* d_count, void* stream);
+
+/* Top-K selection at any count: the rule, order, out_cap truncation and outputs of ag_select_keypoints without its 16384 limit.  When
+ * min(num_features, out_cap) (out_cap when num_features <= 0) is at most 16384 it runs ag_select_keypoints itself (bit-identical by
+ * construction; no scratch is needed).  Above that a cluster radix select of the cut key, a compaction and a global-memory sort (shared-memory
+ * tiles, then merge passes) produce the same answer: the number of launches is fixed on the host from out_cap and num_features, and each
+ * launch reads the device counts (no host synchronisation, CUDA-graph capturable).  In that regime an image whose candidate list overflowed
+ * ws->cand_cap gets d_count[b] = -1 and nothing of it is written.
+ * d_scratch: ag_select_topk_workspace_bytes(plan, ws->cand_cap, out_cap) bytes, 256-B aligned, any content (0 when out_cap <= 16384, else
+ * about B * out_cap * 24 bytes); d_scratch may be NULL when scratch_bytes is 0.  AG_ERR_CAPACITY for a smaller scratch, before any CUDA call. */
+size_t ag_select_topk_workspace_bytes(const ag_pyramid_plan_t* plan, int cand_cap, int out_cap);
+int ag_select_topk_keypoints(const ag_pyramid_plan_t* plan, const ag_detect_ws_t* ws, int num_features, float a_scale, int out_cap,
+                             void* d_scratch, size_t scratch_bytes, float* d_resp, float* d_lafs, int* d_oct, int* d_lvl, int* d_count,
+                             void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Affine bilinear sampler          replaces extract_patches / generate_patch_grid_from_normalized_LAFs
@@ -254,7 +267,8 @@ int ag_net_forward_pyr(const ag_net_t* net, const ag_pyramid_plan_t* plan, const
  * torch.topk returns it in the reference.  All arithmetic is the reference's fp32 CPU arithmetic, without fused multiply-adds
  * (tests/test_gpu_geometry.py pins it bit for bit).
  * Outputs are compacted: d_resp_out/d_lafs_out/d_oct_out/d_lvl_out [B,out_cap..], d_count_out [B]; only the first d_count_out[b] rows
- * of image b are written, and d_count_out[b] = -1 where d_count_in[b] < 0.  cap above 16384 returns AG_ERR_CAPACITY and writes nothing. */
+ * of image b are written, and d_count_out[b] = -1 where d_count_in[b] < 0.  cap above 16384 returns AG_ERR_CAPACITY and writes nothing
+ * (ag_affine_shape_filter_topk has no limit). */
 int ag_affine_shape_filter(const float* d_A, const float* d_resp, const float* d_lafs, const int* d_oct,
                            const int* d_lvl, const int* d_count_in, int B, int cap, int num_features, int out_cap,
                            float* d_resp_out, float* d_lafs_out, int* d_oct_out, int* d_lvl_out, int* d_count_out,
@@ -266,6 +280,16 @@ int ag_affine_shape_filter(const float* d_A, const float* d_resp, const float* d
 int ag_affine_shape_filter_all(const float* d_A, const float* d_resp, const float* d_lafs, const int* d_oct, const int* d_lvl,
                                const int* d_count_in, int B, int cap, float* d_resp_out, float* d_lafs_out, int* d_oct_out,
                                int* d_lvl_out, int* d_count_out, void* stream);
+/* Top-K shape filter at any cap: the rule, order, responses and counts of ag_affine_shape_filter without its 16384 limit.  At cap <= 16384
+ * it runs ag_affine_shape_filter itself (bit-identical by construction; no scratch is needed).  Above, one pass writes every row's keep flag
+ * and key, then the global-memory top-K of ag_select_topk_keypoints picks and sorts the rows, and the writer recomputes them with the same
+ * device arithmetic.  A memset and a number of launches fixed on the host from cap, num_features and out_cap; CUDA-graph capturable.
+ * d_scratch: ag_affine_shape_filter_topk_workspace_bytes(B, cap) bytes, 256-B aligned, any content (0 when cap <= 16384, else about
+ * B * cap * 29 bytes); d_scratch may be NULL when scratch_bytes is 0.  AG_ERR_CAPACITY for a smaller scratch, before any CUDA call. */
+size_t ag_affine_shape_filter_topk_workspace_bytes(int B, int cap);
+int ag_affine_shape_filter_topk(const float* d_A, const float* d_resp, const float* d_lafs, const int* d_oct, const int* d_lvl,
+                                const int* d_count_in, int B, int cap, int num_features, int out_cap, void* d_scratch, size_t scratch_bytes,
+                                float* d_resp_out, float* d_lafs_out, int* d_oct_out, int* d_lvl_out, int* d_count_out, void* stream);
 
 /* LAF_A <- LAF_A * R  then (optionally) denormalise to pixels of a WxH image.  d_lafs [n,2,3] in/out. */
 int ag_lafs_apply_rotation(float* d_lafs, const float* d_R, int n, void* stream);
@@ -421,7 +445,7 @@ typedef struct {
 } ag_pipeline_estimators_t;
 /* Nets the mode does not use may be NULL and are ignored.  AG_ERR_INVALID: a missing net for the chosen mode, num_baum_iters < 1 with
  * a shape estimator, a patch size outside 3..41, cfg->do_ori inconsistent with est->ori.  AG_ERR_CAPACITY: a prefilter of
- * int(1.5 K) > 16384 keypoints with a shape estimator (K > 10923), K > 16384 without. */
+ * int(1.5 K) > 16384 keypoints with a shape estimator (K > 10923), K > 16384 without (ag_pipeline_create_topk has no such limit). */
 int ag_pipeline_create_ex(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_net_t* affnet,
                           const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
 
@@ -451,6 +475,12 @@ int ag_pipeline_create_desc(const ag_pipeline_config_t* cfg, const ag_pipeline_e
  * AG_ERR_INVALID (before any CUDA call) for th NaN or infinite and for everything ag_pipeline_create_desc refuses except its K limits. */
 int ag_pipeline_create_th(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
                           float th, const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
+/* ag_pipeline_create_desc without its K limits: the selection and the shape filter run ag_select_topk_keypoints and
+ * ag_affine_shape_filter_topk, so any K is accepted.  The kernels are chosen by size: while the prefilter (int(1.5 K) with a shape step, K
+ * without) is at most 16384 the pipeline is ag_pipeline_create_desc's - the same workspace bytes, launch count and outputs.  Above, the
+ * workspace adds one scratch region shared by the two steps. */
+int ag_pipeline_create_topk(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
+                            const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
 void ag_pipeline_destroy(ag_pipeline_t* p);
 size_t ag_pipeline_workspace_bytes(const ag_pipeline_t* p);
 const ag_pyramid_plan_t* ag_pipeline_plan(const ag_pipeline_t* p);
