@@ -101,6 +101,7 @@ PROTOTYPES = {
     "ag_debug_pyramid_mode": (i32, [i32]),
     "ag_debug_tcx_layer": (i32, [vp, vp, i32, i32, vp, vp, sz, vp]),
     "ag_debug_libm": (i32, [vp, vp, i32, vp, vp, vp, vp]),
+    "ag_debug_tanhf": (i32, [vp, i32, vp, vp]),
     "ag_debug_orientation_hist_pyr": (i32, [C.POINTER(PyramidPlan), vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
     "ag_debug_baumberg_pyr": (i32, [C.POINTER(PyramidPlan), vp, vp, vp, vp, vp, i32, i32, i32, vp, vp, vp]),
     "ag_affnet_forward": (i32, [vp, vp, i32, vp, i32, vp, vp, sz, vp]),

@@ -63,4 +63,6 @@ int tcx_trunk_affori(const ag_net* net, const tc::FirstSrc& src, int n, int grou
 int tcx_trunk_hardnet(const ag_net* net, const tc::FirstSrc& src, int n, int group, const int* count, void* bufA, void* bufB, void* headbuf,
                       cudaStream_t st, int upto, int bf16 = 0);
 int tc_hardnet_head(const ag_net* net, const void* headbuf, int n, int group, const int* count, float* out, cudaStream_t st, int bf16 = 0);
+// fp32 SIMT engine (nets_simt.cu): conv layers 1..upto on materialised patches, layer upto's fp32 NCHW output copied to out
+int simt_trunk_layer(const ag_net* net, const float* patches, int n, int upto, float* out, void* ws, size_t ws_bytes, cudaStream_t st);
 }  // namespace ag

@@ -549,26 +549,27 @@ size_t ag_net_workspace_bytes(int kind, int n) {
 
 namespace ag {
 
+// Layers 1..upto (odd layers write a, even layers b).
 static int trunk_affnet(const ag_net* net, const float* patches, int n, int group, const int* count, float* a, float* b,
-                        cudaStream_t st) {
+                        cudaStream_t st, int upto = 6) {
     int rc;
-    if ((rc = launch_conv<1, 16, 32, 1, 16, 1, true>(patches, a, net->d_w[0], net->d_b[0], n, group, count, st))) return rc;
-    if ((rc = launch_conv<16, 16, 32, 1, 16, 16, false>(a, b, net->d_w[1], net->d_b[1], n, group, count, st))) return rc;
-    if ((rc = launch_conv<16, 32, 32, 2, 32, 16, false>(b, a, net->d_w[2], net->d_b[2], n, group, count, st))) return rc;
-    if ((rc = launch_conv<32, 32, 16, 1, 32, 32, false>(a, b, net->d_w[3], net->d_b[3], n, group, count, st))) return rc;
-    if ((rc = launch_conv<32, 64, 16, 2, 64, 32, false>(b, a, net->d_w[4], net->d_b[4], n, group, count, st))) return rc;
+    if ((rc = launch_conv<1, 16, 32, 1, 16, 1, true>(patches, a, net->d_w[0], net->d_b[0], n, group, count, st)) || upto <= 1) return rc;
+    if ((rc = launch_conv<16, 16, 32, 1, 16, 16, false>(a, b, net->d_w[1], net->d_b[1], n, group, count, st)) || upto <= 2) return rc;
+    if ((rc = launch_conv<16, 32, 32, 2, 32, 16, false>(b, a, net->d_w[2], net->d_b[2], n, group, count, st)) || upto <= 3) return rc;
+    if ((rc = launch_conv<32, 32, 16, 1, 32, 32, false>(a, b, net->d_w[3], net->d_b[3], n, group, count, st)) || upto <= 4) return rc;
+    if ((rc = launch_conv<32, 64, 16, 2, 64, 32, false>(b, a, net->d_w[4], net->d_b[4], n, group, count, st)) || upto <= 5) return rc;
     if ((rc = launch_conv<64, 64, 8, 1, 64, 32, false>(a, b, net->d_w[5], net->d_b[5], n, group, count, st))) return rc;
     return AG_OK;  // features in b: [n,64,8,8]
 }
 
 static int trunk_hardnet(const ag_net* net, const float* patches, int n, int group, const int* count, float* a, float* b,
-                         cudaStream_t st) {
+                         cudaStream_t st, int upto = 6) {
     int rc;
-    if ((rc = launch_conv<1, 32, 32, 1, 32, 1, true>(patches, a, net->d_w[0], net->d_b[0], n, group, count, st))) return rc;
-    if ((rc = launch_conv<32, 32, 32, 1, 32, 32, false>(a, b, net->d_w[1], net->d_b[1], n, group, count, st))) return rc;
-    if ((rc = launch_conv<32, 64, 32, 2, 64, 32, false>(b, a, net->d_w[2], net->d_b[2], n, group, count, st))) return rc;
-    if ((rc = launch_conv<64, 64, 16, 1, 64, 32, false>(a, b, net->d_w[3], net->d_b[3], n, group, count, st))) return rc;
-    if ((rc = launch_conv<64, 128, 16, 2, 128, 16, false>(b, a, net->d_w[4], net->d_b[4], n, group, count, st))) return rc;
+    if ((rc = launch_conv<1, 32, 32, 1, 32, 1, true>(patches, a, net->d_w[0], net->d_b[0], n, group, count, st)) || upto <= 1) return rc;
+    if ((rc = launch_conv<32, 32, 32, 1, 32, 32, false>(a, b, net->d_w[1], net->d_b[1], n, group, count, st)) || upto <= 2) return rc;
+    if ((rc = launch_conv<32, 64, 32, 2, 64, 32, false>(b, a, net->d_w[2], net->d_b[2], n, group, count, st)) || upto <= 3) return rc;
+    if ((rc = launch_conv<64, 64, 16, 1, 64, 32, false>(a, b, net->d_w[3], net->d_b[3], n, group, count, st)) || upto <= 4) return rc;
+    if ((rc = launch_conv<64, 128, 16, 2, 128, 16, false>(b, a, net->d_w[4], net->d_b[4], n, group, count, st)) || upto <= 5) return rc;
     if ((rc = launch_conv<128, 128, 8, 1, 128, 16, false>(a, b, net->d_w[5], net->d_b[5], n, group, count, st))) return rc;
     return AG_OK;  // features in b: [n,128,8,8]
 }
@@ -610,6 +611,24 @@ static int split_ws(int kind, int n, void* d_ws, size_t ws_bytes, float** a, flo
     *a = (float*)d_ws;
     *b = (float*)((char*)d_ws + need / 2);
     return AG_OK;
+}
+
+int simt_trunk_layer(const ag_net* net, const float* patches, int n, int upto, float* out, void* ws, size_t ws_bytes, cudaStream_t st) {
+    float *a, *b;
+    int rc = split_ws(net->kind, n, ws, ws_bytes, &a, &b);
+    if (rc) return rc;
+    rc = net->kind == AG_NET_HARDNET ? trunk_hardnet(net, patches, n, n, nullptr, a, b, st, upto)
+                                     : trunk_affnet(net, patches, n, n, nullptr, a, b, st, upto);
+    if (rc) return rc;
+    const LayerCfg& c = (net->kind == AG_NET_HARDNET ? kHardCfg : kAffCfg)[upto - 1];
+    const size_t bytes = (size_t)n * c.cout * (c.hin / c.stride) * (c.hin / c.stride) * sizeof(float);
+    return check_cuda(cudaMemcpyAsync(out, (upto & 1) ? a : b, bytes, cudaMemcpyDeviceToDevice, st), "copy layer output");
+}
+
+// tanhf as the AffNet and OriNet heads call it, one element per thread, compiled with this file's flags (ag_debug_tanhf).
+__global__ void tanhf_probe_kernel(const float* __restrict__ x, int n, float* __restrict__ y) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) y[i] = tanhf(x[i]);
 }
 
 }  // namespace ag
@@ -718,6 +737,14 @@ int ag_net_forward_pyr(const ag_net_t* net, const ag_pyramid_plan_t* plan, const
     if (net->kind == AG_NET_AFFNET) return affnet_impl(net, nullptr, &src, n, d_count, cap, d_out, d_ws, ws_bytes, stream);
     if (net->kind == AG_NET_ORINET) return orinet_impl(net, nullptr, &src, n, d_count, cap, d_out, nullptr, d_ws, ws_bytes, stream);
     return hardnet_impl(net, nullptr, &src, n, d_count, cap, d_out, d_ws, ws_bytes, stream);
+}
+
+int ag_debug_tanhf(const float* d_x, int n, float* d_y, void* stream) {
+    AG_REQUIRE(d_x && d_y, "NULL argument");
+    if (n <= 0) return AG_OK;
+    tanhf_probe_kernel<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(d_x, n, d_y);
+    AG_CHECK_LAUNCH("tanhf_probe_kernel");
+    return AG_OK;
 }
 
 }  // extern "C"

@@ -247,13 +247,16 @@ using namespace ag;
 
 extern "C" {
 
-// Developer diagnostic (tests/test_gpu_tcx.py, tests/test_gpu_net_bounds.py): run the second-generation trunk of `net` with the
-// handle's engine (ENGINE_TC2_BF16: the bf16 HardNet trunk; any other engine: the fp16 one) on materialised patches [n,32,32] up to conv
-// layer `upto` (2..6) and decode that layer's output (fp16 / bf16 hi [+ lo] planes in its HBM layout; layer 6: the head operand) to
-// fp32 [n][C][H][H].  d_ws: ag_net_workspace_bytes().
+// Developer diagnostic (tests/test_gpu_tcx.py, tests/test_gpu_net_bounds.py, tests/test_gpu_simt_exact.py): run the trunk of `net` with
+// the handle's engine on materialised patches [n,32,32] up to conv layer `upto` and return that layer's output as fp32 [n][C][H][H].
+// ENGINE_SIMT: the fp32 trunk (upto 1..6), its output copied as it is.  Otherwise the second-generation trunk (ENGINE_TC2_BF16: the bf16
+// HardNet trunk; any other engine: the fp16 one; upto 2..6), that layer's output decoded from its fp16 / bf16 hi [+ lo] planes in its HBM
+// layout (layer 6: the head operand).  d_ws: ag_net_workspace_bytes().
 int ag_debug_tcx_layer(const ag_net_t* net, const float* d_patches, int n, int upto, float* d_out, void* d_ws, size_t ws_bytes, void* stream) {
     AG_REQUIRE(net && d_patches && d_out && d_ws, "NULL argument");
-    AG_REQUIRE(upto >= 2 && upto <= 6 && n >= 1, "layer out of range");
+    const bool simt = net->engine == AG_ENGINE_SIMT;
+    AG_REQUIRE(upto >= (simt ? 1 : 2) && upto <= 6 && n >= 1, "layer out of range");
+    if (simt) return simt_trunk_layer(net, d_patches, n, upto, d_out, d_ws, ws_bytes, (cudaStream_t)stream);
     const size_t act = align_up(tcx_act_bytes(n), 256);
     AG_REQUIRE(ws_bytes >= ag_net_workspace_bytes(net->kind, n), "workspace too small");
     cudaStream_t st = (cudaStream_t)stream;

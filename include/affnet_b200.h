@@ -209,10 +209,14 @@ int ag_net_get_engine(const ag_net_t* net);
 /* Developer switch: 1 = ag_pyramid_build runs one launch per octave (pyramid_fused.cuh: bit-identical, measured slower), 0 = one
  * launch per level (default).  Returns the previous mode. */
 int ag_debug_pyramid_mode(int fused);
-/* Developer diagnostic: run the second-generation trunk with the handle's engine (ENGINE_TC2_BF16: bf16 operands, HardNet; otherwise
- * fp16) on materialised patches [n,32,32] up to conv layer `upto` (2..6) and decode that layer's activations (hi [+ lo] planes in the
- * engine's HBM layout; layer 6: the 8x8 head's operand) to fp32 [n,C,H,H].  d_ws: ag_net_workspace_bytes(). */
+/* Developer diagnostic: run the trunk with the handle's engine on materialised patches [n,32,32] up to conv layer `upto` and return that
+ * layer's activations as fp32 [n,C,H,H].  ENGINE_SIMT: the exact-fp32 trunk, upto 1..6, its fp32 output as it is.  Any other engine: the
+ * second-generation trunk (ENGINE_TC2_BF16: bf16 operands, HardNet; otherwise fp16), upto 2..6, its hi [+ lo] planes in the engine's HBM
+ * layout (layer 6: the 8x8 head's operand) decoded.  d_ws: ag_net_workspace_bytes(). */
 int ag_debug_tcx_layer(const ag_net_t* net, const float* d_patches, int n, int upto, float* d_out, void* d_ws, size_t ws_bytes, void* stream);
+/* Developer diagnostic: d_y[i] = tanhf(d_x[i]) for i < n, compiled with the flags of the exact-fp32 engine's AffNet and OriNet heads.
+ * Lets a test restate those heads bit for bit (tests/nets_simt_restated.py); not used by the pipeline. */
+int ag_debug_tanhf(const float* d_x, int n, float* d_y, void* stream);
 /* Developer diagnostic: the device libm calls of the hand-crafted estimators, compiled with their flags, one element per thread:
  * d_atan2[i] = atan2f(d_y[i], d_x[i]), d_cos[i] = cosf(d_x[i]), d_sin[i] = sinf(d_x[i]) for i < n.  Lets a test restate the estimators
  * bit for bit (tests/handcrafted_restated.py); not used by the pipeline. */

@@ -125,11 +125,12 @@ def operands(kind, sd, fmt="fp16", sw2=1, sw3=1):
 
 
 # ---- input normalisation, bit for bit (tcx_first.cuh producers) -----------------------------------------------------------------
-def _butterfly(a):
-    """xor-shuffle sum over the last axis (32 lanes), as every lane sees it after offsets 16, 8, 4, 2, 1."""
+def _butterfly(a, add=None):
+    """xor-shuffle sum over the last axis (32 lanes), as every lane sees it after offsets 16, 8, 4, 2, 1.  add(x, y): the fp32 sum (default
+    the arrays' own +, for fp32 arrays)."""
     idx = np.arange(32)
     for o in (16, 8, 4, 2, 1):
-        a = a + a[..., idx ^ o]
+        a = a + a[..., idx ^ o] if add is None else add(a, a[..., idx ^ o])
     return a[..., 0]
 
 

@@ -68,6 +68,23 @@ def test_argument_validation_and_error_text(L):
     assert b"blob has 10 floats" in lib.ag_last_error()
 
 
+def test_debug_probe_refusals(L):
+    """The developer diagnostics refuse NULL arguments before any CUDA call, naming themselves; an empty probe is a no-op."""
+    lib = L.lib()
+    buf = np.zeros(4, np.float32)
+    p = buf.ctypes.data_as(C.c_void_p)
+    assert "ag_debug_tanhf" in L.PROTOTYPES
+    for x, y in ((None, p), (p, None), (None, None)):
+        assert lib.ag_debug_tanhf(x, 4, y, None) == -1
+        assert lib.ag_last_error() == b"ag_debug_tanhf: NULL argument"
+    assert lib.ag_debug_tanhf(None, 0, None, None) == -1              # NULL is refused before the size is looked at
+    assert lib.ag_debug_tanhf(p, 0, p, None) == 0 and lib.ag_debug_tanhf(p, -3, p, None) == 0
+    assert lib.ag_debug_tcx_layer(None, p, 1, 1, p, p, 1 << 20, None) == -1
+    assert lib.ag_last_error() == b"ag_debug_tcx_layer: NULL argument"
+    assert lib.ag_debug_libm(p, p, 4, p, None, p, None) == -1
+    assert lib.ag_last_error() == b"ag_debug_libm: NULL argument"
+
+
 def test_blob_sizes_match_checkpoints(L):
     from helpers import load_weights
     W = load_weights()
