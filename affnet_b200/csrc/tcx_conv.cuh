@@ -324,7 +324,7 @@ __device__ __forceinline__ void xconv_block_epilogue(const float* d, const XArgs
 #pragma unroll
     for (int h = 0; h < 2; h++) {
         const int y = b * 4 + wq, x = 2 * xi + h, pi = PAIR ? 2 * u + (i >> 2) : u;   // a warp's 16 rows are image row y
-        ok[h] = xpatch_valid(a, pi);
+        ok[h] = !PAIR || xpatch_valid(a, pi);   // a single-patch unit: the callers only run valid ones
         if (OUT == L_HEAD) {
             obase[h] = reinterpret_cast<unsigned char*>(a.out) + (((size_t)(pi >> 7) * (HOUT * HOUT * COUT / 8) + (size_t)(y * HOUT + x) * (COUT / 8)) * 128 + (pi & 127)) * 16;
             lo_off = (size_t)((a.n + 127) >> 7) * (HOUT * HOUT * COUT / 8) * 128 * 16;

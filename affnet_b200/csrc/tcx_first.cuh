@@ -309,21 +309,20 @@ __global__ void __launch_bounds__(512, 1) tcx_first_kernel(const XArgs a, const 
 #pragma unroll
                 for (int j = 0; j < NT / 8; j++) {
                     const int c = j * 8 + 2 * (lane & 3);
+                    // neighbours (tcx_conv.cuh, frag_left_even) of both columns: x0 - 1 from lane - 4, x0 + 2 from lane + 4, or across
+                    // the two warps of the image row from shared memory (one 8-byte load each)
+                    float2 l0 = make_float2(frag_left_even(d[4 * j + 2], lane), frag_left_even(d[4 * j + 3], lane));
+                    float2 r1 = make_float2(frag_right_odd(d[4 * (j + 2 * NT / 8)], lane), frag_right_odd(d[4 * (j + 2 * NT / 8) + 1], lane));
+                    if (from_prev) l0 = *reinterpret_cast<const float2*>(xw + ((wq - 1) * 2 + 0) * NT + c);
+                    if (from_next) r1 = *reinterpret_cast<const float2*>(xw + ((wq + 1) * 2 + 1) * NT + c);
                     float v[2][2];
 #pragma unroll
                     for (int e = 0; e < 2; e++) {
-                        const float c00 = d[4 * j + e], c01 = d[4 * j + 2 + e];
-                        const float c10 = d[4 * (j + NT / 8) + e], c11 = d[4 * (j + NT / 8) + 2 + e];
-                        const float c20 = d[4 * (j + 2 * NT / 8) + e], c21 = d[4 * (j + 2 * NT / 8) + 2 + e];
-                        // neighbours (tcx_conv.cuh, frag_left_even): x0 - 1 from lane - 4, x0 + 2 from lane + 4, or across the two
-                        // warps of the image row through shared memory
-                        float l0 = frag_left_even(c01, lane), r1 = frag_right_odd(c20, lane);
-                        const float l1 = c00, r0 = c21;
-                        if (from_prev) l0 = xw[((wq - 1) * 2 + 0) * NT + c + e];
-                        if (from_next) r1 = xw[((wq + 1) * 2 + 1) * NT + c + e];
+                        const float l1 = d[4 * j + e], c10 = d[4 * (j + NT / 8) + e], c11 = d[4 * (j + NT / 8) + 2 + e], r0 = d[4 * (j + 2 * NT / 8) + 2 + e];
+                        const float le = e ? l0.y : l0.x, re = e ? r1.y : r1.x;
                         // 0/1 masks: zero padding outside the row (x = 0: h = 0 of even warps' lanes 0-3, x = 31: h = 1 of odd warps' lanes 28-31)
-                        const float acc0 = fmaf(first8 ? l0 : r0, m0, (first8 ? r0 : l0) + c10);
-                        const float acc1 = fmaf(first8 ? l1 : r1, m1, (first8 ? r1 : l1) + c11);
+                        const float acc0 = fmaf(first8 ? le : r0, m0, (first8 ? r0 : le) + c10);
+                        const float acc1 = fmaf(first8 ? l1 : re, m1, (first8 ? re : l1) + c11);
                         v[0][e] = fmaxf(fmaf(acc0, a.inv_scale, s_bias[c + e]), 0.f);
                         v[1][e] = fmaxf(fmaf(acc1, a.inv_scale, s_bias[c + e]), 0.f);
                     }
