@@ -52,18 +52,37 @@ struct DetectParams {
     int* level_emit;
 };
 
+// The larger of a and b, NaN when either is NaN (PTX max.NaN): torch.clamp and MaxPool3d keep NaN, fmaxf drops it.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+
+// The half-difference 0.5 l - 0.5 r of the reference's (0.5, 0, -0.5) filter, with its zero tap: + 0 * c changes no finite value
+// beyond the sign of a zero (which gxy * gxy drops) but makes the result NaN when c is infinite, as the reference's conv does.
+__device__ __forceinline__ float half_diff0(float l, float c, float r) {
+    return fmaf(0.0f, c, __fsub_rn(__fmul_rn(0.5f, l), __fmul_rn(0.5f, r)));
+}
+
 __device__ __forceinline__ float hessian_at(const float (*s)[PW + 1], int py, int px, float s4, float th) {
-    // (py,px) indexes the pyramid window; neighbours already hold replicate-clamped values.
+    // (py,px) indexes the pyramid window; neighbours already hold replicate-clamped values.  gxy keeps the zero taps of both
+    // (0.5, 0, -0.5) filters, so an infinite pixel gives the reference's NaN responses (HandCraftedModules.py:74-77).
     const float c = s[py][px];
     const float gxx = __fadd_rn(__fsub_rn(s[py][px - 1], __fmul_rn(2.0f, c)), s[py][px + 1]);
     const float gyy = __fadd_rn(__fsub_rn(s[py - 1][px], __fmul_rn(2.0f, c)), s[py + 1][px]);
-    const float gxa = __fsub_rn(__fmul_rn(0.5f, s[py - 1][px - 1]), __fmul_rn(0.5f, s[py - 1][px + 1]));
-    const float gxb = __fsub_rn(__fmul_rn(0.5f, s[py + 1][px - 1]), __fmul_rn(0.5f, s[py + 1][px + 1]));
-    const float gxy = __fsub_rn(__fmul_rn(0.5f, gxa), __fmul_rn(0.5f, gxb));
+    const float gxa = half_diff0(s[py - 1][px - 1], s[py - 1][px], s[py - 1][px + 1]);
+    const float gxm = half_diff0(s[py][px - 1], c, s[py][px + 1]);
+    const float gxb = half_diff0(s[py + 1][px - 1], s[py + 1][px], s[py + 1][px + 1]);
+    const float gxy = half_diff0(gxa, gxm, gxb);
     const float det = __fsub_rn(__fmul_rn(gxx, gyy), __fmul_rn(gxy, gxy));
     const float r = __fmul_rn(fabsf(det), s4);
-    return fmaxf(__fsub_rn(r, th), 0.0f);  // torch.clamp(resp - th, min=0), SparseImgRepresenter.py:77
+    return fmax_nan(__fsub_rn(r, th), 0.0f);  // torch.clamp(resp - th, min=0) keeps NaN, SparseImgRepresenter.py:77
 }
+
+// An NMS value that becomes a candidate: nonzero and not NaN.  The reference emits its NaN survivors (NaN and infinite centres,
+// `0 * x`); this detector never does (DESIGN.md §2).
+__device__ __forceinline__ bool emits(float v) { return fabsf(v) > 0.0f; }
 
 __device__ __forceinline__ uint8_t float_to_u8_wrap(float v) {
     // torch-CPU float32 -> uint8: truncate toward zero, keep the low 8 bits (Q4).
@@ -152,10 +171,10 @@ __global__ void __launch_bounds__(DNT) detect_level_kernel(const DetectParams P)
 #pragma unroll
                     for (int dx = -1; dx <= 1; dx++) {
                         const int ny = gy + dy, nx = gx + dx;
-                        if (ny >= 0 && ny < h && nx >= 0 && nx < w) m = fmaxf(m, s_resp[d][ly + 1 + dy][lx + 1 + dx]);
+                        if (ny >= 0 && ny < h && nx >= 0 && nx < w) m = fmax_nan(m, s_resp[d][ly + 1 + dy][lx + 1 + dx]);
                     }
-            // NMS3d: ((x - m + eps) > 0) * x      HandCraftedModules.py:220
-            float nms = (__fadd_rn(__fsub_rn(x, m), 1e-5f) > 0.f) ? x : 0.f;
+            // NMS3d: ((x - m + eps) > 0) * x      HandCraftedModules.py:220  (0 * x: NaN at a NaN or infinite centre)
+            float nms = (__fadd_rn(__fsub_rn(x, m), 1e-5f) > 0.f) ? x : __fmul_rn(0.f, x);
             // zero_response_at_border(int(mrSize))   Utils.py:140-148
             if (!border_ok || gy < P.mr_border || gy >= h - P.mr_border || gx < P.mr_border || gx >= w - P.mr_border) nms = 0.f;
             const size_t p = img_off + (size_t)gy * w + gx;
@@ -164,6 +183,7 @@ __global__ void __launch_bounds__(DNT) detect_level_kernel(const DetectParams P)
             if (O.P_out) O.P_out[p] = om;
             if (O.T_out) O.T_out[p] = float_to_u8_wrap(__fadd_rn((float)om, val));  // (octaveMap.float()+resp).byte()  :256
             n_pos += (val > 0.f);
+            if (!emits(val)) val = 0.f;    // NaN survivors update the octave map (to 0) but are no candidates
             n_emit += (val != 0.f);
         }
         vals[k] = val;
@@ -307,12 +327,12 @@ __global__ void __launch_bounds__(DNT) detect_fused_kernel(const FusedParams P) 
             s_resp[d][ly][lx] = (gy >= 0 && gy < h && gx >= 0 && gx < w) ? hessian_at(s_a[d], ly + 1, lx + 1, O.s4[d], P.th) : 0.f;
         }
     __syncthreads();
-    // 3. separable 3x3 max: row pass into the (dead) pyramid windows.  Zero padding is exact: responses are >= 0 and the
-    //    centre always takes part in the max.
+    // 3. separable 3x3 max: row pass into the (dead) pyramid windows.  Zero padding is exact: responses are >= 0 (or NaN) and the
+    //    centre always takes part in the max.  max.NaN: a NaN anywhere in the window suppresses the centre, as MaxPool3d does.
     float (*s_rm)[RW][DT] = reinterpret_cast<float (*)[RW][DT]>(&s_a[0][0][0]);
     for (int i = threadIdx.x; i < 5 * RW * DT; i += DNT) {
         const int d = i / (RW * DT), r = i - d * RW * DT, ly = r / DT, j = r - ly * DT;
-        s_rm[d][ly][j] = fmaxf(fmaxf(s_resp[d][ly][j], s_resp[d][ly][j + 1]), s_resp[d][ly][j + 2]);
+        s_rm[d][ly][j] = fmax_nan(fmax_nan(s_resp[d][ly][j], s_resp[d][ly][j + 1]), s_resp[d][ly][j + 2]);
     }
     __syncthreads();
     // 4. per pixel: three NMS decisions, hypothesis counters, candidate slots
@@ -331,13 +351,16 @@ __global__ void __launch_bounds__(DNT) detect_fused_kernel(const FusedParams P) 
         if (gy < h && gx < w && border_ok && gy >= P.mr_border && gy < h - P.mr_border && gx >= P.mr_border && gx < w - P.mr_border) {
             float M[5];
 #pragma unroll
-            for (int d = 0; d < 5; d++) M[d] = fmaxf(fmaxf(s_rm[d][ly][lx], s_rm[d][ly + 1][lx]), s_rm[d][ly + 2][lx]);
+            for (int d = 0; d < 5; d++) M[d] = fmax_nan(fmax_nan(s_rm[d][ly][lx], s_rm[d][ly + 1][lx]), s_rm[d][ly + 2][lx]);
 #pragma unroll
             for (int q = 0; q < 3; q++) {
                 const float x = s_resp[q + 1][ly + 1][lx + 1];
-                const float m = fmaxf(fmaxf(M[q], M[q + 1]), M[q + 2]);
+                const float m = fmax_nan(fmax_nan(M[q], M[q + 1]), M[q + 2]);
                 nms[k][q] = (__fadd_rn(__fsub_rn(x, m), 1e-5f) > 0.f) ? x : 0.f;   // NMS3d, HandCraftedModules.py:220
             }
+            // The reference's NMS value is 0 * x, NaN at a NaN or infinite centre, where these kernels keep 0.  Nothing observable
+            // differs: such a value is no candidate (DESIGN.md §2), is not > 0, and turns the octave map to 0 where the map can
+            // only be 0 already (a non-finite x at level q lies in the window of level q-1, which then had no survivor there).
             const float n1 = nms[k][0], n2 = nms[k][1], n3 = nms[k][2];
             if (n1 != 0.f || n2 != 0.f || n3 != 0.f) {
                 n_emit += (n1 != 0.f) + (n2 != 0.f) + (n3 != 0.f);
@@ -456,6 +479,9 @@ struct WarpParams {
     int* variants;
 };
 
+// The register kernels drop the zero taps of the gxy filters (see hessian_at): next to an infinite pixel they give +inf where the
+// reference has NaN.  No decision differs, since an infinite and a NaN response both suppress every window they lie in and never
+// survive themselves.
 __device__ __forceinline__ float hessian_regs(float tl, float tc, float tr, float ml, float mc, float mr, float bl, float bc, float br, float s4, float th) {
     const float gxx = __fadd_rn(__fsub_rn(ml, __fmul_rn(2.0f, mc)), mr);
     const float gyy = __fadd_rn(__fsub_rn(tc, __fmul_rn(2.0f, mc)), bc);
@@ -463,7 +489,7 @@ __device__ __forceinline__ float hessian_regs(float tl, float tc, float tr, floa
     const float gxb = __fsub_rn(__fmul_rn(0.5f, bl), __fmul_rn(0.5f, br));
     const float gxy = __fsub_rn(__fmul_rn(0.5f, gxa), __fmul_rn(0.5f, gxb));
     const float det = __fsub_rn(__fmul_rn(gxx, gyy), __fmul_rn(gxy, gxy));
-    return fmaxf(__fsub_rn(__fmul_rn(fabsf(det), s4), th), 0.0f);
+    return fmax_nan(__fsub_rn(__fmul_rn(fabsf(det), s4), th), 0.0f);
 }
 
 constexpr int WRING = 8;   // ring of pyramid rows per warp (cp.async prefetch distance WPD, 3 rows live)
@@ -579,7 +605,7 @@ __global__ void __launch_bounds__(WNT) detect_warp_kernel(const WarpParams P) {
                 if (lane == 0) l = 0.f;
                 if (lane == 31) rr = 0.f;
                 rs[d][2] = r;
-                rmx[d][2] = fmaxf(fmaxf(l, r), rr);
+                rmx[d][2] = fmax_nan(fmax_nan(l, r), rr);
                 hs[d][2] = (l + r) + rr;
                 hx[d][2] = fmaf(1.5f, rr, fmaf(0.5f, r, -0.5f * l));   // x offsets [-0.5, 0.5, 1.5] (Q2)
             }
@@ -590,11 +616,11 @@ __global__ void __launch_bounds__(WNT) detect_warp_kernel(const WarpParams P) {
             if (col_ok && y >= P.mr_border && y < h - P.mr_border) {
                 float M[5];
 #pragma unroll
-                for (int d = 0; d < 5; d++) M[d] = fmaxf(fmaxf(rmx[d][0], rmx[d][1]), rmx[d][2]);
+                for (int d = 0; d < 5; d++) M[d] = fmax_nan(fmax_nan(rmx[d][0], rmx[d][1]), rmx[d][2]);
                 const float x1 = rs[1][1], x2 = rs[2][1], x3 = rs[3][1];
-                n1 = (__fadd_rn(__fsub_rn(x1, fmaxf(fmaxf(M[0], M[1]), M[2])), 1e-5f) > 0.f) ? x1 : 0.f;   // NMS3d, HandCraftedModules.py:220
-                n2 = (__fadd_rn(__fsub_rn(x2, fmaxf(fmaxf(M[1], M[2]), M[3])), 1e-5f) > 0.f) ? x2 : 0.f;
-                n3 = (__fadd_rn(__fsub_rn(x3, fmaxf(fmaxf(M[2], M[3]), M[4])), 1e-5f) > 0.f) ? x3 : 0.f;
+                n1 = (__fadd_rn(__fsub_rn(x1, fmax_nan(fmax_nan(M[0], M[1]), M[2])), 1e-5f) > 0.f) ? x1 : 0.f;   // NMS3d, HandCraftedModules.py:220
+                n2 = (__fadd_rn(__fsub_rn(x2, fmax_nan(fmax_nan(M[1], M[2]), M[3])), 1e-5f) > 0.f) ? x2 : 0.f;
+                n3 = (__fadd_rn(__fsub_rn(x3, fmax_nan(fmax_nan(M[2], M[3]), M[4])), 1e-5f) > 0.f) ? x3 : 0.f;
             }
             const unsigned m1 = __ballot_sync(0xffffffffu, n1 != 0.f), m2 = __ballot_sync(0xffffffffu, n2 != 0.f), m3 = __ballot_sync(0xffffffffu, n3 != 0.f);
             if (m1 | m2 | m3) {
@@ -797,13 +823,13 @@ __global__ void __launch_bounds__(WNT, AG_DETROWS_MINB) detect_rows_kernel(const
             const float gyy = __fadd_rn(__fsub_rn(pc[d][PO], __fmul_rn(2.0f, pc[d][PM])), C);
             const float gxy = __fsub_rn(__fmul_rn(0.5f, ph[d][PO]), __fmul_rn(0.5f, ph[d][PN]));
             const float det = __fsub_rn(__fmul_rn(pg[d][PM], gyy), __fmul_rn(gxy, gxy));
-            float r = fmaxf(__fsub_rn(__fmul_rn(fabsf(det), s4[d]), th), 0.0f);
+            float r = fmax_nan(__fsub_rn(__fmul_rn(fabsf(det), s4[d]), th), 0.0f);
             r = in ? r : 0.f;
             float l = __shfl_up_sync(0xffffffffu, r, 1), rr = __shfl_down_sync(0xffffffffu, r, 1);
             l = (lane == 0) ? 0.f : l;
             rr = (lane == 31) ? 0.f : rr;
             rs[d][PN] = r;
-            rmx[d][PN] = fmaxf(fmaxf(l, r), rr);
+            rmx[d][PN] = fmax_nan(fmax_nan(l, r), rr);
             hs[d][PN] = (l + r) + rr;
             hx[d][PN] = fmaf(1.5f, rr, fmaf(0.5f, r, -0.5f * l));   // x offsets [-0.5, 0.5, 1.5] (Q2)
         }
@@ -813,11 +839,11 @@ __global__ void __launch_bounds__(WNT, AG_DETROWS_MINB) detect_rows_kernel(const
             if (col_ok && y >= P.mr_border && y < h - P.mr_border) {
                 float M[5];
 #pragma unroll
-                for (int d = 0; d < 5; d++) M[d] = fmaxf(fmaxf(rmx[d][PO], rmx[d][PM]), rmx[d][PN]);
+                for (int d = 0; d < 5; d++) M[d] = fmax_nan(fmax_nan(rmx[d][PO], rmx[d][PM]), rmx[d][PN]);
                 const float x1 = rs[1][PM], x2 = rs[2][PM], x3 = rs[3][PM];
-                n1 = (__fadd_rn(__fsub_rn(x1, fmaxf(fmaxf(M[0], M[1]), M[2])), 1e-5f) > 0.f) ? x1 : 0.f;   // NMS3d, HandCraftedModules.py:220
-                n2 = (__fadd_rn(__fsub_rn(x2, fmaxf(fmaxf(M[1], M[2]), M[3])), 1e-5f) > 0.f) ? x2 : 0.f;
-                n3 = (__fadd_rn(__fsub_rn(x3, fmaxf(fmaxf(M[2], M[3]), M[4])), 1e-5f) > 0.f) ? x3 : 0.f;
+                n1 = (__fadd_rn(__fsub_rn(x1, fmax_nan(fmax_nan(M[0], M[1]), M[2])), 1e-5f) > 0.f) ? x1 : 0.f;   // NMS3d, HandCraftedModules.py:220
+                n2 = (__fadd_rn(__fsub_rn(x2, fmax_nan(fmax_nan(M[1], M[2]), M[3])), 1e-5f) > 0.f) ? x2 : 0.f;
+                n3 = (__fadd_rn(__fsub_rn(x3, fmax_nan(fmax_nan(M[2], M[3]), M[4])), 1e-5f) > 0.f) ? x3 : 0.f;
             }
             const unsigned m1 = __ballot_sync(0xffffffffu, n1 != 0.f), m2 = __ballot_sync(0xffffffffu, n2 != 0.f), m3 = __ballot_sync(0xffffffffu, n3 != 0.f);
             if (m1 | m2 | m3) {

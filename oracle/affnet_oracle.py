@@ -134,15 +134,17 @@ def hessian_response(x, sigma):
     """abs(gxx*gyy - gxy^2) * sigma^4 with replicate (clamped) borders; x float32 [1,1,h,w].
 
     gxx = x[j-1] - 2x[j] + x[j+1]; gyy likewise vertically; gxy = two chained (0.5,0,-0.5)
-    cross-correlations = 0.25*(x[i-1,j-1] - x[i-1,j+1] - x[i+1,j-1] + x[i+1,j+1]).
+    cross-correlations = 0.25*(x[i-1,j-1] - x[i-1,j+1] - x[i+1,j-1] + x[i+1,j+1]).  Their zero
+    taps are kept: 0 * x changes no finite value beyond the sign of a zero (squared away), but an
+    infinite pixel makes them NaN, as the reference's convolutions do.
     sigma^4 is a Python double applied as a scalar multiply (HandCraftedModules.py:78).
     """
     xp = F.pad(x, (1, 1, 1, 1), "replicate")
     c = xp[:, :, 1:-1, 1:-1]
     gxx = xp[:, :, 1:-1, :-2] - 2.0 * c + xp[:, :, 1:-1, 2:]
     gyy = xp[:, :, :-2, 1:-1] - 2.0 * c + xp[:, :, 2:, 1:-1]
-    gx = 0.5 * xp[:, :, :, :-2] - 0.5 * xp[:, :, :, 2:]          # [.., h+2, w]
-    gxy = 0.5 * gx[:, :, :-2, :] - 0.5 * gx[:, :, 2:, :]
+    gx = 0.5 * xp[:, :, :, :-2] - 0.5 * xp[:, :, :, 2:] + 0.0 * xp[:, :, :, 1:-1]     # [.., h+2, w]
+    gxy = 0.5 * gx[:, :, :-2, :] - 0.5 * gx[:, :, 2:, :] + 0.0 * gx[:, :, 1:-1, :]
     return torch.abs(gxx * gyy - gxy * gxy) * (sigma ** 4)
 
 
@@ -154,14 +156,21 @@ NMS_EPS = 1e-5  # HandCraftedModules.py:212
 
 
 def float_to_u8_cpu(v):
-    """float32 -> uint8 the way torch-CPU `.byte()` does it (truncate, wrap mod 256; Q4)."""
-    return (np.trunc(v.astype(np.float64)).astype(np.int64) & 0xFF).astype(np.uint8)
+    """float32 -> uint8 the way torch-CPU `.byte()` does it (truncate, wrap mod 256; Q4).  NaN gives 0, and so does every
+    |v| >= 2^31, whose fp32 values are multiples of 256."""
+    v = v.astype(np.float64)
+    v = np.where(np.abs(v) < 2.0 ** 31, v, 0.0)
+    return (np.trunc(v).astype(np.int64) & 0xFF).astype(np.uint8)
 
 
-def nms3d_mask(low, cur, high):
+def nms3d_mask(low, cur, high, mutate=None):
     """NMS3d on the middle slice (HandCraftedModules.py:208-220, :248): fp32 (x - m + eps) > 0,
-    m = max over the 3x3x3 neighbourhood, spatial padding -inf, depth unpadded."""
+    m = max over the 3x3x3 neighbourhood, spatial padding -inf, depth unpadded.  m is NaN when the
+    window holds a NaN (MaxPool3d), so a NaN suppresses its whole window.  Mutation (tests only):
+    "fmaxf" (a window maximum that ignores NaN)."""
     stack = torch.cat([low, cur, high], dim=1)                  # [1,3,h,w]
+    if mutate == "fmaxf":
+        stack = torch.nan_to_num(stack, nan=-float("inf"), posinf=float("inf"))
     m = F.max_pool2d(stack, 3, stride=1, padding=1).max(dim=1, keepdim=True)[0]
     return ((cur - m + NMS_EPS) > 0).float() * cur
 
@@ -179,14 +188,20 @@ def soft_argmax_weights(scales):
     return g
 
 
-def nms3d_and_compose(low, cur, high, num_features, octave_map, scales, mrSize):
+def nms3d_and_compose(low, cur, high, num_features, octave_map, scales, mrSize, mutate=None):
     """NMS3dAndComposeA.forward (HandCraftedModules.py:240-291).
 
     low/cur/high: float32 [1,1,h,w]; octave_map: uint8 numpy [h,w].  Returns
     (resp[n], LAFs[n,2,3] normalised, new_octave_map, flat_idxs[n]) or (None, None, octave_map, None).
+
+    One deviation (DESIGN.md §2): a NaN survivor of the NMS (`0 * x` at a NaN or infinite response)
+    is no keypoint.  The reference emits it (nonzero() keeps NaN, topk ranks it first) with a NaN LAF;
+    here it is removed before the level's top-k and keep-all.  Everything else counts it as the
+    reference does: not in (nmsed > 0), and 0 in the octave map ((om + NaN).byte() is 0 on the CPU).
+    Mutations (tests only): those of nms3d_mask, and "emit_nan" (the reference's NaN survivors kept).
     """
     h, w = cur.size(2), cur.size(3)
-    nmsed = nms3d_mask(low, cur, high).clone()
+    nmsed = nms3d_mask(low, cur, high, mutate).clone()
     b = int(mrSize)
     if b < w and b < h:                                          # Utils.py:140-148
         nmsed[:, :, :b, :] = 0; nmsed[:, :, h - b:, :] = 0
@@ -200,6 +215,8 @@ def nms3d_and_compose(low, cur, high, num_features, octave_map, scales, mrSize):
         return None, None, octave_map, None
     new_map = float_to_u8_cpu((om + nmsed).numpy().reshape(h, w))
     flat = nmsed.view(-1)
+    if mutate != "emit_nan":
+        flat = torch.where(torch.isnan(flat), torch.zeros_like(flat), flat)   # NaN survivors: no keypoints
     if 0 < num_features < n_pos:
         vals, idxs = torch.topk(flat, k=num_features)
     else:
@@ -229,17 +246,20 @@ def nms3d_and_compose(low, cur, high, num_features, octave_map, scales, mrSize):
 # ----------------------------------------------------------------------------------------------
 
 
-def multi_scale_detector(pyr, sigmas, num_features, mrSize, th=0.0, return_levels=False):
-    """Returns (resp[M], LAFs[M,2,3] normalised, pyr_idxs[M], level_idxs[M]) (+ per-level dump)."""
+def multi_scale_detector(pyr, sigmas, num_features, mrSize, th=0.0, return_levels=False, mutate=None):
+    """Returns (resp[M], LAFs[M,2,3] normalised, pyr_idxs[M], level_idxs[M]) (+ per-level dump).
+    Mutations (tests only): those of nms3d_and_compose, and "clamp_drops_nan" (NaN responses clamped to 0)."""
     resps, lafs, pidx, lidx, dump = [], [], [], [], []
     for o in range(len(pyr)):
         octave = pyr[o]
         h, w = octave[0].size(2), octave[0].size(3)
         omap = np.zeros((h, w), np.uint8)
         maps = [torch.clamp(hessian_response(octave[l], sigmas[o][l]) - th, min=0) for l in range(len(octave))]
+        if mutate == "clamp_drops_nan":
+            maps = [torch.nan_to_num(m, nan=0.0, posinf=float("inf")) for m in maps]
         for l in range(1, len(octave) - 1):
             r, A, omap, idxs = nms3d_and_compose(maps[l - 1], maps[l], maps[l + 1], num_features, omap,
-                                                 sigmas[o][l - 1:l + 2], mrSize)
+                                                 sigmas[o][l - 1:l + 2], mrSize, mutate)
             dump.append((o, l, None if r is None else idxs.clone(), None if r is None else r.clone()))
             if r is None:
                 continue

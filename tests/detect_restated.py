@@ -20,7 +20,10 @@ enough for that rounding to be the correctly rounded fp32 result, subnormal resu
 for large candidate sets, on the device; no library kernel is called.
 
 Next to them is the float64 soft-argmax of the same fp32 inputs with a per-candidate bound that holds for any summation order, so
-it covers both kernel orders, the oracle's F.conv2d and the reference's goldens alike."""
+it covers both kernel orders, the oracle's F.conv2d and the reference's goldens alike.  The bound holds where every sum stays
+finite in fp32 (`finite_sums`); where a sum overflows (images scaled far up), the fp32 functions are still exact IEEE arithmetic
+(infinities and NaN pass through the float64 operations and `fmaf32` as through the kernel's), so the kernel's rows must have the
+restatement's bits and NaN positions there (`same_bits`)."""
 import numpy as np
 import torch
 import torch.nn.functional as F
@@ -205,6 +208,22 @@ def softargmax64(maps3, sc, pix, a_scale=1.0):
     return lafs, bound
 
 
+def finite_sums(R):
+    """Rows of windows R [n, 3, 3, 3] whose ns, ny, nx and den stay finite in fp32 in any summation order: the sum of the absolute
+    terms (weights <= 1.5 and sc_d < 2^7), grown by every rounding on the way, is below FLT_MAX."""
+    a = _d(R).abs().sum((1, 2, 3)) * 128.0 * (1.0 + 2.0 ** -18)
+    return torch.isfinite(_d(R)).all(3).all(2).all(1) & (a < float(np.finfo(np.float32).max))
+
+
+def same_bits(a, b):
+    """fp32 tensors equal bit for bit where not NaN, and NaN at the same positions (NaN payloads differ between the CPU and the GPU)."""
+    a, b = a.to(torch.float32).cpu(), b.to(torch.float32).cpu()
+    if a.shape != b.shape:
+        return False
+    na, nb = torch.isnan(a), torch.isnan(b)
+    return torch.equal(na, nb) and torch.equal(bits(a)[~na], bits(b)[~nb])
+
+
 def bound_ratio(lafs, ref64, bound):
     """max |lafs - ref64| / bound over the bounded entries (lafs fp32 [n, 2, 3]); the off-diagonals must be exactly +0."""
     if lafs.numel() == 0:
@@ -230,6 +249,7 @@ class Restated:
         self.lafs32 = torch.zeros(seq.numel(), 2, 3, dtype=torch.float32)
         self.lafs64 = torch.zeros(seq.numel(), 2, 3, dtype=torch.float64)
         self.bound = torch.zeros(seq.numel(), 2, 3, dtype=torch.float64)
+        self.finite = torch.ones(seq.numel(), dtype=torch.bool)   # rows whose sums are finite in any order: the bound applies
         slot = seq >> SEQ_PIX_BITS
         pix = seq & ((1 << SEQ_PIX_BITS) - 1)
         for o in range(len(pyr)):
@@ -247,6 +267,7 @@ class Restated:
                     self.lafs32[sel] = softargmax32(m[k:k + 3], sc, p, order, a_scale, mutate).cpu()
                 L64, B64 = softargmax64(m[k:k + 3], sc, p, a_scale)
                 self.lafs64[sel], self.bound[sel] = L64.cpu(), B64.cpu()
+                self.finite[sel] = finite_sums(windows(m[k:k + 3], p)).cpu()
 
 
 def bits(x):
