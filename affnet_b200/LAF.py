@@ -1,5 +1,5 @@
 """LAF helpers with the reference's names (LAF.py): the affine sampler, (de)normalisation, level routing and the
-Oxford-ellipse output conversion."""
+Oxford-ellipse conversions in both directions."""
 import ctypes as C
 
 import numpy as np
@@ -95,6 +95,19 @@ def LAFs2ellT(LAFs):
     if n:
         L.check(L.lib().ag_lafs_to_ell(L.ptr(LAFs), n, L.ptr(ell), L.stream_ptr()))
     return ell
+
+
+def ells2LAFsT(ells):
+    """LAF.py:76-89 on the device (`ag_ells_to_lafs`): [n,5] Oxford-affine rows (x, y, a, b, c) -> [n,2,3] upright pixel LAFs, the
+    reference's fp32 arithmetic bit for bit (NaN for an ellipse that is not positive definite, as there)."""
+    if not ells.is_cuda:
+        raise L.AffnetB200Error("ells2LAFsT: CUDA tensor expected (there is no CPU path)")
+    ells = ells.contiguous().float().view(-1, 5)
+    n = ells.size(0)
+    lafs = torch.empty(n, 2, 3, device=ells.device)
+    if n:
+        L.check(L.lib().ag_ells_to_lafs(L.ptr(ells), n, L.ptr(lafs), L.stream_ptr()))
+    return lafs
 
 
 def save_ells(fname, ells):

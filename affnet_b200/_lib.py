@@ -115,6 +115,7 @@ PROTOTYPES = {
     "ag_lafs_apply_rotation": (i32, [vp, vp, i32, vp]),
     "ag_lafs_scale": (i32, [vp, vp, i32, f32, f32, f32, vp]),
     "ag_lafs_to_ell": (i32, [vp, i32, vp, vp]),
+    "ag_ells_to_lafs": (i32, [vp, i32, vp, vp]),
     "ag_circular_gauss_kernel": (i32, [i32, f64, vp]),
     "ag_orientation_hist": (i32, [vp, i32, i32, vp, vp, vp]),
     "ag_baumberg_shape": (i32, [vp, i32, i32, vp, vp, vp]),
@@ -136,6 +137,9 @@ PROTOTYPES = {
                                     C.POINTER(vp)]),
     "ag_pipeline_create_topk": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), C.POINTER(PipelineDescriptor), vp, vp, vp,
                                       C.POINTER(vp)]),
+    "ag_pipeline_create_given": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), C.POINTER(PipelineDescriptor), vp, vp, vp,
+                                       C.POINTER(vp)]),
+    "ag_pipeline_run_given": (i32, [vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]),
     "ag_pipeline_destroy": (None, [vp]),
     "ag_pipeline_workspace_bytes": (sz, [vp]),
     "ag_pipeline_plan": (C.POINTER(PyramidPlan), [vp]),

@@ -272,6 +272,42 @@ __global__ void lafs_to_ell_kernel(const float* __restrict__ lafs, float* __rest
     o[4] = sn * w0 * sn + c * w1 * c;          // [1][1]
 }
 
+// ells2LAFsT (LAF.py:76-89) with invSqrtTorch (:52-74): one thread per ellipse, each torch operation one rounded fp32 operation in the
+// expression's left-to-right order (tests/given_restated.py states the same).  torch.sign is (x > 0) - (x < 0): 0 for +-0 and NaN.
+__global__ void ells_to_lafs_kernel(const float* __restrict__ ell, float* __restrict__ lafs, int n) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float* E = ell + (size_t)i * 5;
+    const float a = E[2], b = E[3], c = E[4];
+    const float sc = __fsqrt_rn(__fsqrt_rn(__fadd_rn(__fsub_rn(__fmul_rn(a, c), __fmul_rn(b, b)), 1e-12f)));
+    // invSqrtTorch
+    const float mask = (b != 0.f) ? 1.f : 0.f;
+    const float r1 = __fdiv_rn(__fmul_rn(mask, __fsub_rn(c, a)), __fadd_rn(__fmul_rn(2.f, b), 1e-12f));
+    const float sg = (r1 > 0.f) ? 1.f : ((r1 < 0.f) ? -1.f : 0.f);
+    const float t1 = __fdiv_rn(sg, __fadd_rn(fabsf(r1), __fsqrt_rn(__fadd_rn(1.f, __fmul_rn(r1, r1)))));
+    float r = __fdiv_rn(1.f, __fsqrt_rn(__fadd_rn(1.f, __fmul_rn(t1, t1))));
+    float t = __fmul_rn(t1, r);
+    r = __fadd_rn(__fmul_rn(r, mask), __fmul_rn(1.f, __fsub_rn(1.f, mask)));
+    t = __fmul_rn(t, mask);
+    const float rr = __fmul_rn(r, r), tt = __fmul_rn(t, t), rt2 = __fmul_rn(__fmul_rn(2.f, r), t);
+    float x = __fdiv_rn(1.f, __fsqrt_rn(__fadd_rn(__fsub_rn(__fmul_rn(rr, a), __fmul_rn(rt2, b)), __fmul_rn(tt, c))));
+    float z = __fdiv_rn(1.f, __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(tt, a), __fmul_rn(rt2, b)), __fmul_rn(rr, c))));
+    const float d = __fsqrt_rn(__fmul_rn(x, z));
+    x = __fdiv_rn(x, d);
+    z = __fdiv_rn(z, d);
+    const float ia = __fadd_rn(__fmul_rn(rr, x), __fmul_rn(tt, z));
+    const float ib = __fadd_rn(__fmul_rn(__fmul_rn(-r, t), x), __fmul_rn(__fmul_rn(t, r), z));
+    const float ic = __fadd_rn(__fmul_rn(tt, x), __fmul_rn(rr, z));
+    // A = [[ia, ib], [ib, ic]] / sc; its scale; rectifyAffineTransformationUpIsUp(A / scale) * scale
+    const float a00 = __fdiv_rn(ia, sc), a01 = __fdiv_rn(ib, sc), a11 = __fdiv_rn(ic, sc);
+    const float s = __fsqrt_rn(fabsf(__fsub_rn(__fmul_rn(a00, a11), __fmul_rn(a01, a01))));
+    float R[4];
+    rectify_up_is_up(__fdiv_rn(a00, s), __fdiv_rn(a01, s), __fdiv_rn(a01, s), __fdiv_rn(a11, s), R);
+    float* L = lafs + (size_t)i * 6;
+    L[0] = __fmul_rn(R[0], s); L[1] = __fmul_rn(R[1], s); L[2] = E[0];
+    L[3] = __fmul_rn(R[2], s); L[4] = __fmul_rn(R[3], s); L[5] = E[1];
+}
+
 }  // namespace ag
 
 using namespace ag;
@@ -428,6 +464,14 @@ int ag_lafs_to_ell(const float* d_lafs, int n, float* d_ell, void* stream) {
     if (n <= 0) return AG_OK;
     lafs_to_ell_kernel<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(d_lafs, d_ell, n);
     AG_CHECK_LAUNCH("lafs_to_ell_kernel");
+    return AG_OK;
+}
+
+int ag_ells_to_lafs(const float* d_ell, int n, float* d_lafs, void* stream) {
+    AG_REQUIRE(d_ell && d_lafs, "NULL argument");
+    if (n <= 0) return AG_OK;
+    ells_to_lafs_kernel<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(d_ell, d_lafs, n);
+    AG_CHECK_LAUNCH("ells_to_lafs_kernel");
     return AG_OK;
 }
 

@@ -1,7 +1,8 @@
 """Batched detect-and-describe for B same-sized images (new API; the reference handles one image at a time):
 the whole ScaleSpaceAffinePatchExtractor.forward + extract_patches_from_pyr + HardNet (or SIFTNet) chain as one fixed kernel
 sequence with device-side counters, optionally replayed as a CUDA graph.  The estimators follow ScaleSpaceAffinePatchExtractor's
-constructor (SparseImgRepresenter.py:26-49): AffNet or Baumberg iterations or no shape step, OriNet or gradient-histogram orientation."""
+constructor (SparseImgRepresenter.py:26-49): AffNet or Baumberg iterations or no shape step, OriNet or gradient-histogram orientation.
+DescribeGivenPipeline runs the same estimators and descriptor on keypoints the caller supplies."""
 import ctypes as C
 
 import torch
@@ -167,3 +168,104 @@ class DetectDescribePipeline:
             self._static_in.copy_(imgs.view_as(self._static_in), non_blocking=True)
         self._graphs[slot].replay()
         return self._slots[slot]
+
+
+class DescribeGivenPipeline:
+    def __init__(self, B, H, W, AffNet, HardNet, OriNet=None, capacity=2000, border=5, nlevels=3, init_sigma=1.6, do_ori=True,
+                 num_Baum_iters=1, device="cuda"):
+        """Describe caller-supplied keypoints of B same-sized images (ag_pipeline_create_given): the reference's getAffineShape
+        (keep-all: every survivor, in input order), getOrientation and extract_patches_from_pyr + descriptor on arbitrary pixel LAFs, as
+        its SIFT-AffNet-HardNet notebook composes them.  Nothing is detected or sorted, so there is no mrSize, th or top-K.
+        capacity: the rows C per image of the inputs and outputs ([B,C,2,3] LAFs), at most 2^24.  AffNet / OriNet / do_ori /
+        num_Baum_iters / HardNet select the estimators and the descriptor exactly as in DetectDescribePipeline."""
+        self.cfg = L.PipelineConfig(B, H, W, capacity, nlevels, border, float(init_sigma), 0.0, 1 if do_ori else 0, 0)
+        self.est, aff, ori = estimators(AffNet, OriNet, do_ori, num_Baum_iters)
+        self.desc_cfg, hard = descriptor(HardNet)
+        self.nets = (AffNet, OriNet, HardNet)  # keep the modules alive; the C pipeline only BORROWS their ag_net_t handles
+        self._used = (aff, ori, hard)
+        self._h = None
+        self._net_handles = None
+        self._bind_nets()
+        self.B, self.H, self.W, self.C = B, H, W, capacity
+        self.device = torch.device(device)
+        self.ws_bytes = L.lib().ag_pipeline_workspace_bytes(self._h)
+        self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=self.device)
+        self.lafs = torch.empty(B, capacity, 2, 3, dtype=torch.float32, device=self.device)
+        self.src = torch.empty(B, capacity, dtype=torch.int32, device=self.device)
+        self.desc = torch.empty(B, capacity, 128, dtype=torch.float32, device=self.device)
+        self.count = torch.zeros(B, dtype=torch.int32, device=self.device)
+        self._graph = None
+        self._static_in = None
+
+    def _bind_nets(self):
+        """(Re)create the C pipeline over the nets' current handles (see DetectDescribePipeline._bind_nets)."""
+        hs = tuple(n.handle() if n is not None else None for n in self._used)
+        if self._h is not None:
+            L.lib().ag_pipeline_destroy(self._h)
+            self._h = None
+        h = C.c_void_p()
+        L.check(L.lib().ag_pipeline_create_given(C.byref(self.cfg), C.byref(self.est), C.byref(self.desc_cfg), hs[0], hs[1], hs[2], C.byref(h)))
+        self._h, self._net_handles, self._graph = h, hs, None
+
+    def _nets_current(self):
+        return all(n is None or n._handle is h for n, h in zip(self._used, self._net_handles))
+
+    def __del__(self):
+        try:
+            L.lib().ag_pipeline_destroy(self._h)
+        except Exception:
+            pass
+
+    @property
+    def launches(self):
+        return L.lib().ag_pipeline_launch_count(self._h)
+
+    def _inputs(self, imgs, lafs, counts):
+        imgs, lafs = L.f32c(imgs, "imgs"), L.f32c(lafs, "lafs")
+        counts = L.require_cuda(counts, "counts")
+        if imgs.numel() != self.B * self.H * self.W:
+            raise L.AffnetB200Error("expected %d x %d x %d pixels" % (self.B, self.H, self.W))
+        if lafs.numel() != self.B * self.C * 6:
+            raise L.AffnetB200Error("lafs: expected [%d,%d,2,3] pixel LAFs" % (self.B, self.C))
+        if counts.numel() != self.B:
+            raise L.AffnetB200Error("counts: expected %d per-image counts" % self.B)
+        return imgs, lafs, counts.to(torch.int32).contiguous()
+
+    def run(self, imgs, lafs, counts):
+        """imgs CUDA float32 [B,1,H,W] or [B,H,W], lafs [B,C,2,3] pixel LAFs, counts [B] (rows of each image to describe) ->
+        (lafs [B,C,2,3] px, src [B,C] int32 input row of each output row, desc [B,C,128], count [B]).  An image whose count lies outside
+        0..C gets count -1 and nothing else written; rows >= count[b] are not written.  No host synchronisation."""
+        imgs, lafs, counts = self._inputs(imgs, lafs, counts)
+        if not self._nets_current() or any(n is not None and n.handle() is not h for n, h in zip(self._used, self._net_handles)):
+            self._bind_nets()      # a net was reloaded / moved since the pipeline was built
+        L.check(L.lib().ag_pipeline_run_given(self._h, L.ptr(imgs), L.ptr(lafs), L.ptr(counts), L.ptr(self.ws), self.ws_bytes, L.ptr(self.lafs),
+                                              L.ptr(self.src), L.ptr(self.desc), L.ptr(self.count), L.stream_ptr()))
+        return self.lafs, self.src, self.desc, self.count
+
+    def capture(self):
+        """Capture one run() into a CUDA graph over static input buffers; use replay(imgs, lafs, counts) afterwards."""
+        self._static_in = (torch.zeros(self.B, 1, self.H, self.W, dtype=torch.float32, device=self.device),
+                           torch.zeros(self.B, self.C, 2, 3, dtype=torch.float32, device=self.device),
+                           torch.zeros(self.B, dtype=torch.int32, device=self.device))
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            self.run(*self._static_in)  # warm-up: sets kernel attributes outside capture
+        torch.cuda.current_stream().wait_stream(s)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self.run(*self._static_in)
+        self._graph = g
+        return self
+
+    def replay(self, imgs=None, lafs=None, counts=None):
+        """Copy the given inputs into the static buffers (None: keep what they hold) and replay the captured run."""
+        if self._graph is None:
+            raise L.AffnetB200Error("call capture() first")
+        if not self._nets_current():
+            raise L.AffnetB200Error("a net of this pipeline was reloaded after capture(): the graph holds the old weights - call capture() again")
+        for dst, src in zip(self._static_in, (imgs, lafs, counts)):
+            if src is not None:
+                dst.copy_(src.reshape(dst.shape), non_blocking=True)
+        self._graph.replay()
+        return self.lafs, self.src, self.desc, self.count

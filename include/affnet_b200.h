@@ -306,6 +306,11 @@ int ag_lafs_left_multiply(const float* d_A, const float* d_lafs, float* d_out, i
  * d_lafs [n,2,3] in pixels -> d_ell [n,5] = (x, y, a, b, c) with a u^2 + 2 b u v + c v^2 = 1.  A LAF with a negative
  * determinant gives NaN, as in the reference. */
 int ag_lafs_to_ell(const float* d_lafs, int n, float* d_ell, void* stream);
+/* The reference's reader of that format: replaces ells2LAFsT (LAF.py:76-89, invSqrtTorch :52-74, rectifyAffineTransformationUpIsUp
+ * :285-291).  d_ell [n,5] = (x, y, a, b, c) -> d_lafs [n,2,3] in pixels, upright (A[0][1] = 0).  Each torch operation of the reference is
+ * one fp32 operation in its order (IEEE division and square root, no fused multiply-add), so the rows equal the reference's fp32 CPU
+ * result bit for bit, including the b == 0 branch and the NaN of an ellipse that is not positive definite.  One launch. */
+int ag_ells_to_lafs(const float* d_ell, int n, float* d_lafs, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Hand-crafted estimators (SURVEY.md §8f "next" rows): what the reference uses when OriNet / AffNet are None.
@@ -492,8 +497,33 @@ const ag_pyramid_plan_t* ag_pipeline_plan(const ag_pipeline_t* p);
  * Enqueues kernels only (CUDA-graph capturable). */
 int ag_pipeline_run(ag_pipeline_t* p, const float* d_img, void* d_ws, size_t ws_bytes, float* d_lafs, float* d_resp,
                     float* d_desc, int* d_count, void* stream);
-/* Number of kernel launches one ag_pipeline_run enqueues (for bench.py's gpu_launches). */
+/* Number of kernel launches the last ag_pipeline_run / ag_pipeline_run_given enqueued (for bench.py's gpu_launches). */
 int ag_pipeline_launch_count(const ag_pipeline_t* p);
+
+/* Given keypoints (new; the reference composes these steps by hand, e.g. its SIFT-AffNet-HardNet notebook): describe caller-supplied
+ * pixel LAFs with the pipeline's estimators and descriptor, nothing detected and nothing sorted.  cfg->num_features is the per-image
+ * capacity C of the input and output rows (1 .. 2^24, no 16384 limit); cfg->cand_cap and cfg->mrSize are ignored; est and desc as
+ * ag_pipeline_create_desc, with its refusals (AG_ERR_INVALID before any CUDA call).  Per image b, rows i < d_count_in[b]:
+ *   1. the ScalePyramid of image b (the plan of ag_pipeline_create);
+ *   2. (oct, lvl) = get_pyramid_and_level_index_for_LAFs(dLAF, PS = 32) (LAF.py:453-472), the level every estimator samples, as
+ *      getAffineShape and getOrientation reuse one level (SparseImgRepresenter.py:113-180);
+ *   3. normalizeLAFs with the coefficients of ag_pipeline_run;
+ *   4. with a shape estimator, num_baum_iters iterations of it, then getAffineShape's keep-all branch (num_features <= 0, :151-156): every
+ *      survivor of the eigenvalue-ratio and boundary tests in input order; d_src[b,j] is the input row of output row j.  Without one
+ *      every row survives and d_src[b,j] = j;
+ *   5. the orientation estimator, if any (getOrientation), at the same (oct, lvl);
+ *   6. denormalizeLAFs into d_lafs, then extract_patches_from_pyr(·, desc->ps) and the descriptor into d_desc.  With neither a shape nor
+ *      an orientation step the LAFs are not touched: d_lafs[b,j] equals the input row bit for bit (no normalise / denormalise round trip).
+ * d_img [B,H,W]; d_lafs_in [B,C,2,3] pixel LAFs; d_count_in [B].  Outputs d_lafs [B,C,2,3], d_src [B,C] int32, d_desc [B,C,128],
+ * d_count [B] = the survivors.  A count_in[b] outside 0..C gives d_count[b] = -1 and nothing else of image b is written (the pipeline's
+ * overflow count travels through the matcher this way); rows at or beyond d_count[b] of every output are never written.  Launches are
+ * fixed on the host and counts read on the device: no host synchronisation, CUDA-graph capturable.  The workspace holds the pyramid, the
+ * per-row buffers of C rows and the net scratch, no detector or selection regions.  ag_pipeline_run refuses a given-keypoints pipeline
+ * and ag_pipeline_run_given every other kind, with AG_ERR_INVALID before any CUDA call. */
+int ag_pipeline_create_given(const ag_pipeline_config_t* cfg, const ag_pipeline_estimators_t* est, const ag_pipeline_descriptor_t* desc,
+                             const ag_net_t* affnet, const ag_net_t* orinet, const ag_net_t* hardnet, ag_pipeline_t** out);
+int ag_pipeline_run_given(ag_pipeline_t* p, const float* d_img, const float* d_lafs_in, const int* d_count_in, void* d_ws, size_t ws_bytes,
+                          float* d_lafs, int* d_src, float* d_desc, int* d_count, void* stream);
 
 #ifdef __cplusplus
 }
