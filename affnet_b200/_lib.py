@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("AFFNET_B200_LIB", os.path.join(HERE, "lib", "libaffnet_b200.so"))   # override: developer builds only
 AG_MAX_OCTAVES, AG_MAX_LEVELS = 16, 8
 NET_AFFNET, NET_ORINET, NET_HARDNET = 0, 1, 2
-ENGINE_SIMT, ENGINE_TC, ENGINE_TC_EXACT, ENGINE_TC_FAST, ENGINE_TC2, ENGINE_TC2_BF16 = 0, 1, 2, 3, 4, 5
+ENGINE_SIMT, ENGINE_TC2, ENGINE_TC2_BF16 = 0, 4, 5
 
 
 class AffnetB200Error(RuntimeError):

@@ -1,7 +1,7 @@
 // Second-generation tensor-core engine of AffNet / OriNet / HardNet (tcx_first.cuh, tcx_conv.cuh): row tiles without x padding, the
 // three taps of a kernel row stacked along N, x shifts by warp shuffles in the epilogue.  Replaces the conv stacks of
-// architectures.py:207-235 / 36-82 and HardNet.py:67-101 (BatchNorm folded, ReLU fused); the 8x8 heads stay the GEMM kernels of
-// tc_head.cuh (same head-operand layout).  Per net:  AffNet / OriNet  tcx_first_kernel (sampler + input_norm + conv1 + conv2 + conv3)
+// architectures.py:207-235 / 36-82 and HardNet.py:67-101 (BatchNorm folded, ReLU fused); the 8x8 heads are the GEMM kernels of
+// tc_head.cuh over the trunk's last output.  Per net:  AffNet / OriNet  tcx_first_kernel (sampler + input_norm + conv1 + conv2 + conv3)
 // ->  tcx_conv_kernel x3;  HardNet  tcx_first_kernel (sampler + input_norm + conv1 + conv2)  ->  tcx_conv_kernel x4.
 // Numerics: AffNet / OriNet with fp16 residual planes of weights and activations in every layer (three MMAs per K step, fp32-grade);
 // HardNet fp16 activations, weights with their fp16 residual in layers 2 and 3 (emulation on the 2000 graf patches: plain fp16 weights give a
@@ -15,6 +15,7 @@
 #include <cuda_bf16.h>
 
 #include "net_impl.cuh"
+#include "tc_head.cuh"
 #include "tcx_conv.cuh"
 #include "tcx_first.cuh"
 
@@ -32,22 +33,12 @@ static int num_sms() {
     return n;
 }
 
-static int ensure_smem_attr(const void* func, int bytes, bool* configured, const char* what) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    dev &= 63;
-    if (configured[dev]) return AG_OK;
-    int rc = check_cuda(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes), what);
-    if (rc == AG_OK) configured[dev] = true;
-    return rc;
-}
-
 template <int CIN, int COUT, int H, int STRIDE, int NSPLIT, int STAGES, int OUT, int SA, int SW, int OSA, int BF = 0, int MC = 0, int PPS = 0>
 static int launch_conv(const void* in, void* out, const __half* w, const float* b, float inv_scale, int n, int group, const int* count, cudaStream_t st) {
     using Cfg = XCfg<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA>;
     auto kern = tcx_conv_kernel<CIN, COUT, H, STRIDE, NSPLIT, STAGES, OUT, SA, SW, OSA, BF, MC, PPS>;
-    static bool configured[64] = {};   // per device (the attribute is per device)
-    int rc = ensure_smem_attr((const void*)kern, (int)Cfg::SMEM, configured, "tcx_conv smem attr");
+    static SmemAttrOnce attr_once;
+    int rc = attr_once.ensure(kern, Cfg::SMEM, "tcx_conv smem attr");
     if (rc != AG_OK) return rc;
     XArgs a;
     a.in = (const __half*)in; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.n = n; a.group = group; a.count = count;
@@ -77,8 +68,8 @@ static int launch_first(void* out, const __half* w, const float* b, float inv_sc
                         void* out3 = nullptr, const __half* w3 = nullptr, const float* b3 = nullptr, float inv_scale3 = 0.f) {
     using Cfg = XFirstCfg<C1, COUT, SA, SW, OSA, L3>;
     auto kern = tcx_first_kernel<C1, COUT, SA, SW, OSA, BF, L3>;
-    static bool configured[64] = {};
-    int rc = ensure_smem_attr((const void*)kern, (int)Cfg::SMEM, configured, "tcx_first smem attr");
+    static SmemAttrOnce attr_once;
+    int rc = attr_once.ensure(kern, Cfg::SMEM, "tcx_first smem attr");
     if (rc != AG_OK) return rc;
     XArgs a;
     a.in = nullptr; a.out = out; a.wpk = w; a.bias = b; a.inv_scale = inv_scale; a.n = n; a.group = group; a.count = count;
@@ -119,6 +110,26 @@ __global__ void tcx_decode_kernel(const __half* __restrict__ buf, int layout, in
 }
 
 }  // namespace tcx
+
+tc::FirstSrc tc_src_patches(const float* patches) {
+    tc::FirstSrc s;
+    memset(&s, 0, sizeof(s));
+    s.patches = patches;
+    s.cap = 1;
+    return s;
+}
+
+tc::FirstSrc tc_src_pyramid(const ag_pyramid_plan_t* p, const float* pyr, const float* lafs, const int* oct, const int* lvl, int cap) {
+    tc::FirstSrc s;
+    memset(&s, 0, sizeof(s));
+    s.pyr = pyr; s.lafs = lafs; s.oct = oct; s.lvl = lvl; s.cap = cap;
+    s.geom.n_octaves = p->n_octaves; s.geom.n_levels = p->n_levels;
+    for (int o = 0; o < AG_MAX_OCTAVES; o++) {
+        s.geom.h[o] = p->h[o]; s.geom.w[o] = p->w[o];
+        for (int l = 0; l < AG_MAX_LEVELS; l++) s.geom.off[o][l] = p->level_offset[o][l];
+    }
+    return s;
+}
 
 // ---- weight packing (host) --------------------------------------------------------------------------------------------------------
 // wf: fp32 [tap = dy*3+dx][ci][co] (BatchNorm folded), scale: power of two.  Blocks per (split, dy, 16 input channels):
@@ -240,6 +251,41 @@ int tcx_trunk_hardnet(const ag_net* net, const tc::FirstSrc& src0, int n, int gr
     return bf16 ? trunk_hardnet_t<1>(net, src0, n, group, count, bufA, bufB, headbuf, st, upto)
                 : trunk_hardnet_t<0>(net, src0, n, group, count, bufA, bufB, headbuf, st, upto);
 }
+
+// ---- heads ---------------------------------------------------------------------------------------------------------------------------
+// HardNet 8x8 head GEMM + BatchNorm + L2 norm over the head operand a trunk left in `headbuf`
+int tc_hardnet_head(const ag_net* net, const void* headbuf, int n, int group, const int* count, float* out, cudaStream_t st, int bf16) {
+    using namespace tc;
+    static SmemAttrOnce once0, once1;
+    {
+        int rc = once0.ensure(tc_head_kernel<0>, HEAD_SMEM, "tc_head smem attr");
+        if (rc == AG_OK) rc = once1.ensure(tc_head_kernel<1>, HEAD_SMEM, "tc_head smem attr");
+        if (rc != AG_OK) return rc;
+    }
+    if (bf16) tc_head_kernel<1><<<(n + 127) / 128, 288, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh_bf, net->d_head_b, out, n, group, count);
+    else tc_head_kernel<0><<<(n + 127) / 128, 288, HEAD_SMEM, st>>>((const __half*)headbuf, net->d_headh, net->d_head_bx, out, n, group, count);
+    AG_CHECK_LAUNCH("tc_head_kernel");
+    return AG_OK;
+}
+
+// AffNet / OriNet head on tensor cores over the hi/lo feature planes tcx_trunk_affori leaves in `feat`
+int tc_headx_forward(const ag_net* net, const void* feat, int n, int group, const int* count, float* out, float* angle, cudaStream_t st, float* raw) {
+    using namespace tc;
+    static SmemAttrOnce once0, once1;
+    {
+        int rc = once0.ensure(tc_headx_kernel<0>, HX_SMEM, "tc_headx smem attr");
+        if (rc == AG_OK) rc = once1.ensure(tc_headx_kernel<1>, HX_SMEM, "tc_headx smem attr");
+        if (rc != AG_OK) return rc;
+    }
+    const int tiles = (n + 127) / 128;
+    if (net->kind == AG_NET_AFFNET) tc_headx_kernel<0><<<tiles, 288, HX_SMEM, st>>>((const __half*)feat, net->d_headh, net->d_head_b, net->head_inv_scale, out, nullptr, raw, n, group, count);
+    else tc_headx_kernel<1><<<tiles, 288, HX_SMEM, st>>>((const __half*)feat, net->d_headh, net->d_head_b, net->head_inv_scale, out, angle, raw, n, group, count);
+    AG_CHECK_LAUNCH("tc_headx_kernel");
+    return AG_OK;
+}
+
+// bytes of the head-GEMM operand of n patches (hi + lo planes, padded to whole 128-patch tiles)
+size_t tc_headx_bytes(int n) { return (size_t)((n + 127) / 128) * 2 * tc::HX_PLANE_TILE; }
 
 }  // namespace ag
 

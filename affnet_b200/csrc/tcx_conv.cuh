@@ -14,7 +14,7 @@
 //   row; the neighbour outside the row is the zero padding).
 // Stride-2 layers read four parity planes; the taps dx = 0 and dx = 2 share the odd-x plane (N = 2 C), dx = 1 reads the even-x
 // plane (N = C):   out[x] = Dodd[x-1, dx0] + Dodd[x, dx2] + Deven[x, dx1].
-// Split precision as before: x = hi + lo fp16 planes (SA), w = hi + lo fp16 copies (SW), D = A_hi W_hi + A_hi W_lo + A_lo W_hi, each
+// Split precision: x = hi + lo fp16 planes (SA), w = hi + lo fp16 copies (SW), D = A_hi W_hi + A_hi W_lo + A_lo W_hi, each
 // product its own MMA into the SAME accumulator registers.
 //
 // Activations between layers (HBM): fp16, 16-byte slots of 8 channels, [unit][channel group (hi groups, then lo groups)][plane][slot],
@@ -48,7 +48,7 @@
 #pragma once
 #include <cuda_bf16.h>
 
-#include "tc_conv.cuh"
+#include "tc_common.cuh"
 
 #ifndef AG_CONV_PINGPONG
 #define AG_CONV_PINGPONG 1

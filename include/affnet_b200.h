@@ -194,16 +194,14 @@ typedef struct ag_net ag_net_t;
 int ag_net_create(int kind, const float* h_blob, size_t n_floats, ag_net_t** out);
 void ag_net_destroy(ag_net_t* net);
 size_t ag_net_blob_floats(int kind);
-/* Compute engine: 0 = exact fp32 SIMT (needs materialised patches); 1 = first-generation tensor-core engine (one MMA per tap): fp16
- * operands, fp32 accumulation, all six conv layers and the 8x8 heads as MMAs; AffNet and OriNet carry fp16 residual
- * planes of weights AND activations in every layer (fp32-grade: A 1e-5, angle 3e-5 rad - OriNet's atan2 amplifies an error of
- * AffNet's A about 15x, so the 1e-3 LAF contract needs A to 5e-5), HardNet plain fp16 operands (descriptors 6e-4);
- * 2 = as 1 with fp32 FMA-chain heads (A 2e-6, angle 3e-6 rad; AffNet/OriNet only); 3 = AffNet with the weight residual only
- * (A 2e-4; for A/B timing, AffNet only);
- * 4 = second-generation tensor-core engine, THE DEFAULT for all three nets (same operand precision as 1, plus fp16 residuals of HardNet's
- * layer 2-3 weights: descriptors 4e-4): 64-pixel
- * row tiles without x padding, the three taps of a kernel row stacked along N of one MMA, x shifts by warp shuffles in the epilogue;
- * 5 = engine 4 with bf16 operands (HardNet only; BASELINE.json configs[4] "bf16 HardNet tensor-core path"; descriptors ~4e-3). */
+/* Compute engine: 0 = exact fp32 SIMT (needs materialised patches);
+ * 4 = tensor-core engine, THE DEFAULT for all three nets: fp16 operands, fp32 accumulation, all six conv layers and the 8x8 heads as
+ * MMAs; AffNet and OriNet carry fp16 residual planes of weights AND activations in every layer (fp32-grade - OriNet's atan2 amplifies
+ * an error of AffNet's A about 15x, so the 1e-3 LAF contract needs A to 5e-5), HardNet fp16 operands with fp16 residuals of its
+ * layer 2-3 weights (descriptors 4e-4); 64-pixel row tiles without x padding, the three taps of a kernel row stacked along N of one
+ * MMA, x shifts by warp shuffles in the epilogue;
+ * 5 = engine 4 with bf16 operands (HardNet only; BASELINE.json configs[4] "bf16 HardNet tensor-core path"; descriptors ~4e-3).
+ * Any other value is refused with AG_ERR_INVALID and leaves the engine as it was. */
 int ag_net_set_engine(ag_net_t* net, int engine);
 int ag_net_get_engine(const ag_net_t* net);
 /* Developer switch: 1 = ag_pyramid_build runs one launch per octave (pyramid_fused.cuh: bit-identical, measured slower), 0 = one
@@ -249,7 +247,7 @@ int ag_hardnet_forward(const ag_net_t* net, const float* d_patches, int n, const
 /* f4: the TorchScript exports' contract (convertJIT/AffNetJIT.pt, OriNetJIT.pt; convert_OriNet_and_AffNet_to_JIT.ipynb): the RAW head
  * outputs.  AffNet: xy + [1, 0, 1] = (1 + x0, x1, 1 + x2) -> d_raw [n,3] (architectures.py:228-230 before rectification);
  * OriNet: the mean over the 3x3 map of tanh(conv8x8) -> d_raw [n,2] = (sin-like, cos-like) (architectures.py:57-59,76).
- * Tensor-core engines only (1, 3, 4). */
+ * Tensor-core engine (4) only. */
 int ag_affnet_forward_raw(const ag_net_t* net, const float* d_patches, int n, float* d_raw, void* d_ws, size_t ws_bytes, void* stream);
 int ag_orinet_forward_raw(const ag_net_t* net, const float* d_patches, int n, float* d_raw, void* d_ws, size_t ws_bytes, void* stream);
 /* Fused sampler + net (tensor-core engine): LAF i of image b is sampled at pyr[oct][lvl] INSIDE the first tensor-core

@@ -135,22 +135,19 @@ def test_layers_and_heads(L, kind, fmt, ckpt):
     print("\n%s raw head: max err/bound %.3f (max err %.2e)" % (tag, (err / Braw).max().item(), err.max().item()))
     assert (err <= Braw).all(), tag
     rawf = raw.float().cpu().numpy()
-    engines = (L.ENGINE_TC2, L.ENGINE_TC) + ((L.ENGINE_TC_FAST,) if kind == "affnet" else ())
-    for eng in engines:          # every engine with the GEMM head: its outputs are a function of its own raw outputs
-        net.set_engine(eng)
-        rawf = net.forward_raw(Pd).cpu().numpy()
-        if kind == "affnet":
-            A = net(Pd).cpu().numpy().reshape(n, 4)
-            ref = R.rectify_up_is_up(rawf[:, 0], np.zeros(n, np.float32), rawf[:, 1], rawf[:, 2])
-            assert same(A, ref), (tag, eng)
-        else:
-            F32 = np.float32
-            ang_ref = probe(L, rawf[:, 0] + F32(1e-8), rawf[:, 1] + F32(1e-8))[0]
-            _, c, s = probe(L, np.zeros(n, F32), ang_ref)
-            ang = net(Pd, return_rot_matrix=False).cpu().numpy()
-            Rm = net(Pd).cpu().numpy().reshape(n, 4)
-            assert same(ang, ang_ref), (tag, eng)
-            assert same(Rm, np.stack([c, s, -s, c], 1)), (tag, eng)
+    # the outputs of the GEMM head are a function of its own raw outputs
+    if kind == "affnet":
+        A = net(Pd).cpu().numpy().reshape(n, 4)
+        ref = R.rectify_up_is_up(rawf[:, 0], np.zeros(n, np.float32), rawf[:, 1], rawf[:, 2])
+        assert same(A, ref), tag
+    else:
+        F32 = np.float32
+        ang_ref = probe(L, rawf[:, 0] + F32(1e-8), rawf[:, 1] + F32(1e-8))[0]
+        _, c, s = probe(L, np.zeros(n, F32), ang_ref)
+        ang = net(Pd, return_rot_matrix=False).cpu().numpy()
+        Rm = net(Pd).cpu().numpy().reshape(n, 4)
+        assert same(ang, ang_ref), tag
+        assert same(Rm, np.stack([c, s, -s, c], 1)), tag
 
 
 @pytest.mark.parametrize("ckpt", CKPTS)

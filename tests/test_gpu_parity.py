@@ -244,13 +244,12 @@ def test_level_selection_identical(L):
     assert torch.equal(o.cpu().float(), oo) and torch.equal(l.cpu().float(), lo)
 
 
-@pytest.mark.parametrize("engine", ["simt", "tc"])
+@pytest.mark.parametrize("engine", ["simt"])
 def test_nets_vs_oracle(L, nets, engine):
-    """a9/a12/a16.  simt = exact fp32 engine: differences to the oracle reported, every stage held to its float64 bound; tc = first-generation
-    tensor-core engine (the default second-generation engine has the same checks in tests/test_gpu_tcx.py): north_star's 1e-3 for
-    descriptors, fp32-grade A matrices and angles."""
+    """a9/a12/a16.  simt = exact fp32 engine: differences to the oracle reported, every stage held to its float64 bound.  The default
+    tensor-core engine has its oracle checks on the same patch sets in tests/test_gpu_tcx.py::test_tcx_nets_vs_oracle."""
     aff, ori, hn = nets
-    e = L.ENGINE_SIMT if engine == "simt" else L.ENGINE_TC
+    e = L.ENGINE_SIMT
     z = gold("graf_crop.npz")
     g = torch.Generator().manual_seed(8)
     sets = [torch.from_numpy(z["aff_patches"]), torch.from_numpy(z["ori_desc_patches"]), torch.rand(37, 1, 32, 32, generator=g) * 255,
@@ -269,31 +268,15 @@ def test_nets_vs_oracle(L, nets, engine):
             dD = (hn(Pd).cpu() - O.hardnet_forward(P, W["hardnet"])).abs().max().item()
             worst = [max(a, b) for a, b in zip(worst, (dA, dR, dang, dD))]
         print("\nengine %s: max|dA| %.2e  max|dR| %.2e  max|dangle| %.2e rad  max|ddesc| %.2e" % ((engine,) + tuple(worst)))
-        if engine == "simt":   # every stage within its float64 bound, from the engine's own previous stage (tests/nets_simt_restated.py)
-            from test_gpu_simt_exact import layer_out, outputs
-            for P in sets:
-                for kind, m in zip(("affnet", "orinet", "hardnet"), (aff, ori, hn)):
-                    S.check_bounds("simt %s, %d patches" % (kind, P.size(0)), kind, W[kind], P, [layer_out(L, m, P, l) for l in range(1, 7)],
-                                   outputs(L, m, kind, P))
-        else:
-            # tensor cores: HardNet fp16 operands (1e-3); AffNet / OriNet weight and activation residuals (fp32-grade: the LAF
-            # contract needs A to 5e-5 because OriNet's atan2 amplifies an error of A about 15x)
-            assert worst[3] < 1e-3 and worst[0] < 5e-5 and worst[1] < 1e-4 and worst[2] < 1e-4, worst
+        # every stage within its float64 bound, from the engine's own previous stage (tests/nets_simt_restated.py)
+        from test_gpu_simt_exact import layer_out, outputs
+        for P in sets:
+            for kind, m in zip(("affnet", "orinet", "hardnet"), (aff, ori, hn)):
+                S.check_bounds("simt %s, %d patches" % (kind, P.size(0)), kind, W[kind], P, [layer_out(L, m, P, l) for l in range(1, 7)],
+                               outputs(L, m, kind, P))
     finally:
         aff.set_engine(L.ENGINE_TC2); ori.set_engine(L.ENGINE_TC2); hn.set_engine(L.ENGINE_TC2)
     assert aff(torch.empty(0, 1, 32, 32, device=DEV)).shape == (0, 2, 2)
-    if engine == "tc":   # exact tensor-core engine for AffNet: fp32-grade A
-        try:
-            aff.set_engine(L.ENGINE_TC_EXACT)
-            P = sets[0]
-            dA = (aff(P.to(DEV)).cpu() - O.affnet_forward(P, W["affnet"])).abs().max().item()
-            ori.set_engine(L.ENGINE_TC_EXACT)
-            dang = ori(P.to(DEV), return_rot_matrix=False).cpu() - O.orinet_angle(P, W["orinet"])
-            dang = torch.atan2(torch.sin(dang), torch.cos(dang)).abs().max().item()
-            print("engine tc-exact: max|dA| %.2e  max|dangle| %.2e rad" % (dA, dang))
-            assert dA < 2e-5 and dang < 1e-4
-        finally:
-            aff.set_engine(L.ENGINE_TC2); ori.set_engine(L.ENGINE_TC2)
 
 
 def test_nets_batching_invariance(L, nets):

@@ -88,16 +88,17 @@ def test_tcx_nets_vs_oracle(L, nets):
     sets = [torch.from_numpy(z["aff_patches"]), torch.from_numpy(z["ori_desc_patches"]), torch.rand(37, 1, 32, 32, generator=g) * 255,
             torch.from_numpy(gold("face_patches.npz")["patches_u8"].astype(np.float32) / 255.0).view(-1, 1, 32, 32),
             torch.rand(300, 1, 32, 32, generator=g)]
-    worst = [0.0, 0.0, 0.0]
+    worst = [0.0, 0.0, 0.0, 0.0]
     for P in sets:
         Pd = P.to(DEV)
         dA = (aff(Pd).cpu() - O.affnet_forward(P, W["affnet"])).abs().max().item()
+        dR = (ori(Pd).cpu() - O.orinet_forward(P, W["orinet"])).abs().max().item()
         dang = (ori(Pd, return_rot_matrix=False).cpu() - O.orinet_angle(P, W["orinet"]))
         dang = torch.atan2(torch.sin(dang), torch.cos(dang)).abs().max().item()
         dD = (hn(Pd).cpu() - O.hardnet_forward(P, W["hardnet"])).abs().max().item()
-        worst = [max(a, b) for a, b in zip(worst, (dA, dang, dD))]
-    print("\nengine tc2: max|dA| %.2e  max|dangle| %.2e rad  max|ddesc| %.2e" % tuple(worst))
-    assert worst[0] < 5e-5 and worst[1] < 1e-4 and worst[2] < 6e-4, worst
+        worst = [max(a, b) for a, b in zip(worst, (dA, dR, dang, dD))]
+    print("\nengine tc2: max|dA| %.2e  max|dR| %.2e  max|dangle| %.2e rad  max|ddesc| %.2e" % tuple(worst))
+    assert worst[0] < 5e-5 and worst[1] < 1e-4 and worst[2] < 1e-4 and worst[3] < 6e-4, worst
 
 
 def test_tcx_batching_invariance(L, nets):
@@ -125,10 +126,6 @@ def test_raw_heads_vs_reference_torchscript(L):
     print("\nraw heads vs TorchScript goldens: AffNet %.2e, OriNet %.2e" % (da, do))
     assert a(P).shape == (P.size(0), 3) and o(P).shape == (P.size(0), 2)
     assert da < 2e-5 and do < 2e-5
-    for eng in (L.ENGINE_TC,):      # first-generation engine: same entry points
-        a.set_engine(eng); o.set_engine(eng)
-        assert (a(P).cpu() - torch.from_numpy(z["affnet_raw"])).abs().max() < 2e-5
-        assert (o(P).cpu() - torch.from_numpy(z["orinet_raw"])).abs().max() < 2e-5
 
 
 def test_hardnet_bf16_engine(L):
@@ -149,3 +146,8 @@ def test_hardnet_bf16_engine(L):
     assert worst < 8e-3, worst
     hn.set_engine(L.ENGINE_TC2)
     assert (hn(P.to(DEV)).cpu() - O.hardnet_forward(P, W["hardnet"])).abs().max() < 6e-4      # and back
+    # engine numbers other than 0, 4 and 5 are refused and leave the engine as it was
+    lib = L.lib()
+    for eng in (1, 2, 3):
+        assert lib.ag_net_set_engine(hn.handle(), eng) == -1 and b"unknown engine" in lib.ag_last_error(), eng
+        assert hn.engine == L.ENGINE_TC2, eng
