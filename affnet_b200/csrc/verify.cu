@@ -1,9 +1,11 @@
 // Geometric verification of the batched matcher's tentatives (after ag_match_pairs), one CTA per pair:
 //   ag_homography_ransac         homography RANSAC (the notebook's ransac_validate: findHomography(src, dst, 2.0, 0.99, 50000))
+//   ag_fundamental_ransac        fundamental-matrix RANSAC (the notebook's commented-out findFundamentalMatrix(src, dst, 0.5))
 //   ag_gt_correspondences_pairs  ReprojectionStuff.get_GT_correspondence_indexes (the reference's "true matches" count), per pair
 //
-// RANSAC is deterministic and restated line by line in numpy by tests/oracle_ransac.py, so its decisions (samples, degeneracy, inlier
-// counts, the stopping point) are reproduced exactly.  For that reason all its arithmetic is fp64 and this file is compiled with
+// Both RANSACs are deterministic and restated line by line in numpy by tests/oracle_ransac.py and tests/oracle_fransac.py, so their
+// decisions (samples, degeneracy, inlier counts, the stopping point) are reproduced exactly.  For that reason all their arithmetic is
+// fp64, with + - * / sqrt only where a decision depends on it, and this file is compiled with
 // -fmad=false (build.sh): numpy rounds every product and sum separately, so fused multiply-adds here would move near-threshold decisions.
 // The block reductions of the refit run in a fixed order (strided per-thread sums, an xor butterfly per warp, warps in ascending order)
 // that the restatement repeats.
@@ -171,12 +173,98 @@ struct RansacShared {
     int bad;
 };
 
-// Inliers of H over all n tentatives (thread t handles rows t, t + VT, ...); writes the mask when `inl` is not NULL.  Block total.
+// Jacobi rotation (p, q) of the symmetric N x N A (row-major), accumulated into V, for row / column k: the column step, then (after
+// the caller's barrier) the row step.  Each element is one rounded product pair, in the restatement's order.
+struct JacobiRot {
+    double cs, sn;
+    bool skip;
+};
+__device__ __forceinline__ JacobiRot jacobi_rot(double app, double aqq, double apq) {
+    if (apq == 0.0) return {1.0, 0.0, true};
+    const double theta = (aqq - app) / (2.0 * apq);
+    const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+    const double cs = 1.0 / sqrt(t * t + 1.0);
+    return {cs, t * cs, false};
+}
+template <int N>
+__device__ __forceinline__ void jacobi_cols(double* A, int p, int q, int k, JacobiRot r) {
+    const double akp = A[N * k + p], akq = A[N * k + q];
+    A[N * k + p] = r.cs * akp - r.sn * akq;
+    A[N * k + q] = r.sn * akp + r.cs * akq;
+}
+template <int N>
+__device__ __forceinline__ void jacobi_rows(double* A, double* V, int p, int q, int k, JacobiRot r) {
+    const double apk = A[N * p + k], aqk = A[N * q + k];
+    A[N * p + k] = r.cs * apk - r.sn * aqk;
+    A[N * q + k] = r.sn * apk + r.cs * aqk;
+    const double vkp = V[N * k + p], vkq = V[N * k + q];
+    V[N * k + p] = r.cs * vkp - r.sn * vkq;
+    V[N * k + q] = r.sn * vkp + r.cs * vkq;
+}
+
+// Cyclic Jacobi of the symmetric 9x9 s.A with s.V = I, on warp 0 (lane k < 9 owns row / column k): JACOBI_SWEEPS sweeps of the pairs
+// (p, q), p < q, in row order.  Block-wide; on return s.A is (nearly) diagonal and s.V holds the eigenvectors in its columns.
+__device__ void jacobi9_warp(double* A, double* V) {
+    if (threadIdx.x < 32) {
+        const int k = threadIdx.x;
+        for (int sweep = 0; sweep < JACOBI_SWEEPS; sweep++)
+            for (int p = 0; p < 8; p++)
+                for (int q = p + 1; q < 9; q++) {
+                    const JacobiRot r = jacobi_rot(A[9 * p + p], A[9 * q + q], A[9 * p + q]);
+                    __syncwarp();
+                    if (r.skip) continue;
+                    if (k < 9) jacobi_cols<9>(A, p, q, k, r);
+                    __syncwarp();
+                    if (k < 9) jacobi_rows<9>(A, V, p, q, k, r);
+                    __syncwarp();
+                }
+    }
+    __syncthreads();
+}
+
+// The same sweeps on one thread, for a 3x3.
+__device__ __forceinline__ void jacobi3(double* A, double* V) {
+    for (int sweep = 0; sweep < JACOBI_SWEEPS; sweep++)
+        for (int p = 0; p < 2; p++)
+            for (int q = p + 1; q < 3; q++) {
+                const JacobiRot r = jacobi_rot(A[3 * p + p], A[3 * q + q], A[3 * p + q]);
+                if (r.skip) continue;
+                for (int k = 0; k < 3; k++) jacobi_cols<3>(A, p, q, k, r);
+                for (int k = 0; k < 3; k++) jacobi_rows<3>(A, V, p, q, k, r);
+            }
+}
+
+// Index of the smallest diagonal entry (the lowest on ties).
+template <int N>
+__device__ __forceinline__ int smallest_diag(const double* A) {
+    int m = 0;
+    for (int e = 1; e < N; e++)
+        if (A[N * e + e] < A[N * m + m]) m = e;
+    return m;
+}
+
+// s.A = the symmetric 9x9 whose upper triangle is s.sums (row by row), s.V = I, then jacobi9_warp.  Block-wide.
+__device__ void normal_matrix_eigen(RansacShared& s) {
+    if (threadIdx.x < 81) {
+        const int r = threadIdx.x / 9, c = threadIdx.x % 9, lo = min(r, c), hi = max(r, c);
+        s.A[threadIdx.x] = s.sums[lo * 9 - lo * (lo - 1) / 2 + (hi - lo)];
+        s.V[threadIdx.x] = r == c ? 1.0 : 0.0;
+    }
+    __syncthreads();
+    jacobi9_warp(s.A, s.V);
+}
+
+__device__ __forceinline__ bool is_inlier_f(const double* F, float4 c, double th2);
+
+// Inliers of H (a homography, or a fundamental matrix when FUND) over all n tentatives (thread t handles rows t, t + VT, ...); writes
+// the mask when `inl` is not NULL.  Block total.
+template <bool FUND = false>
 __device__ int score_rows(const double* H, const float* L1, const float* L2, const int* tent, int n, double th2, unsigned char* inl,
                           RansacShared& s) {
     int cnt = 0;
     for (int t = threadIdx.x; t < n; t += VT) {
-        const bool in = is_inlier(H, tent_centres(L1, L2, tent, t), th2);
+        const float4 c = tent_centres(L1, L2, tent, t);
+        const bool in = FUND ? is_inlier_f(H, c, th2) : is_inlier(H, c, th2);
         cnt += in;
         if (inl) inl[t] = in;
     }
@@ -228,51 +316,16 @@ __device__ bool refit(const float* L1, const float* L2, const int* tent, int n, 
             for (int l = k; l < 9; l++, e++) nm[e] = nm[e] + (in ? a1[k] * a1[l] + a2[k] * a2[l] : 0.0);
     }
     block_sum<45>(nm, s.red, s.sums);
-    if (threadIdx.x < 81) {
-        const int r = threadIdx.x / 9, c = threadIdx.x % 9, lo = min(r, c), hi = max(r, c);
-        s.A[threadIdx.x] = s.sums[lo * 9 - lo * (lo - 1) / 2 + (hi - lo)];
-        s.V[threadIdx.x] = r == c ? 1.0 : 0.0;
-    }
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        const int k = threadIdx.x;
-        for (int sweep = 0; sweep < JACOBI_SWEEPS; sweep++)
-            for (int p = 0; p < 8; p++)
-                for (int q = p + 1; q < 9; q++) {
-                    const double apq = s.A[9 * p + q], app = s.A[9 * p + p], aqq = s.A[9 * q + q];
-                    __syncwarp();
-                    if (apq == 0.0) continue;
-                    const double theta = (aqq - app) / (2.0 * apq);
-                    const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-                    const double cs = 1.0 / sqrt(t * t + 1.0), sn = t * cs;
-                    if (k < 9) {
-                        const double akp = s.A[9 * k + p], akq = s.A[9 * k + q];
-                        s.A[9 * k + p] = cs * akp - sn * akq;
-                        s.A[9 * k + q] = sn * akp + cs * akq;
-                    }
-                    __syncwarp();
-                    if (k < 9) {
-                        const double apk = s.A[9 * p + k], aqk = s.A[9 * q + k];
-                        s.A[9 * p + k] = cs * apk - sn * aqk;
-                        s.A[9 * q + k] = sn * apk + cs * aqk;
-                        const double vkp = s.V[9 * k + p], vkq = s.V[9 * k + q];
-                        s.V[9 * k + p] = cs * vkp - sn * vkq;
-                        s.V[9 * k + q] = sn * vkp + cs * vkq;
-                    }
-                    __syncwarp();
-                }
-        if (k == 0) {
-            int m = 0;
-            for (int e = 1; e < 9; e++)
-                if (s.A[9 * e + e] < s.A[9 * m + m]) m = e;
-            double Hn[9], tmp[9];
-            for (int e = 0; e < 9; e++) Hn[e] = s.V[9 * e + m];
-            const double T1[9] = {s1, 0.0, -(s1 * c1x), 0.0, s1, -(s1 * c1y), 0.0, 0.0, 1.0};
-            const double T2i[9] = {1.0 / s2, 0.0, c2x, 0.0, 1.0 / s2, c2y, 0.0, 0.0, 1.0};
-            mul3(T2i, Hn, tmp);
-            mul3(tmp, T1, s.Hr);
-            s.bad = !normalise_h(s.Hr);
-        }
+    normal_matrix_eigen(s);
+    if (threadIdx.x == 0) {
+        const int m = smallest_diag<9>(s.A);
+        double Hn[9], tmp[9];
+        for (int e = 0; e < 9; e++) Hn[e] = s.V[9 * e + m];
+        const double T1[9] = {s1, 0.0, -(s1 * c1x), 0.0, s1, -(s1 * c1y), 0.0, 0.0, 1.0};
+        const double T2i[9] = {1.0 / s2, 0.0, c2x, 0.0, 1.0 / s2, c2y, 0.0, 0.0, 1.0};
+        mul3(T2i, Hn, tmp);
+        mul3(tmp, T1, s.Hr);
+        s.bad = !normalise_h(s.Hr);
     }
     __syncthreads();
     return !s.bad;
@@ -459,6 +512,422 @@ __global__ void __launch_bounds__(VT) gt_kernel(const float* __restrict__ lafs1,
     if (tid == 0) ntrue[p] = run;
 }
 
+// ---- fundamental-matrix RANSAC (the notebook's alternative line, findFundamentalMatrix(src, dst, 0.5)) ----------------------------
+constexpr int F_SAMPLE = 7;            // correspondences per hypothesis
+constexpr int F_REFIT_MIN = 8;         // inliers needed by the 8-point refit
+constexpr double PIVOT_EPS = 1e-9;     // 7-point elimination: a column whose largest candidate |pivot| <= PIVOT_EPS * max|A| is free
+constexpr int BISECT_STEPS = 1100;     // bisection cap per bracketed cubic root: enough to close any bracket in the double range
+
+// Sampson test in pixels, division-free: (x2' F x1)^2 <= th^2 ((F x1)_0^2 + (F x1)_1^2 + (F' x2)_0^2 + (F' x2)_1^2), the right-hand
+// side positive.  A NaN anywhere fails both comparisons.
+__device__ __forceinline__ bool is_inlier_f(const double* F, float4 c, double th2) {
+    const double x = c.x, y = c.y, x2 = c.z, y2 = c.w;
+    const double a = F[0] * x + F[1] * y + F[2], b = F[3] * x + F[4] * y + F[5], d = F[6] * x + F[7] * y + F[8];
+    const double g = F[0] * x2 + F[3] * y2 + F[6], k = F[1] * x2 + F[4] * y2 + F[7];
+    const double e = x2 * a + y2 * b + d;
+    const double den = a * a + b * b + g * g + k * k;
+    return den > 0.0 && e * e <= th2 * den;
+}
+
+// F /= +-|F|_F, the sign making the largest-magnitude entry (the lowest index on ties) positive; false when F is zero or not finite.
+__device__ __forceinline__ bool normalise_f(double* F) {
+    double ss = 0.0;
+    int m = 0;
+    for (int k = 0; k < 9; k++) {
+        ss = ss + F[k] * F[k];
+        if (fabs(F[k]) > fabs(F[m])) m = k;
+    }
+    if (!(ss > 0.0) || !isfinite(ss)) return false;
+    const double nr = F[m] < 0.0 ? -sqrt(ss) : sqrt(ss);
+    for (int k = 0; k < 9; k++) F[k] = F[k] / nr;
+    return true;
+}
+
+// Hartley normalisation x -> T x, T = [s 0 -s cx; 0 s -s cy; 0 0 1], of both images.
+struct Hartley {
+    double c1x, c1y, s1, c2x, c2y, s2;
+};
+
+// F = T2' Fn T1, normalised by normalise_f.
+__device__ __forceinline__ bool denormalise_f(const Hartley& T, const double* Fn, double* F) {
+    const double T1[9] = {T.s1, 0.0, -(T.s1 * T.c1x), 0.0, T.s1, -(T.s1 * T.c1y), 0.0, 0.0, 1.0};
+    const double T2t[9] = {T.s2, 0.0, 0.0, 0.0, T.s2, 0.0, -(T.s2 * T.c2x), -(T.s2 * T.c2y), 1.0};
+    double tmp[9];
+    mul3(T2t, Fn, tmp);
+    mul3(tmp, T1, F);
+    return normalise_f(F);
+}
+
+// Real roots of a3 x^3 + a2 x^2 + a1 x + a0 in ascending order, with + - * / sqrt only (no libm transcendentals, so every platform gets
+// the same bits).  a3 == 0 drops to the quadratic (numerically stable form) or linear case.  Otherwise, on the monic form, the
+// critical points c1 < c2 (when the derivative has two real roots) split [-R, R], R = 1 + max|b_k| the Cauchy bound, into monotone
+// pieces; each piece whose end values change sign (a zero at its right end counts) is bisected, keeping the end with the left
+// value's strict sign as `lo`, until the midpoint equals an end (at most BISECT_STEPS times), and gives its `hi`.  Values are
+// evaluated from the original coefficients (Horner): a tiny a3 makes the monic ones huge and cancel at the finite roots.  Non-finite coefficients give no roots.
+__device__ __forceinline__ int cubic_roots(double a3, double a2, double a1, double a0, double* r) {
+    if (!isfinite(a3) || !isfinite(a2) || !isfinite(a1) || !isfinite(a0)) return 0;
+    if (a3 == 0.0) {
+        if (a2 == 0.0) {
+            if (a1 == 0.0) return 0;
+            r[0] = -a0 / a1;
+            return 1;
+        }
+        const double disc = a1 * a1 - 4.0 * a2 * a0;
+        if (disc < 0.0) return 0;
+        if (disc == 0.0) {
+            r[0] = -a1 / (2.0 * a2);
+            return 1;
+        }
+        const double sq = sqrt(disc);
+        const double q = a1 >= 0.0 ? -0.5 * (a1 + sq) : -0.5 * (a1 - sq);
+        const double x1 = q / a2, x2 = a0 / q;
+        r[0] = x1 < x2 ? x1 : x2;
+        r[1] = x1 < x2 ? x2 : x1;
+        return 2;
+    }
+    const double b2 = a2 / a3, b1 = a1 / a3, b0 = a0 / a3;
+    double m = fabs(b2);
+    if (fabs(b1) > m) m = fabs(b1);
+    if (fabs(b0) > m) m = fabs(b0);
+    const double R = 1.0 + m;
+    if (!isfinite(R)) return 0;
+    double x[4];
+    int np = 2;
+    x[0] = -R;
+    const double d = b2 * b2 - 3.0 * b1;
+    if (d > 0.0) {
+        const double sq = sqrt(d);
+        x[1] = (-b2 - sq) / 3.0;
+        x[2] = (-b2 + sq) / 3.0;
+        np = 4;
+    }
+    x[np - 1] = R;
+    int nr = 0;
+    for (int i = 0; i + 1 < np; i++) {
+        double lo = x[i], hi = x[i + 1];
+        const double fl = ((a3 * lo + a2) * lo + a1) * lo + a0, fh = ((a3 * hi + a2) * hi + a1) * hi + a0;
+        if (!((fl < 0.0 && fh >= 0.0) || (fl > 0.0 && fh <= 0.0))) continue;
+        for (int it = 0; it < BISECT_STEPS; it++) {
+            const double mid = 0.5 * (lo + hi);
+            if (mid == lo || mid == hi) break;   // the bracket is two adjacent doubles
+            const double fm = ((a3 * mid + a2) * mid + a1) * mid + a0;
+            if (fl < 0.0 ? fm < 0.0 : fm > 0.0) lo = mid;
+            else hi = mid;
+        }
+        r[nr++] = hi;
+    }
+    return nr;
+}
+
+// det(F2 + l D) = a3 l^3 + a2 l^2 + a1 l + a0: a0 = det F2, a1 = tr(adj(F2) D), a2 = tr(adj(D) F2), a3 = det D (first-row cofactor
+// expansions; traces summed over the 9 products in row-major order of the adjugate).
+__device__ __forceinline__ void det_cubic(const double* F2, const double* D, double* a) {
+    double A2[9], AD[9];
+    adj3(F2, A2);
+    adj3(D, AD);
+    a[0] = F2[0] * A2[0] + F2[1] * A2[3] + F2[2] * A2[6];
+    a[3] = D[0] * AD[0] + D[1] * AD[3] + D[2] * AD[6];
+    double t1 = 0.0, t2 = 0.0;
+    for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 3; c++) {
+            t1 = t1 + A2[3 * r + c] * D[3 * c + r];
+            t2 = t2 + AD[3 * r + c] * F2[3 * c + r];
+        }
+    a[1] = t1;
+    a[2] = t2;
+}
+
+// 7-point solver on normalised correspondences u[k] = (u1, v1, u2, v2): row k of the 7x9 constraint matrix is
+// (u2 u1, u2 v1, u2, v2 u1, v2 v1, v2, u1, v1, 1), so row k . vec(F) = x2' F x1.  Gauss-Jordan elimination column by column with
+// partial pivoting (largest |A[r][c]| over the rows not yet pivots, the lowest row on ties; a column is free when that is
+// <= PIVOT_EPS * max|A|); a rank below 7 is a degenerate sample (0 models).  The two free columns f1 < f2 give the null vectors F1, F2
+// (1 at their own free column, 0 at the other, -A[i][f] / A[i][pivot_i] at pivot column i); every real root l of det(F2 + l (F1 - F2))
+// (l of the form l F1 + (1 - l) F2) gives a model Fn = F2 + l D, in ascending l.  Returns the number of models (<= 3).
+__device__ __forceinline__ int seven_point(const double (&u)[F_SAMPLE][4], double (&Fn)[3][9]) {
+    double A[F_SAMPLE][9];
+    double mx = 0.0;
+    for (int k = 0; k < F_SAMPLE; k++) {
+        const double u1 = u[k][0], v1 = u[k][1], u2 = u[k][2], v2 = u[k][3];
+        const double row[9] = {u2 * u1, u2 * v1, u2, v2 * u1, v2 * v1, v2, u1, v1, 1.0};
+        for (int c = 0; c < 9; c++) {
+            A[k][c] = row[c];
+            if (fabs(row[c]) > mx) mx = fabs(row[c]);
+        }
+    }
+    const double tol = PIVOT_EPS * mx;
+    int pc[F_SAMPLE], rank = 0;
+    unsigned freemask = 0;
+    for (int c = 0; c < 9; c++) {
+        if (rank == F_SAMPLE) {
+            freemask |= 1u << c;
+            continue;
+        }
+        int pr = rank;
+        double pa = fabs(A[rank][c]);
+        for (int r = rank + 1; r < F_SAMPLE; r++)
+            if (fabs(A[r][c]) > pa) { pa = fabs(A[r][c]); pr = r; }
+        if (!(pa > tol)) {
+            freemask |= 1u << c;
+            continue;
+        }
+        if (pr != rank)
+            for (int k = 0; k < 9; k++) {
+                const double t = A[rank][k];
+                A[rank][k] = A[pr][k];
+                A[pr][k] = t;
+            }
+        for (int r = 0; r < F_SAMPLE; r++) {
+            if (r == rank) continue;
+            const double f = A[r][c] / A[rank][c];
+            for (int k = 0; k < 9; k++) A[r][k] = k == c ? 0.0 : A[r][k] - f * A[rank][k];
+        }
+        pc[rank++] = c;
+    }
+    if (rank < F_SAMPLE) return 0;
+    int f1 = -1, f2 = -1;
+    for (int c = 0; c < 9; c++)
+        if ((freemask >> c) & 1u) {
+            if (f1 < 0) f1 = c;
+            else if (f2 < 0) f2 = c;
+        }
+    double F1[9], F2[9], D[9];
+    for (int k = 0; k < 9; k++) { F1[k] = 0.0; F2[k] = 0.0; }
+    F1[f1] = 1.0;
+    F2[f2] = 1.0;
+    for (int i = 0; i < F_SAMPLE; i++) {
+        F1[pc[i]] = -(A[i][f1] / A[i][pc[i]]);
+        F2[pc[i]] = -(A[i][f2] / A[i][pc[i]]);
+    }
+    // Scale both null vectors to unit norm: in normalised coordinates the true F's constant entry is ~0, so the vector with its 1
+    // there is huge, all roots then bunch near l = 1 and the cubic's coefficients cancel.
+    double n1 = 0.0, n2 = 0.0;
+    for (int k = 0; k < 9; k++) {
+        n1 = n1 + F1[k] * F1[k];
+        n2 = n2 + F2[k] * F2[k];
+    }
+    n1 = sqrt(n1);
+    n2 = sqrt(n2);
+    for (int k = 0; k < 9; k++) {
+        F1[k] = F1[k] / n1;
+        F2[k] = F2[k] / n2;
+    }
+    for (int k = 0; k < 9; k++) D[k] = F1[k] - F2[k];
+    double a[4], l[3];
+    det_cubic(F2, D, a);
+    const int nl = cubic_roots(a[3], a[2], a[1], a[0], l);
+    for (int m = 0; m < nl; m++)
+        for (int k = 0; k < 9; k++) Fn[m][k] = F2[k] + l[m] * D[k];
+    return nl;
+}
+
+// Rank-2 fundamental matrix from the normalised 9x9 normal matrix in s.A / s.V (after normal_matrix_eigen): Fn = the eigenvector of
+// the smallest eigenvalue, then Fn <- Fn (I - v v'), v the eigenvector of the smallest eigenvalue of Fn'Fn (jacobi3), then
+// denormalised.  Thread 0.
+__device__ bool rank2_refit_f(const RansacShared& s, const Hartley& T, double* F) {
+    const int m = smallest_diag<9>(s.A);
+    double Fn[9], G[9], V[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0}, P[9], Fr[9];
+    for (int e = 0; e < 9; e++) Fn[e] = s.V[9 * e + m];
+    for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 3; c++) G[3 * r + c] = Fn[r] * Fn[c] + Fn[3 + r] * Fn[3 + c] + Fn[6 + r] * Fn[6 + c];
+    jacobi3(G, V);
+    const int m3 = smallest_diag<3>(G);
+    const double v[3] = {V[m3], V[3 + m3], V[6 + m3]};
+    for (int r = 0; r < 3; r++)
+        for (int c = 0; c < 3; c++) P[3 * r + c] = (r == c ? 1.0 : 0.0) - v[r] * v[c];
+    mul3(Fn, P, Fr);
+    return denormalise_f(T, Fr, F);
+}
+
+// Normalised 8-point least squares on the rows of the mask `inl` (Hartley normalisation of those rows, the 9x9 normal matrix of the
+// constraint rows reduced in the fixed order, its smallest eigenvector, rank 2).  Writes s.Hr; false when the inliers do not give a
+// finite non-zero F.
+__device__ bool refit_f(const float* L1, const float* L2, const int* tent, int n, const unsigned char* inl, int cnt, RansacShared& s) {
+    double st[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    for (int t = threadIdx.x; t < n; t += VT) {
+        const float4 c = tent_centres(L1, L2, tent, t);
+        const bool in = inl[t];
+        const double x1 = in ? (double)c.x : 0.0, y1 = in ? (double)c.y : 0.0, x2 = in ? (double)c.z : 0.0, y2 = in ? (double)c.w : 0.0;
+        st[0] = st[0] + x1; st[1] = st[1] + y1; st[2] = st[2] + x1 * x1; st[3] = st[3] + y1 * y1;
+        st[4] = st[4] + x2; st[5] = st[5] + y2; st[6] = st[6] + x2 * x2; st[7] = st[7] + y2 * y2;
+    }
+    block_sum<8>(st, reinterpret_cast<double(*)[8]>(&s.red[0][0]), s.sums);
+    const double nd = (double)cnt;
+    Hartley T;
+    T.c1x = s.sums[0] / nd; T.c1y = s.sums[1] / nd; T.c2x = s.sums[4] / nd; T.c2y = s.sums[5] / nd;
+    const double var1 = (s.sums[2] + s.sums[3]) / nd - (T.c1x * T.c1x + T.c1y * T.c1y);
+    const double var2 = (s.sums[6] + s.sums[7]) / nd - (T.c2x * T.c2x + T.c2y * T.c2y);
+    if (!(var1 > 0.0) || !(var2 > 0.0)) return false;   // uniform across the block: every thread returns
+    T.s1 = sqrt(2.0 / var1);
+    T.s2 = sqrt(2.0 / var2);
+    double nm[45];
+#pragma unroll
+    for (int k = 0; k < 45; k++) nm[k] = 0.0;
+    for (int t = threadIdx.x; t < n; t += VT) {
+        const float4 c = tent_centres(L1, L2, tent, t);
+        const bool in = inl[t];
+        const double u = (c.x - T.c1x) * T.s1, v = (c.y - T.c1y) * T.s1, up = (c.z - T.c2x) * T.s2, vp = (c.w - T.c2y) * T.s2;
+        const double a[9] = {up * u, up * v, up, vp * u, vp * v, vp, u, v, 1.0};
+        int e = 0;
+#pragma unroll
+        for (int k = 0; k < 9; k++)
+#pragma unroll
+            for (int l = k; l < 9; l++, e++) nm[e] = nm[e] + (in ? a[k] * a[l] : 0.0);
+    }
+    block_sum<45>(nm, s.red, s.sums);
+    normal_matrix_eigen(s);
+    if (threadIdx.x == 0) s.bad = !rank2_refit_f(s, T, s.Hr);
+    __syncthreads();
+    return !s.bad;
+}
+
+__device__ __forceinline__ bool finite4(float4 c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z) && isfinite(c.w); }
+
+__global__ void __launch_bounds__(VT) fransac_kernel(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2, int S2,
+                                                     int cap2, const int* __restrict__ pairs, const int* __restrict__ tent_all,
+                                                     const int* __restrict__ ntent, int tcap, double th2, double log1mconf, int max_iters,
+                                                     uint64_t seed, float* __restrict__ Fout, unsigned char* __restrict__ inl_all,
+                                                     int* __restrict__ ninl, int* __restrict__ iters) {
+    __shared__ RansacShared s;
+    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int i, j;
+    const int n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
+    const int* tent = tent_all + (size_t)p * tcap * 2;
+    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
+        if (tid == 0) ninl[p] = -1;
+        return;
+    }
+    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
+    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
+    unsigned char* inl = inl_all + (size_t)p * tcap;
+    int best = 0, h_done = 0;
+    if (n >= F_SAMPLE) {
+        // Hartley normalisation of the rows whose four coordinates are finite (their number in st[8])
+        double st[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        for (int t = tid; t < n; t += VT) {
+            const float4 c = tent_centres(L1, L2, tent, t);
+            const bool in = finite4(c);
+            const double x1 = in ? (double)c.x : 0.0, y1 = in ? (double)c.y : 0.0, x2 = in ? (double)c.z : 0.0, y2 = in ? (double)c.w : 0.0;
+            st[0] = st[0] + x1; st[1] = st[1] + y1; st[2] = st[2] + x1 * x1; st[3] = st[3] + y1 * y1;
+            st[4] = st[4] + x2; st[5] = st[5] + y2; st[6] = st[6] + x2 * x2; st[7] = st[7] + y2 * y2;
+            st[8] = st[8] + (in ? 1.0 : 0.0);
+        }
+        block_sum<9>(st, reinterpret_cast<double(*)[9]>(&s.red[0][0]), s.sums);
+        const double nd = s.sums[8];
+        Hartley T;
+        T.c1x = s.sums[0] / nd; T.c1y = s.sums[1] / nd; T.c2x = s.sums[4] / nd; T.c2y = s.sums[5] / nd;
+        const double var1 = (s.sums[2] + s.sums[3]) / nd - (T.c1x * T.c1x + T.c1y * T.c1y);
+        const double var2 = (s.sums[6] + s.sums[7]) / nd - (T.c2x * T.c2x + T.c2y * T.c2y);
+        T.s1 = sqrt(2.0 / var1);
+        T.s2 = sqrt(2.0 / var2);
+        // fewer than 7 finite rows, or all of them on one point in an image: no hypothesis is drawn (iters = 0)
+        const bool search = nd >= (double)F_SAMPLE && var1 > 0.0 && var2 > 0.0;
+        const int ntiles = (n + VTILE - 1) / VTILE;
+        for (int h0 = 0; search; h0 += VT) {
+            const int h = h0 + tid;
+            double Fm[3][9];
+            bool okm[3] = {false, false, false};   // model r (root r in ascending order) exists
+            if (h < max_iters) {
+                int idx[F_SAMPLE], got = 0;
+                for (int d = 0; d < MAX_DRAWS && got < F_SAMPLE; d++) {
+                    const int v = draw_index(seed, h, d, n);
+                    bool dup = false;
+                    for (int q = 0; q < got; q++) dup |= idx[q] == v;
+                    if (!dup) idx[got++] = v;
+                }
+                if (got == F_SAMPLE) {
+                    double u[F_SAMPLE][4];
+                    bool fin = true;
+                    for (int q = 0; q < F_SAMPLE; q++) {
+                        const float4 c = tent_centres(L1, L2, tent, idx[q]);
+                        fin &= finite4(c);
+                        u[q][0] = (c.x - T.c1x) * T.s1; u[q][1] = (c.y - T.c1y) * T.s1;
+                        u[q][2] = (c.z - T.c2x) * T.s2; u[q][3] = (c.w - T.c2y) * T.s2;
+                    }
+                    double Fn[3][9];
+                    const int nl = fin ? seven_point(u, Fn) : 0;
+#pragma unroll
+                    for (int r = 0; r < 3; r++)
+                        if (r < nl) okm[r] = denormalise_f(T, Fn[r], Fm[r]);
+                }
+            }
+            const bool any = okm[0] || okm[1] || okm[2];
+            int cnt[3] = {0, 0, 0};
+            for (int tb = 0; tb < ntiles; tb++) {
+                const int t0 = tb * VTILE, m = min(VTILE, n - t0);
+                if (ntiles > 1 || h0 == 0) {
+                    __syncthreads();
+                    for (int t = tid; t < m; t += VT) s.tile[t] = tent_centres(L1, L2, tent, t0 + t);
+                    __syncthreads();
+                }
+                if (any)
+                    for (int t = 0; t < m; t++) {
+                        const float4 c = s.tile[t];
+#pragma unroll
+                        for (int r = 0; r < 3; r++)
+                            if (okm[r]) cnt[r] += is_inlier_f(Fm[r], c, th2);
+                    }
+            }
+            // best of the chunk: highest count, then lowest h, then lowest root
+            int rb = -1, cb = -1;
+#pragma unroll
+            for (int r = 0; r < 3; r++)
+                if (okm[r] && cnt[r] > cb) { cb = cnt[r]; rb = r; }
+            const unsigned long long mine =
+                any ? ((unsigned long long)cb << 34) | ((unsigned long long)(0x7fffffff - h) << 2) | (unsigned long long)(3 - rb) : 0ull;
+            unsigned long long key = mine;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
+                key = k2 > key ? k2 : key;
+            }
+            if (lane == 0) s.key[warp] = key;
+            __syncthreads();
+            unsigned long long bk = 0;
+#pragma unroll
+            for (int w = 0; w < VT / 32; w++) bk = s.key[w] > bk ? s.key[w] : bk;
+            const int bc = (int)(bk >> 34);
+            if (bk != 0 && bc > best) {
+                if (mine == bk) {
+#pragma unroll
+                    for (int r = 0; r < 3; r++)
+                        if (r == rb)
+#pragma unroll
+                            for (int k = 0; k < 9; k++) s.H[k] = Fm[r][k];
+                }
+                best = bc;
+            }
+            h_done = min(h0 + VT, max_iters);
+            double need;   // adaptive number of samples for `confidence`
+            const double pr = (double)best / (double)n, p7 = pr * pr * pr * pr * pr * pr * pr;
+            if (p7 >= 1.0) need = 0.0;
+            else if (p7 <= 0.0 || 1.0 - p7 == 1.0) need = INFINITY;   // log(1 - p7) would be 0: no sample count reaches confidence
+            else need = ceil(log1mconf / log(1.0 - p7));
+            __syncthreads();
+            if ((double)h_done >= fmin(need, (double)max_iters)) break;
+        }
+    }
+    if (best > 0) {
+        int cnt = score_rows<true>(s.H, L1, L2, tent, n, th2, inl, s);   // = best
+        for (int r = 0; r < REFIT_ROUNDS && cnt >= F_REFIT_MIN; r++) {
+            if (!refit_f(L1, L2, tent, n, inl, cnt, s)) break;
+            const int c2 = score_rows<true>(s.Hr, L1, L2, tent, n, th2, nullptr, s);
+            if (c2 < cnt) break;
+            cnt = c2;
+            if (tid < 9) s.H[tid] = s.Hr[tid];
+            __syncthreads();
+            score_rows<true>(s.H, L1, L2, tent, n, th2, inl, s);
+        }
+        best = cnt;
+    } else {
+        for (int t = tid; t < n; t += VT) inl[t] = 0;
+    }
+    if (tid < 9) Fout[(size_t)p * 9 + tid] = best > 0 ? (float)s.H[tid] : 0.f;
+    if (tid == 0) {
+        ninl[p] = best;
+        if (iters) iters[p] = h_done;
+    }
+}
+
 int verify_args(const char* fn, const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                 const int* d_tent, const int* d_ntent, int tcap) {
     const char* msg = nullptr;
@@ -490,6 +959,22 @@ int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_
     ransac_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
                                                       log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_H, d_inl, d_ninl, d_iters);
     AG_CHECK_LAUNCH("ransac_kernel");
+    return AG_OK;
+}
+
+int ag_fundamental_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                          const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
+                          float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
+    int rc = verify_args("ag_fundamental_ransac", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc) return rc;
+    AG_REQUIRE(d_F && d_inl && d_ninl, "NULL output");
+    AG_REQUIRE(inl_th > 0.f && isfinite(inl_th), "inl_th must be finite and > 0");
+    AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
+    AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
+    const double th = inl_th;
+    fransac_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
+                                                       log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_F, d_inl, d_ninl, d_iters);
+    AG_CHECK_LAUNCH("fransac_kernel");
     return AG_OK;
 }
 

@@ -392,6 +392,25 @@ int ag_match_pairs(const float* d_desc1, const int* d_count1, int S1, int cap1, 
  *   d_H [P,3,3] (H[2][2] = 1), d_inl [P,tcap] u8, d_ninl [P], d_iters [P] (hypotheses evaluated; may be NULL).  n < 4 tentatives or no
  *   hypothesis with an inlier: ninl = 0, H = 0, mask rows < n = 0.
  *   AG_ERR_INVALID also for inl_th not finite and > 0, confidence outside (0, 1), max_iters < 1.
+ * ag_fundamental_ransac: fundamental-matrix RANSAC per pair (the notebook's alternative, findFundamentalMatrix(src, dst, 0.5)), for
+ * scenes with depth, which one homography does not explain; the arguments, refusals and -1 rule of ag_homography_ransac.  Everything is
+ * fp64 in a fixed operation order.  The centres of the rows whose four coordinates are finite are Hartley-normalised (centroid, scale
+ * sqrt(2) / RMS radius) once per pair.  Hypothesis h draws 7 distinct indices with the homography's sampler; its 7x9 constraint matrix
+ * is reduced by Gauss-Jordan elimination with partial pivoting (a column whose best pivot is <= 1e-9 max|A| is free; rank < 7, or a
+ * non-finite centre, is a degenerate sample).  The two null vectors F1, F2, each scaled to unit norm, give the cubic
+ * det(l F1 + (1 - l) F2), whose real roots are found with + - * / sqrt only (critical points by the quadratic formula, sign changes on
+ * [-R, c1, c2, R] with R the Cauchy bound, each bracket bisected until it is two adjacent doubles, at most 1100 times); each root is a
+ * model, denormalised as F = T2' Fn T1 (at most 3 per sample).  Inlier, in pixels and without
+ * division: (x2' F x1)^2 <= inl_th^2 ((F x1)_0^2 + (F x1)_1^2 + (F' x2)_0^2 + (F' x2)_1^2) with a positive right-hand side (the Sampson
+ * distance; a NaN row is never an inlier).  Best: most inliers, then lowest h, then lowest root.  Samples are evaluated in chunks of
+ * 256; after each chunk the search stops once the samples evaluated reach min(N, max_iters), N = ceil(log(1 - confidence) /
+ * log(1 - (best/n)^7)), infinite when 1 - (best/n)^7 rounds to 1 (inlier ratios below ~0.5 %).  Then up to 3 rounds of normalised 8-point least squares on the inliers (at least 8): the smallest eigenvector
+ * of the 9x9 normal matrix, rank 2 enforced as F (I - v v') with v the smallest eigenvector of F'F, each round kept only if the inlier
+ * count does not drop.
+ *   d_F [P,3,3]: unit Frobenius norm, its largest-magnitude entry (the lowest index on ties) positive; d_inl [P,tcap] the mask of that
+ *   F; d_ninl [P], d_iters [P] (samples evaluated; may be NULL).  n < 7 tentatives, fewer than 7 finite ones, all of them on one point
+ *   of an image (iters = 0), or no model with an inlier: ninl = 0, F = 0, mask rows < n = 0.
+ *   AG_ERR_INVALID also for inl_th not finite and > 0, confidence outside (0, 1), max_iters < 1.
  * ag_gt_correspondences_pairs: get_GT_correspondence_indexes (ReprojectionStuff.py:126-137) per pair with d_H1to2 [P,3,3]: the image-2
  * centres of all the pair's tentatives are mapped through H^-1 into image 1, and tentative t is true when ANY of them lies within
  * dist_threshold of its image-1 centre, by the fp32 distance sqrt(|(|p|^2 + |a|^2) - 2 a.p + 1e-12|) (nearest: the lowest index among the
@@ -400,6 +419,9 @@ int ag_match_pairs(const float* d_desc1, const int* d_count1, int S1, int cap1, 
 int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                          const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
                          float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
+int ag_fundamental_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                          const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
+                          float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
 int ag_gt_correspondences_pairs(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                                 const int* d_tent, const int* d_ntent, int tcap, const float* d_H1to2, float dist_threshold,
                                 float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream);
