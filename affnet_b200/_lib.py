@@ -98,7 +98,6 @@ PROTOTYPES = {
     "ag_lafs_left_multiply": (i32, [vp, vp, vp, i32, vp]),
     "ag_affnet_forward_raw": (i32, [vp, vp, i32, vp, vp, sz, vp]),
     "ag_orinet_forward_raw": (i32, [vp, vp, i32, vp, vp, sz, vp]),
-    "ag_debug_pyramid_mode": (i32, [i32]),
     "ag_debug_tcx_layer": (i32, [vp, vp, i32, i32, vp, vp, sz, vp]),
     "ag_debug_libm": (i32, [vp, vp, i32, vp, vp, vp, vp]),
     "ag_debug_tanhf": (i32, [vp, i32, vp, vp]),

@@ -3,16 +3,15 @@
 //
 // Replaces HessianResp.forward (HandCraftedModules.py:58-78), NMS3d / NMS3dAndComposeA
 // (HandCraftedModules.py:208-291) and the detection loop + global top-k of multiScaleDetector
-// (SparseImgRepresenter.py:53-111).  Response maps never touch HBM in the fused path: each CTA stages a
-// 36x36 window of three pyramid levels in shared memory, derives the three 34x34 response windows and
-// runs NMS, border/octave-map masking, counting, soft-argmax and compaction from there.
+// (SparseImgRepresenter.py:53-111).  Response maps never touch HBM when detecting on a pyramid: at nlevels = 3
+// detect_rows_kernel streams the rows of an octave's five levels through registers; at other level counts each
+// CTA of detect_level_kernel stages a 36x36 window of three pyramid levels in shared memory, derives the three
+// 34x34 response windows and runs NMS, border/octave-map masking, counting, soft-argmax and compaction from there.
 //
 // Integer exactness: given identical inputs the set of surviving pixels is identical to the reference's
 // because every float op that decides survival is done in the reference's order with explicit
 // non-contracted intrinsics (__fmul_rn/__fsub_rn/__fadd_rn): the Hessian determinant, `(x - max) + 1e-5 > 0`,
 // `resp * (1 - octaveMap)` and the float->uint8 wrap of the octave map (Q4).
-#include <stdlib.h>
-
 #include <type_traits>
 
 #include "common.cuh"
@@ -259,206 +258,34 @@ __global__ void __launch_bounds__(DNT) detect_level_kernel(const DetectParams P)
 
 
 // ======================================================================================================================
-// Fused single-launch detector for nlevels = 3 (the reference's only configuration): one CTA stages a 36x36 window of all
-// FIVE pyramid levels of its octave, derives the five 34x34 response windows once, and runs the three detection levels
-// from shared memory.  The reference's sequential octave-map logic (level k sees the map left by the accepted levels
-// below it; a level with <= 1 positive maxima is dropped and leaves no trace, HandCraftedModules.py:246-256) is made
-// launch-free by counting every acceptance hypothesis (a1, a2 in {0,1}) in the same pass and storing, with each candidate,
+// Single-launch detector for nlevels = 3 (the reference's only configuration): one launch runs the three detection levels of
+// every octave from its five pyramid levels.  The reference's sequential octave-map logic (level k sees the map left by the
+// accepted levels below it; a level with <= 1 positive maxima is dropped and leaves no trace, HandCraftedModules.py:246-256) is
+// made launch-free by counting every acceptance hypothesis (a1, a2 in {0,1}) in the same pass and storing, with each candidate,
 // the raw NMS values of the same pixel at the levels below; `resolve_kernel` then picks the branch the counters select and
 // computes the masked response with the reference's exact fp32 / uint8-wrap arithmetic.
 // ======================================================================================================================
 constexpr int NVAR = 16;  // per (image, octave): [0] pos1, [1..2] pos2[a1], [3..6] pos3[a1][a2], [7] emit1, [8..9] emit2[a1], [10..13] emit3[a1][a2]
 
-struct FusedOctave {
-    const float* lvl[5];
-    float s4[5], sc[5];
-    int h, w, tiles_x, tiles_y, tile_base;
-};
-struct FusedParams {
-    FusedOctave oct[AG_MAX_OCTAVES];
-    int n_oct, total_tiles;
-    float th;
-    int mr_border, cand_cap;
-    float* cand_val;
-    float* cand_aux;
-    uint32_t* cand_seq;
-    float* cand_scyx;
-    int* cand_count;
-    int* variants;  // [B][n_oct][NVAR]
-};
-
 __device__ __forceinline__ uint8_t om_after(uint8_t om, float val) { return float_to_u8_wrap(__fadd_rn((float)om, val)); }
 __device__ __forceinline__ float masked(float nms, uint8_t om) { return __fmul_rn(nms, __fsub_rn(1.0f, (float)om)); }
 
-__global__ void __launch_bounds__(DNT) detect_fused_kernel(const FusedParams P) {
-    extern __shared__ __align__(16) float s_dyn[];
-    float (*s_a)[PW][PW + 1] = reinterpret_cast<float (*)[PW][PW + 1]>(s_dyn);                            // pyramid windows, later row-max maps
-    float (*s_resp)[RW][RW + 1] = reinterpret_cast<float (*)[RW][RW + 1]>(s_dyn + 5 * PW * (PW + 1));     // response windows
-    __shared__ int s_var[NVAR];
-    __shared__ int s_base[2];
-    int t = blockIdx.x, oi = 0;
-#pragma unroll 1
-    for (int i = 1; i < P.n_oct; i++)
-        if (t >= P.oct[i].tile_base) oi = i;
-    const FusedOctave& O = P.oct[oi];
-    t -= O.tile_base;
-    const int b = blockIdx.y, h = O.h, w = O.w;
-    const int ty = t / O.tiles_x, tx = t - ty * O.tiles_x;
-    const int y0 = ty * DT, x0 = tx * DT;
-    const size_t img_off = (size_t)b * h * w;
-    if (threadIdx.x < NVAR) s_var[threadIdx.x] = 0;
-    if (threadIdx.x < 2) s_base[threadIdx.x] = 0;
-    // 1. pyramid windows (origin y0-2, x0-2), replicate-clamped
-#pragma unroll
-    for (int d = 0; d < 5; d++) {
-        const float* src = O.lvl[d] + img_off;
-        for (int i = threadIdx.x; i < PW * PW; i += DNT) {
-            const int ly = i / PW, lx = i - ly * PW;
-            s_a[d][ly][lx] = __ldg(src + (size_t)clampi(y0 - 2 + ly, 0, h - 1) * w + clampi(x0 - 2 + lx, 0, w - 1));
-        }
-    }
-    __syncthreads();
-    // 2. response windows (origin y0-1, x0-1), zero outside the image
-#pragma unroll
-    for (int d = 0; d < 5; d++)
-        for (int i = threadIdx.x; i < RW * RW; i += DNT) {
-            const int ly = i / RW, lx = i - ly * RW;
-            const int gy = y0 - 1 + ly, gx = x0 - 1 + lx;
-            s_resp[d][ly][lx] = (gy >= 0 && gy < h && gx >= 0 && gx < w) ? hessian_at(s_a[d], ly + 1, lx + 1, O.s4[d], P.th) : 0.f;
-        }
-    __syncthreads();
-    // 3. separable 3x3 max: row pass into the (dead) pyramid windows.  Zero padding is exact: responses are >= 0 (or NaN) and the
-    //    centre always takes part in the max.  max.NaN: a NaN anywhere in the window suppresses the centre, as MaxPool3d does.
-    float (*s_rm)[RW][DT] = reinterpret_cast<float (*)[RW][DT]>(&s_a[0][0][0]);
-    for (int i = threadIdx.x; i < 5 * RW * DT; i += DNT) {
-        const int d = i / (RW * DT), r = i - d * RW * DT, ly = r / DT, j = r - ly * DT;
-        s_rm[d][ly][j] = fmax_nan(fmax_nan(s_resp[d][ly][j], s_resp[d][ly][j + 1]), s_resp[d][ly][j + 2]);
-    }
-    __syncthreads();
-    // 4. per pixel: three NMS decisions, hypothesis counters, candidate slots
-    const bool border_ok = (P.mr_border < w) && (P.mr_border < h);
-    constexpr int PPT = DT * DT / DNT;
-    float nms[PPT][3];
-    int var[NVAR];
-#pragma unroll
-    for (int i = 0; i < NVAR; i++) var[i] = 0;
-    int n_emit = 0;
-#pragma unroll
-    for (int k = 0; k < PPT; k++) {
-        const int i = threadIdx.x + k * DNT, ly = i / DT, lx = i - ly * DT;
-        const int gy = y0 + ly, gx = x0 + lx;
-        nms[k][0] = nms[k][1] = nms[k][2] = 0.f;
-        if (gy < h && gx < w && border_ok && gy >= P.mr_border && gy < h - P.mr_border && gx >= P.mr_border && gx < w - P.mr_border) {
-            float M[5];
-#pragma unroll
-            for (int d = 0; d < 5; d++) M[d] = fmax_nan(fmax_nan(s_rm[d][ly][lx], s_rm[d][ly + 1][lx]), s_rm[d][ly + 2][lx]);
-#pragma unroll
-            for (int q = 0; q < 3; q++) {
-                const float x = s_resp[q + 1][ly + 1][lx + 1];
-                const float m = fmax_nan(fmax_nan(M[q], M[q + 1]), M[q + 2]);
-                nms[k][q] = (__fadd_rn(__fsub_rn(x, m), 1e-5f) > 0.f) ? x : 0.f;   // NMS3d, HandCraftedModules.py:220
-            }
-            // The reference's NMS value is 0 * x, NaN at a NaN or infinite centre, where these kernels keep 0.  Nothing observable
-            // differs: such a value is no candidate (DESIGN.md §2), is not > 0, and turns the octave map to 0 where the map can
-            // only be 0 already (a non-finite x at level q lies in the window of level q-1, which then had no survivor there).
-            const float n1 = nms[k][0], n2 = nms[k][1], n3 = nms[k][2];
-            if (n1 != 0.f || n2 != 0.f || n3 != 0.f) {
-                n_emit += (n1 != 0.f) + (n2 != 0.f) + (n3 != 0.f);
-                var[0] += n1 > 0.f; var[7] += n1 != 0.f;
-#pragma unroll
-                for (int a1 = 0; a1 < 2; a1++) {
-                    const uint8_t om1 = a1 ? om_after(0, n1) : (uint8_t)0;
-                    const float v2 = masked(n2, om1);
-                    var[1 + a1] += v2 > 0.f; var[8 + a1] += v2 != 0.f;
-#pragma unroll
-                    for (int a2 = 0; a2 < 2; a2++) {
-                        const uint8_t om2 = a2 ? om_after(om1, v2) : om1;
-                        const float v3 = masked(n3, om2);
-                        var[3 + a1 * 2 + a2] += v3 > 0.f; var[10 + a1 * 2 + a2] += v3 != 0.f;
-                    }
-                }
-            }
-        }
-    }
-    const unsigned lane = threadIdx.x & 31;
-    const unsigned any = __ballot_sync(0xffffffffu, n_emit > 0);
-    int incl = n_emit, warp_base = 0;
-    if (any) {
-#pragma unroll
-        for (int i = 0; i < 14; i++) {
-            int v = var[i];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-            if (lane == 0 && v) atomicAdd(&s_var[i], v);
-        }
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= (unsigned)o) incl += v;
-        }
-        const int wsum = __shfl_sync(0xffffffffu, incl, 31);
-        if (lane == 0) warp_base = atomicAdd(&s_base[0], wsum);
-        warp_base = __shfl_sync(0xffffffffu, warp_base, 0);
-    }
-    __syncthreads();
-    if (s_base[0] == 0) return;
-    if (threadIdx.x < 14 && s_var[threadIdx.x]) atomicAdd(&P.variants[((size_t)b * P.n_oct + oi) * NVAR + threadIdx.x], s_var[threadIdx.x]);
-    if (threadIdx.x == 0) s_base[1] = atomicAdd(&P.cand_count[b], s_base[0]);
-    __syncthreads();
-    if (n_emit == 0) return;
-    int dst = s_base[1] + warp_base + (incl - n_emit);
-    // 5. soft-argmax + emission (HandCraftedModules.py:266-290)
-    const float min_size = (float)min(h, w);
-#pragma unroll
-    for (int k = 0; k < PPT; k++) {
-        const int i = threadIdx.x + k * DNT, ly = i / DT, lx = i - ly * DT;
-        const int gy = y0 + ly, gx = x0 + lx;
-#pragma unroll
-        for (int q = 0; q < 3; q++) {
-            if (nms[k][q] == 0.f) continue;
-            if (dst < P.cand_cap) {
-                float ns = 0.f, ny = 0.f, nx = 0.f, den = 0.f;
-#pragma unroll
-                for (int d = 0; d < 3; d++)
-#pragma unroll
-                    for (int dy = 0; dy < 3; dy++)
-#pragma unroll
-                        for (int dx = 0; dx < 3; dx++) {
-                            const float r = s_resp[q + d][ly + dy][lx + dx];
-                            ns = fmaf(O.sc[q + d], r, ns);
-                            ny = fmaf(-0.5f + (float)dy, r, ny);
-                            nx = fmaf(-0.5f + (float)dx, r, nx);
-                            den += r;
-                        }
-                den = __fadd_rn(den, 1e-8f);
-                const size_t o = (size_t)b * P.cand_cap + dst;
-                P.cand_val[o] = nms[k][q];
-                P.cand_aux[o * 2 + 0] = nms[k][0];
-                P.cand_aux[o * 2 + 1] = nms[k][1];
-                P.cand_seq[o] = ((uint32_t)(oi * 3 + q) << SEQ_PIX_BITS) | (uint32_t)(gy * w + gx);
-                P.cand_scyx[o * 3 + 0] = __fdiv_rn(__fdiv_rn(ns, den), min_size);
-                P.cand_scyx[o * 3 + 1] = __fdiv_rn(__fadd_rn(__fdiv_rn(ny, den), (float)gy), (float)h);
-                P.cand_scyx[o * 3 + 2] = __fdiv_rn(__fadd_rn(__fdiv_rn(nx, den), (float)gx), (float)w);
-            }
-            dst++;
-        }
-    }
-}
-
-
 // ======================================================================================================================
-// Register-resident formulation of the fused detector: one warp owns a band of rows of a 30-column strip (32 lanes = 30
-// output columns + one response-halo column each side), walks down the rows keeping three pyramid rows of all five levels
-// in registers, takes horizontal neighbours by warp shuffle, and never touches shared memory on the common path:
-//   per pixel and level: 1 coalesced load + 2 shuffles + the Hessian; separable 3x3 max via 2 shuffles + FMNMX3.
-// Candidates (about 1 % of the pixels) take a warp-cooperative slow path that gathers the 3x3x3 response neighbourhood by
-// shuffle for the soft-argmax.  Semantics are identical to detect_fused_kernel (same hypothesis counters, same records).
+// detect_rows_kernel: one warp owns a band of rows of a 30-column strip (32 lanes = 30 output columns + one response-halo column
+// each side) and walks down the rows, the pyramid rows of all five levels streamed through a per-warp cp.async ring:
+//   * every pyramid row is read from the ring ONCE (3 LDS per level); what later rows need of it stays in registers: the centre, the
+//     half difference 0.5 l - 0.5 r (the gxy term of the rows above / below) and (l - 2 c) + r (gxx of the row itself);
+//   * horizontal neighbours come by warp shuffle: the separable 3x3 max and the horizontal sums of the soft-argmax;
+//   * the row loop is unrolled by three with compile-time slot indices: no register rotation;
+//   * the row fetch is branch-free: one cp.async per level from a per-lane offset, the two halo columns by a predicated second one;
+//   * candidates are staged per warp and flushed with one atomic; the soft-argmax divisions wait for the flush, where 32 lanes
+//     finish 32 candidates at once.
+// Unlike hessian_at, the kernel drops the zero taps of the gxy filters: next to an infinite pixel it gives +inf where the reference
+// has NaN.  No decision differs, since an infinite and a NaN response both suppress every window they lie in and never survive
+// themselves.
 // ======================================================================================================================
 constexpr int WCOLS = 30;   // output columns per warp strip
-#ifndef AG_WROWS
-#define AG_WROWS 48   // 32: 0.43 ms, 48: 0.40, 64: 0.39 per step of 16 images (4 halo rows per band); 48 keeps enough warps for one image
-#endif
-constexpr int WROWS = AG_WROWS;   // output rows per warp band
+constexpr int WROWS = 48;   // output rows per warp band.  32: 0.43 ms, 48: 0.40, 64: 0.39 per step of 16 images (4 halo rows per band); 48 keeps enough warps for one image
 constexpr int WNT = 128;    // 4 warps per CTA, one band each
 
 struct WarpOctave {
@@ -479,223 +306,11 @@ struct WarpParams {
     int* variants;
 };
 
-// The register kernels drop the zero taps of the gxy filters (see hessian_at): next to an infinite pixel they give +inf where the
-// reference has NaN.  No decision differs, since an infinite and a NaN response both suppress every window they lie in and never
-// survive themselves.
-__device__ __forceinline__ float hessian_regs(float tl, float tc, float tr, float ml, float mc, float mr, float bl, float bc, float br, float s4, float th) {
-    const float gxx = __fadd_rn(__fsub_rn(ml, __fmul_rn(2.0f, mc)), mr);
-    const float gyy = __fadd_rn(__fsub_rn(tc, __fmul_rn(2.0f, mc)), bc);
-    const float gxa = __fsub_rn(__fmul_rn(0.5f, tl), __fmul_rn(0.5f, tr));
-    const float gxb = __fsub_rn(__fmul_rn(0.5f, bl), __fmul_rn(0.5f, br));
-    const float gxy = __fsub_rn(__fmul_rn(0.5f, gxa), __fmul_rn(0.5f, gxb));
-    const float det = __fsub_rn(__fmul_rn(gxx, gyy), __fmul_rn(gxy, gxy));
-    return fmax_nan(__fsub_rn(__fmul_rn(fabsf(det), s4), th), 0.0f);
-}
-
 constexpr int WRING = 8;   // ring of pyramid rows per warp (cp.async prefetch distance WPD, 3 rows live)
 constexpr int WPD = 5;
 constexpr int WROWLEN = 34;  // 32 lane columns + one extra column each side
 constexpr int WCBUF = 96;    // staged candidates per warp (a row yields at most 90); flushed with ONE atomic
 
-__device__ __forceinline__ void cp_async4(float* dst, const float* src) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
-}
-
-template <int S0, int S1, int S2>   // response slots holding rows y-1, y, y+1
-struct Slots {};
-
-__global__ void __launch_bounds__(WNT) detect_warp_kernel(const WarpParams P) {
-    __shared__ float s_ring[WNT / 32][WRING][5][WROWLEN];
-    __shared__ float s_cbuf[WNT / 32][7][WCBUF];   // per-warp candidate staging: val, aux0, aux1, seq, sc, y, x
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    int u = blockIdx.x * (WNT / 32) + wib;
-    if (u >= P.total_units) return;
-    int oi = 0;
-#pragma unroll 1
-    for (int i = 1; i < P.n_oct; i++)
-        if (u >= P.oct[i].unit_base) oi = i;
-    const WarpOctave& O = P.oct[oi];
-    u -= O.unit_base;
-    const int b = blockIdx.y, h = O.h, w = O.w;
-    const int band = u / O.strips_x, strip = u - band * O.strips_x;
-    const int r0 = band * WROWS;
-    const int gx = strip * WCOLS - 1 + lane;            // lane's column; lanes 0 / 31 are the response halo
-    const bool col_in = gx >= 0 && gx < w;
-    const int cx = clampi(gx, 0, w - 1), cxl = clampi(gx - 1, 0, w - 1), cxr = clampi(gx + 1, 0, w - 1);
-    const size_t img_off = (size_t)b * h * w;
-    const bool border_ok = (P.mr_border < w) && (P.mr_border < h);
-    const bool col_ok = lane >= 1 && lane <= WCOLS && col_in && border_ok && gx >= P.mr_border && gx < w - P.mr_border;
-    const int rows_out = min(WROWS, h - r0);
-    const int n_rows = rows_out + 4;                     // pyramid rows r0-2 .. r0+rows_out+1
-    float (*ring)[5][WROWLEN] = s_ring[wib];
-
-    auto issue_row = [&](int c) {                        // pyramid row r0-2+c -> ring slot c % WRING (replicate-clamped)
-        if (c < n_rows) {
-            const int cy = clampi(r0 - 2 + c, 0, h - 1);
-#pragma unroll
-            for (int d = 0; d < 5; d++) {
-                const float* rowp = O.lvl[d] + img_off + (size_t)cy * w;
-                float* dst = ring[c % WRING][d];
-                cp_async4(dst + lane + 1, rowp + cx);
-                if (lane == 0) cp_async4(dst, rowp + cxl);
-                if (lane == 31) cp_async4(dst + 33, rowp + cxr);
-            }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-
-    // rotating register state of the three most recent response rows (slot 0 = oldest): response, horizontal 3-max, and the
-    // horizontal sums the soft-argmax needs (sum r, sum x_off * r), all taken from the same two shuffles
-    float rs[5][3], rmx[5][3], hs[5][3], hx[5][3];
-#pragma unroll
-    for (int d = 0; d < 5; d++)
-#pragma unroll
-        for (int q = 0; q < 3; q++) { rs[d][q] = 0.f; rmx[d][q] = 0.f; hs[d][q] = 0.f; hx[d][q] = 0.f; }
-    int var[14];
-#pragma unroll
-    for (int i = 0; i < 14; i++) var[i] = 0;
-    const float min_size = (float)min(h, w);
-
-    int buf_n = 0;   // warp-uniform
-    float (*cbuf)[WCBUF] = s_cbuf[wib];
-    auto flush = [&]() {
-        if (buf_n == 0) return;
-        int base = 0;
-        if (lane == 0) base = atomicAdd(&P.cand_count[b], buf_n);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        __syncwarp();
-        for (int i = lane; i < buf_n; i += 32) {
-            const int dst = base + i;
-            if (dst < P.cand_cap) {
-                const size_t o = (size_t)b * P.cand_cap + dst;
-                P.cand_val[o] = cbuf[0][i];
-                P.cand_aux[o * 2 + 0] = cbuf[1][i];
-                P.cand_aux[o * 2 + 1] = cbuf[2][i];
-                P.cand_seq[o] = __float_as_uint(cbuf[3][i]);
-                P.cand_scyx[o * 3 + 0] = cbuf[4][i];
-                P.cand_scyx[o * 3 + 1] = cbuf[5][i];
-                P.cand_scyx[o * 3 + 2] = cbuf[6][i];
-            }
-        }
-        __syncwarp();
-        buf_n = 0;
-    };
-
-#pragma unroll 1
-    for (int c = 0; c < WPD; c++) issue_row(c);
-    // consume pyramid row c: response row (image row r0-3+c) enters slot 2; output row y = r0+c-4 sits in slot 1
-#pragma unroll 1
-    for (int c = 0; c < n_rows; c++) {
-        asm volatile("cp.async.wait_group %0;" ::"n"(WPD - 1) : "memory");
-        __syncwarp();
-        if (c >= 2) {
-            const int yy = r0 - 3 + c;
-            const bool in = col_in && yy >= 0 && yy < h;
-            const float (*t)[WROWLEN] = ring[(c - 2) % WRING];
-            const float (*m)[WROWLEN] = ring[(c - 1) % WRING];
-            const float (*bt)[WROWLEN] = ring[c % WRING];
-#pragma unroll
-            for (int d = 0; d < 5; d++) {
-                rs[d][0] = rs[d][1]; rs[d][1] = rs[d][2]; rmx[d][0] = rmx[d][1]; rmx[d][1] = rmx[d][2];
-                hs[d][0] = hs[d][1]; hs[d][1] = hs[d][2]; hx[d][0] = hx[d][1]; hx[d][1] = hx[d][2];
-                float r = 0.f;
-                if (in) r = hessian_regs(t[d][lane], t[d][lane + 1], t[d][lane + 2], m[d][lane], m[d][lane + 1], m[d][lane + 2], bt[d][lane], bt[d][lane + 1],
-                                         bt[d][lane + 2], O.s4[d], P.th);
-                float l = __shfl_up_sync(0xffffffffu, r, 1), rr = __shfl_down_sync(0xffffffffu, r, 1);
-                if (lane == 0) l = 0.f;
-                if (lane == 31) rr = 0.f;
-                rs[d][2] = r;
-                rmx[d][2] = fmax_nan(fmax_nan(l, r), rr);
-                hs[d][2] = (l + r) + rr;
-                hx[d][2] = fmaf(1.5f, rr, fmaf(0.5f, r, -0.5f * l));   // x offsets [-0.5, 0.5, 1.5] (Q2)
-            }
-        }
-        if (c >= 4) {
-            const int y = r0 + c - 4;
-            float n1 = 0.f, n2 = 0.f, n3 = 0.f;
-            if (col_ok && y >= P.mr_border && y < h - P.mr_border) {
-                float M[5];
-#pragma unroll
-                for (int d = 0; d < 5; d++) M[d] = fmax_nan(fmax_nan(rmx[d][0], rmx[d][1]), rmx[d][2]);
-                const float x1 = rs[1][1], x2 = rs[2][1], x3 = rs[3][1];
-                n1 = (__fadd_rn(__fsub_rn(x1, fmax_nan(fmax_nan(M[0], M[1]), M[2])), 1e-5f) > 0.f) ? x1 : 0.f;   // NMS3d, HandCraftedModules.py:220
-                n2 = (__fadd_rn(__fsub_rn(x2, fmax_nan(fmax_nan(M[1], M[2]), M[3])), 1e-5f) > 0.f) ? x2 : 0.f;
-                n3 = (__fadd_rn(__fsub_rn(x3, fmax_nan(fmax_nan(M[2], M[3]), M[4])), 1e-5f) > 0.f) ? x3 : 0.f;
-            }
-            const unsigned m1 = __ballot_sync(0xffffffffu, n1 != 0.f), m2 = __ballot_sync(0xffffffffu, n2 != 0.f), m3 = __ballot_sync(0xffffffffu, n3 != 0.f);
-            if (m1 | m2 | m3) {
-                const int row_total = __popc(m1) + __popc(m2) + __popc(m3);
-                if (buf_n + row_total > WCBUF) flush();
-                if ((n1 != 0.f) || (n2 != 0.f) || (n3 != 0.f)) {
-                    var[0] += n1 > 0.f; var[7] += n1 != 0.f;
-#pragma unroll
-                    for (int a1 = 0; a1 < 2; a1++) {
-                        const uint8_t om1 = a1 ? om_after(0, n1) : (uint8_t)0;
-                        const float v2 = masked(n2, om1);
-                        var[1 + a1] += v2 > 0.f; var[8 + a1] += v2 != 0.f;
-#pragma unroll
-                        for (int a2 = 0; a2 < 2; a2++) {
-                            const uint8_t om2 = a2 ? om_after(om1, v2) : om1;
-                            const float v3 = masked(n3, om2);
-                            var[3 + a1 * 2 + a2] += v3 > 0.f; var[10 + a1 * 2 + a2] += v3 != 0.f;
-                        }
-                    }
-                    // soft-argmax (HandCraftedModules.py:266-290) from the rotating horizontal sums: no shuffles, no loop over lanes
-                    const unsigned lt = (1u << lane) - 1u;
-                    const float nn[3] = {n1, n2, n3};
-                    const int pos[3] = {buf_n + __popc(m1 & lt), buf_n + __popc(m1) + __popc(m2 & lt), buf_n + __popc(m1) + __popc(m2) + __popc(m3 & lt)};
-#pragma unroll
-                    for (int q = 0; q < 3; q++) {
-                        if (nn[q] == 0.f) continue;
-                        float ns = 0.f, ny = 0.f, nx = 0.f, den = 0.f;
-#pragma unroll
-                        for (int d = 0; d < 3; d++) {
-                            const float S = (hs[q + d][0] + hs[q + d][1]) + hs[q + d][2];
-                            ns = fmaf(O.sc[q + d], S, ns);
-                            ny += fmaf(1.5f, hs[q + d][2], fmaf(0.5f, hs[q + d][1], -0.5f * hs[q + d][0]));
-                            nx += (hx[q + d][0] + hx[q + d][1]) + hx[q + d][2];
-                            den += S;
-                        }
-                        den = __fadd_rn(den, 1e-8f);
-                        const int dst = pos[q];
-                        cbuf[0][dst] = nn[q];
-                        cbuf[1][dst] = n1;
-                        cbuf[2][dst] = n2;
-                        cbuf[3][dst] = __uint_as_float(((uint32_t)(oi * 3 + q) << SEQ_PIX_BITS) | (uint32_t)(y * w + gx));
-                        cbuf[4][dst] = __fdiv_rn(__fdiv_rn(ns, den), min_size);
-                        cbuf[5][dst] = __fdiv_rn(__fadd_rn(__fdiv_rn(ny, den), (float)y), (float)h);
-                        cbuf[6][dst] = __fdiv_rn(__fadd_rn(__fdiv_rn(nx, den), (float)gx), (float)w);
-                    }
-                }
-                buf_n += row_total;
-            }
-        }
-        __syncwarp();            // every lane has finished reading ring rows <= c before slot (c+WPD)%WRING is refilled
-        issue_row(c + WPD);
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    flush();
-#pragma unroll
-    for (int i = 0; i < 14; i++) {
-        int v = var[i];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0 && v) atomicAdd(&P.variants[((size_t)b * P.n_oct + oi) * NVAR + i], v);
-    }
-}
-
-// ======================================================================================================================
-// Same detector, rows in registers (r02; ncu source view of detect_warp_kernel: 691 warp instructions per row, of which 155 issue the
-// next row's cp.async through divergent halo branches and dynamically indexed constant loads, 45 re-read the 3x3 pyramid windows from
-// shared memory, 40 rotate state registers, ~90 are the lone-lane soft-argmax divisions):
-//   * every pyramid row is read from the ring ONCE (3 LDS per level); what later rows need of it stays in registers: the centre, the
-//     half difference 0.5 l - 0.5 r (the gxy term of the rows above / below) and (l - 2 c) + r (gxx of the row itself) - the same
-//     float operations in the same order as hessian_regs, so the response is bit-identical;
-//   * the row loop is unrolled by three with compile-time slot indices: no register rotation;
-//   * the row fetch is branch-free: one cp.async per level from a per-lane offset, the two halo columns by a predicated second one;
-//   * the soft-argmax divisions move to the candidate flush, where 32 lanes finish 32 candidates at once.
-// Records, counters and their semantics are those of detect_warp_kernel / detect_fused_kernel.
-// ======================================================================================================================
 template <int I> struct IC { static constexpr int value = I; };
 
 template <int OFF>
@@ -711,10 +326,11 @@ __device__ __forceinline__ void cp_async4_off_if(uint32_t dst, const float* src,
 static_assert(WROWS <= 255, "8-bit per-lane hypothesis counters");
 constexpr int RCB = 10;   // staged candidate record: val, n1, n2, seq, ns, ny, nx, den, y, x
 
-#ifndef AG_DETROWS_MINB
-#define AG_DETROWS_MINB 3   // 168 registers (4 B of spills), three CTAs per SM: 0.43 - 0.44 ms; 2 CTAs at 202 registers 0.47 - 0.49; 4 CTAs at 128 registers 0.59
-#endif
-__global__ void __launch_bounds__(WNT, AG_DETROWS_MINB) detect_rows_kernel(const WarpParams P) {
+constexpr int DETROWS_MINB = 3;   // 168 registers, no spills, three CTAs per SM: 0.43 - 0.44 ms; 2 CTAs at 202 registers 0.47 - 0.49; 4 CTAs at 128 registers 0.59
+
+// Off: the type of the element offsets from an octave's first level, int when they fit (ag_detect decides), long long otherwise
+template <typename Off>
+__global__ void __launch_bounds__(WNT, DETROWS_MINB) detect_rows_kernel(const WarpParams P) {
     __shared__ float s_ring[WNT / 32][WRING][5][WROWLEN];
     __shared__ float s_cbuf[WNT / 32][RCB][WCBUF];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -726,12 +342,12 @@ __global__ void __launch_bounds__(WNT, AG_DETROWS_MINB) detect_rows_kernel(const
         if (u >= P.oct[i].unit_base) oi = i;
     u -= P.oct[oi].unit_base;
     // octave constants into registers (dynamically indexed kernel parameters are constant-bank loads at every use otherwise)
-    // (the five level pointers become one pointer + 32-bit element offsets: the levels of an octave lie in one pyramid allocation)
+    // (the five level pointers become one pointer + element offsets: the levels of an octave lie in one pyramid allocation)
     const float* const lvl0 = P.oct[oi].lvl[0];
-    int loff[5];
+    Off loff[5];
     float s4[5];
 #pragma unroll
-    for (int d = 0; d < 5; d++) { loff[d] = (int)(P.oct[oi].lvl[d] - lvl0); s4[d] = P.oct[oi].s4[d]; }
+    for (int d = 0; d < 5; d++) { loff[d] = (Off)(P.oct[oi].lvl[d] - lvl0); s4[d] = P.oct[oi].s4[d]; }
     const int h = P.oct[oi].h, w = P.oct[oi].w, strips_x = P.oct[oi].strips_x;
     const float th = P.th;
     const int b = blockIdx.y;
@@ -742,7 +358,7 @@ __global__ void __launch_bounds__(WNT, AG_DETROWS_MINB) detect_rows_kernel(const
     const int cx = clampi(gx, 0, w - 1);
     const bool halo_lane = lane == 0 || lane == 31;
     const int hdelta = (lane == 0 ? clampi(gx - 1, 0, w - 1) : clampi(gx + 1, 0, w - 1)) - cx;   // extra column of the halo lanes
-    const int base_off = b * h * w + cx;                 // element offsets inside one pyramid allocation fit an int (ag_detect checks)
+    const Off base_off = (Off)b * h * w + cx;
     const bool border_ok = (P.mr_border < w) && (P.mr_border < h);
     const bool col_ok = lane >= 1 && lane <= WCOLS && col_in && border_ok && gx >= P.mr_border && gx < w - P.mr_border;
     const int rows_out = min(WROWS, h - r0);
@@ -754,7 +370,7 @@ __global__ void __launch_bounds__(WNT, AG_DETROWS_MINB) detect_rows_kernel(const
     auto issue_row = [&](int c) {                        // pyramid row r0-2+c -> ring slot c % WRING (replicate-clamped)
         if (c < n_rows) {
             const int cy = clampi(r0 - 2 + c, 0, h - 1);
-            const int off = base_off + cy * w;
+            const Off off = base_off + (Off)cy * w;
             const uint32_t so = (uint32_t)((c % WRING) * (5 * WROWLEN * 4));
             cp_async4_off<0 * WROWLEN * 4>(sdst + so, lvl0 + (loff[0] + off)); cp_async4_off_if<0 * WROWLEN * 4>(sdst_h + so, lvl0 + (loff[0] + off + hdelta), halo_lane);
             cp_async4_off<1 * WROWLEN * 4>(sdst + so, lvl0 + (loff[1] + off)); cp_async4_off_if<1 * WROWLEN * 4>(sdst_h + so, lvl0 + (loff[1] + off + hdelta), halo_lane);
@@ -772,7 +388,7 @@ __global__ void __launch_bounds__(WNT, AG_DETROWS_MINB) detect_rows_kernel(const
     for (int d = 0; d < 5; d++)
 #pragma unroll
         for (int q = 0; q < 3; q++) { pc[d][q] = 0.f; ph[d][q] = 0.f; pg[d][q] = 0.f; rs[d][q] = 0.f; rmx[d][q] = 0.f; hs[d][q] = 0.f; hx[d][q] = 0.f; }
-    // hypothesis counters of this lane, four 8-bit counters per register (a lane counts at most once per row and counter: <= WROWS = 32)
+    // hypothesis counters of this lane, four 8-bit counters per register (a lane counts at most once per row and counter: <= WROWS = 48)
     unsigned varp[4] = {0u, 0u, 0u, 0u};
     auto bump = [&](int i, bool cond) { varp[i >> 2] += cond ? (1u << ((i & 3) * 8)) : 0u; };
     const float min_size = (float)min(h, w);
@@ -819,7 +435,7 @@ __global__ void __launch_bounds__(WNT, AG_DETROWS_MINB) detect_rows_kernel(const
             pc[d][PN] = C;
             ph[d][PN] = __fsub_rn(__fmul_rn(0.5f, L), __fmul_rn(0.5f, R));
             pg[d][PN] = __fadd_rn(__fsub_rn(L, __fmul_rn(2.0f, C)), R);
-            // hessian_regs with t = slot PO, m = slot PM, b = this row
+            // the Hessian of row slot PM, from the rows above (slot PO) and below (this row)
             const float gyy = __fadd_rn(__fsub_rn(pc[d][PO], __fmul_rn(2.0f, pc[d][PM])), C);
             const float gxy = __fsub_rn(__fmul_rn(0.5f, ph[d][PO]), __fmul_rn(0.5f, ph[d][PN]));
             const float det = __fsub_rn(__fmul_rn(pg[d][PM], gyy), __fmul_rn(gxy, gxy));
@@ -1424,68 +1040,37 @@ int ag_detect(const ag_pyramid_plan_t* p, const float* d_pyr, float th, int mr_b
                         "memset counters");
     if (rc != AG_OK) return rc;
     if (n_det == 3) {
-        // single-launch fused detector + hypothesis resolution
-        FusedParams F;
-        memset(&F, 0, sizeof(F));
-        F.n_oct = p->n_octaves; F.th = th; F.mr_border = mr_border; F.cand_cap = ws->cand_cap;
-        F.cand_val = ws->d_cand_val; F.cand_aux = ws->d_cand_aux; F.cand_seq = ws->d_cand_seq; F.cand_scyx = ws->d_cand_scyx;
-        F.cand_count = ws->d_cand_count; F.variants = ws->d_variants;
-        int tiles = 0;
+        // single-launch detector + hypothesis resolution
+        WarpParams Wp;
+        memset(&Wp, 0, sizeof(Wp));
+        Wp.n_oct = p->n_octaves; Wp.th = th; Wp.mr_border = mr_border; Wp.cand_cap = ws->cand_cap;
+        Wp.cand_val = ws->d_cand_val; Wp.cand_aux = ws->d_cand_aux; Wp.cand_seq = ws->d_cand_seq; Wp.cand_scyx = ws->d_cand_scyx;
+        Wp.cand_count = ws->d_cand_count; Wp.variants = ws->d_variants;
+        int units = 0;
         for (int o = 0; o < p->n_octaves; o++) {
-            FusedOctave& O = F.oct[o];
+            WarpOctave& O = Wp.oct[o];
             for (int d = 0; d < 5; d++) {
                 O.lvl[d] = d_pyr + p->level_offset[o][d];
                 O.s4[d] = (float)pow(p->sigma[o][d], 4.0);
                 O.sc[d] = (float)p->sigma[o][d];
             }
             O.h = p->h[o]; O.w = p->w[o];
-            O.tiles_x = cdiv(O.w, DT); O.tiles_y = cdiv(O.h, DT);
-            O.tile_base = tiles;
-            tiles += O.tiles_x * O.tiles_y;
+            O.strips_x = cdiv(O.w, WCOLS); O.bands_y = cdiv(O.h, WROWS);
+            O.unit_base = units;
+            units += O.strips_x * O.bands_y;
         }
-        F.total_tiles = tiles;
-        static const bool use_tiled = getenv("AG_DETECT_TILED") != nullptr;   // A/B switch: shared-memory tiled variant
-        if (!use_tiled) {
-            WarpParams Wp;
-            memset(&Wp, 0, sizeof(Wp));
-            Wp.n_oct = p->n_octaves; Wp.th = th; Wp.mr_border = mr_border; Wp.cand_cap = ws->cand_cap;
-            Wp.cand_val = ws->d_cand_val; Wp.cand_aux = ws->d_cand_aux; Wp.cand_seq = ws->d_cand_seq; Wp.cand_scyx = ws->d_cand_scyx;
-            Wp.cand_count = ws->d_cand_count; Wp.variants = ws->d_variants;
-            int units = 0;
-            for (int o = 0; o < p->n_octaves; o++) {
-                WarpOctave& O = Wp.oct[o];
-                for (int d = 0; d < 5; d++) { O.lvl[d] = F.oct[o].lvl[d]; O.s4[d] = F.oct[o].s4[d]; O.sc[d] = F.oct[o].sc[d]; }
-                O.h = p->h[o]; O.w = p->w[o];
-                O.strips_x = cdiv(O.w, WCOLS); O.bands_y = cdiv(O.h, WROWS);
-                O.unit_base = units;
-                units += O.strips_x * O.bands_y;
-            }
-            Wp.total_units = units;
-            static const bool use_v1 = getenv("AG_DETECT_WARP_V1") != nullptr;     // A/B switch: the first register formulation
-            // detect_rows_kernel addresses an octave's levels with 32-bit element offsets from its first level
-            bool fits32 = true;
-            for (int o = 0; o < p->n_octaves; o++) {
-                long long lo = 0, hi = 0;
-                for (int d = 0; d < 5; d++) { const long long off = Wp.oct[o].lvl[d] - Wp.oct[o].lvl[0]; lo = off < lo ? off : lo; hi = off > hi ? off : hi; }
-                if (lo < -(1ll << 30) || hi + (long long)p->B * p->h[o] * p->w[o] >= (1ll << 31) - 64) fits32 = false;
-            }
-            if (use_v1 || !fits32) {
-                detect_warp_kernel<<<dim3(cdiv(units, WNT / 32), p->B), WNT, 0, st>>>(Wp);
-                AG_CHECK_LAUNCH("detect_warp_kernel");
-            } else {
-                detect_rows_kernel<<<dim3(cdiv(units, WNT / 32), p->B), WNT, 0, st>>>(Wp);
-                AG_CHECK_LAUNCH("detect_rows_kernel");
-            }
-            resolve_kernel<<<dim3(8, p->B), 256, 0, st>>>(ws->d_variants, p->n_octaves, ws->cand_cap, ws->d_cand_count, ws->d_cand_val, ws->d_cand_aux,
-                                                           ws->d_cand_seq, ws->d_level_pos, ws->d_level_emit);
-            AG_CHECK_LAUNCH("resolve_kernel");
-            return AG_OK;
+        Wp.total_units = units;
+        // 32-bit element offsets from an octave's first level when every level of every octave allows them
+        bool fits32 = true;
+        for (int o = 0; o < p->n_octaves; o++) {
+            long long lo = 0, hi = 0;
+            for (int d = 0; d < 5; d++) { const long long off = Wp.oct[o].lvl[d] - Wp.oct[o].lvl[0]; lo = off < lo ? off : lo; hi = off > hi ? off : hi; }
+            if (lo < -(1ll << 30) || hi + (long long)p->B * p->h[o] * p->w[o] >= (1ll << 31) - 64) fits32 = false;
         }
-        constexpr size_t fsmem = sizeof(float) * (5 * PW * (PW + 1) + 5 * RW * (RW + 1));
-        static SmemAttrOnce attr_once;
-        if ((rc = attr_once.ensure(detect_fused_kernel, fsmem, "detect smem attr")) != AG_OK) return rc;
-        detect_fused_kernel<<<dim3(tiles, p->B), DNT, fsmem, st>>>(F);
-        AG_CHECK_LAUNCH("detect_fused_kernel");
+        const dim3 grid(cdiv(units, WNT / 32), p->B);
+        if (fits32) detect_rows_kernel<int><<<grid, WNT, 0, st>>>(Wp);
+        else detect_rows_kernel<long long><<<grid, WNT, 0, st>>>(Wp);
+        AG_CHECK_LAUNCH("detect_rows_kernel");
         resolve_kernel<<<dim3(8, p->B), 256, 0, st>>>(ws->d_variants, p->n_octaves, ws->cand_cap, ws->d_cand_count, ws->d_cand_val, ws->d_cand_aux,
                                                        ws->d_cand_seq, ws->d_level_pos, ws->d_level_emit);
         AG_CHECK_LAUNCH("resolve_kernel");

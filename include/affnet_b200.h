@@ -204,9 +204,6 @@ size_t ag_net_blob_floats(int kind);
  * Any other value is refused with AG_ERR_INVALID and leaves the engine as it was. */
 int ag_net_set_engine(ag_net_t* net, int engine);
 int ag_net_get_engine(const ag_net_t* net);
-/* Developer switch: 1 = ag_pyramid_build runs one launch per octave (pyramid_fused.cuh: bit-identical, measured slower), 0 = one
- * launch per level (default).  Returns the previous mode. */
-int ag_debug_pyramid_mode(int fused);
 /* Developer diagnostic: run the trunk with the handle's engine on materialised patches [n,32,32] up to conv layer `upto` and return that
  * layer's activations as fp32 [n,C,H,H].  ENGINE_SIMT: the exact-fp32 trunk, upto 1..6, its fp32 output as it is.  Any other engine: the
  * second-generation trunk (ENGINE_TC2_BF16: bf16 operands, HardNet; otherwise fp16), upto 2..6, its hi [+ lo] planes in the engine's HBM

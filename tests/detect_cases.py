@@ -1,5 +1,5 @@
 """Detector inputs aimed at the soft-argmax's edges (test infrastructure, not product): pyramids with isolated blobs on the seams of
-the register kernels' 30-column strips and 48-row bands and at the image's edges and corners, pyramids scaled down by powers of two
+the register kernel's 30-column strips and 48-row bands and at the image's edges and corners, pyramids scaled down by powers of two
 (low contrast: the 1e-8 of den goes from negligible to dominant, and the responses become fp32 subnormals), and the reference's
 golden detector rows with their candidates' (slot, pixel)."""
 import torch
@@ -8,7 +8,7 @@ import affnet_oracle as O
 from detect_restated import EPS_DEN, level_maps, windows
 from helpers import SEQ_PIX_BITS, gold, gray_from_rgb, synthetic_image
 
-WCOLS, WROWS = 30, 48                   # output columns per strip and rows per band of detect_rows_kernel / detect_warp_kernel
+WCOLS, WROWS = 30, 48                   # output columns per strip and rows per band of detect_rows_kernel
 LOW_K = (0, 8, 12, 16, 20, 60, 66)      # low-contrast cases: the pyramid times 2^-k (exact), the responses times 2^-2k
 SEAM_SHAPE = (100, 130)                 # octave 0 holds the band seam at rows 47 / 48 and 95 / 96, strip seams at 29 / 30 and 59 / 60
 TINY = 2.0 ** -126                      # smallest normal fp32

@@ -6,9 +6,9 @@ The soft-argmax of every candidate reads the 3x3x3 window of response maps aroun
     ns = sum sc_d r,  ny = sum (dy - 0.5) r,  nx = sum (dx - 0.5) r,  den = sum r,   (d, dy, dx in 0..2, sc_d = (float)sigma_d)
 
 in one of two fixed orders:
-- "taps" (detect_level_kernel, detect_fused_kernel): for d, dy, dx in turn, ns = fmaf(sc_d, r, ns), ny = fmaf(dy - 0.5, r, ny),
+- "taps" (detect_level_kernel): for d, dy, dx in turn, ns = fmaf(sc_d, r, ns), ny = fmaf(dy - 0.5, r, ny),
   nx = fmaf(dx - 0.5, r, nx), den = den + r;
-- "rows" (detect_rows_kernel, detect_warp_kernel): per level and window row, hs = (l + c) + r and hx = fmaf(1.5, r, fmaf(0.5, c,
+- "rows" (detect_rows_kernel): per level and window row, hs = (l + c) + r and hx = fmaf(1.5, r, fmaf(0.5, c,
   -0.5 * l)); per level S = (hs0 + hs1) + hs2, ns = fmaf(sc_d, S, ns), ny += fmaf(1.5, hs2, fmaf(0.5, hs1, -0.5 * hs0)),
   nx += (hx0 + hx1) + hx2, den += S.
 Both end in den + 1e-8f, sc = (ns / den) / min(h, w), y = ((ny / den) + y) / h, x = ((nx / den) + x) / w, and write_keypoint's

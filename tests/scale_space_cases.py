@@ -30,9 +30,6 @@ PYR_CASES = ([("noise", 1, 97, 127, nl, s, 5) for nl in (2, 3, 4, 5, 6) for s in
              + [("noise", 2, 97, 127, 3, 1.6, 5), ("noise", 2, 97, 127, 2, 2.0, 0), ("noise", 2, 97, 127, 6, 0.5, 33),
                 ("noise", 2, 97, 127, 4, 1.0, 5)]
              + [("noise", 1, 767, 1023, 3, 1.6, 5), ("noise", 1, 767, 1023, 5, 1.0, 0)])
-# ag_debug_pyramid_mode(1); the fused kernel needs w % 4 == 0 and aligned levels, so 200x328 runs it for octaves 0 and 1 and the
-# per-level launches for the rest (w = 82, 41)
-FUSED_CASES = [("graf", 1) + GRAF + (3, 1.6, 5), ("noise", 2, 200, 328, 3, 1.6, 5)]
 NO_TMA_PYR_CASES = [("graf", 1) + GRAF + (3, 1.6, 5), ("noise", 2, 97, 127, 3, 1.6, 5), ("noise", 1, 767, 1023, 3, 1.6, 5)]
 NO_TMA_BLUR_CASES = [(3, 200, 328, R) for R in (1, 6, 12)]                                # AG_BLUR_NO_TMA=1 subprocess
 BATCH_CASE = (3, 97, 127, 3, 1.6, 5)                                                       # == three B = 1 pyramids
@@ -41,7 +38,7 @@ MAX_TAPS = 25
 
 
 def pyramid_blurs(plan):
-    """The blur_kernel launches of ag_pyramid_build's per-level path: (h, w, sigma, input offset, output offset), offsets in floats
+    """The blur_kernel launches of ag_pyramid_build: (h, w, sigma, input offset, output offset), offsets in floats
     from the pyramid buffer (None: the input image)."""
     out = []
     for o in range(plan.n_octaves):

@@ -1,6 +1,6 @@
 """An exact fp32 restatement of the scale-space kernels, operation by operation (test infrastructure, not product).
 
-`blur_kernel` / `octave_kernel` (pyramid.cu, pyramid_fused.cuh) and the bilinear sampler (`laf_sample_xy` + `bilinear_zero`,
+`blur_kernel` (pyramid.cu) and the bilinear sampler (`laf_sample_xy` + `bilinear_zero`,
 common.cuh) are written with explicit fp32 roundings and fused multiply-adds in a fixed order, so their outputs are a function of
 the inputs alone.  This module computes the same function on the CPU (or, for large images, on the device) from float64 tensor
 operations: every fp32 step is one float64 operation whose exact result is then rounded to fp32, and the one step that float64

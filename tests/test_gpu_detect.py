@@ -9,9 +9,6 @@ then raster index), the rule the C ABI documents (tests/helpers.py::OracleCandid
 The pyramids come from the GPU blur (bench shapes, odd and tiny shapes, many images) or are built directly (level-drop pyramids,
 tiled pyramids whose responses tie), so the stage is tested on inputs no blur would produce as well."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -25,7 +22,6 @@ from helpers import (SENTINEL, Detector, OracleCandidates, adversarial_pyramid, 
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda"
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 MR = 5.192
 ISENT = int(SENTINEL)
 AG_ERR_CAPACITY = -3
@@ -391,61 +387,3 @@ def test_pipeline_other_level_counts_equal_single_image_api(L, nlevels):
             d = hn(det.extract_patches_from_pyr(dL, PS=32))
             assert torch.equal(resp[b, :n], r) and torch.equal(lafs[b, :n], dL) and torch.equal(desc[b, :n], d), (nlevels, b)
     print("\npipeline nlevels %d: counts %s" % (nlevels, cnt.tolist()))
-
-
-# ---- A/B kernel variants ----------------------------------------------------------------------------------------------------------
-_SCRIPT = r"""
-import sys, torch
-sys.path.insert(0, sys.argv[2]); sys.path.insert(0, sys.argv[2] + "/tests"); sys.path.insert(0, sys.argv[2] + "/oracle")
-import affnet_b200._lib as L
-from helpers import Detector, adversarial_pyramid, flat_pyramid, gpu_pyramids, mixed_batch
-res = {}
-plan, buf, _ = gpu_pyramids(L, mixed_batch(97, 131, 5), 3)
-plan8 = L.make_plan(8, 40, 40, 3, 1.6, 5)
-for name, (p, b) in {"odd": (plan, buf), "adv": (plan8, flat_pyramid(plan8, [adversarial_pyramid(s) for s in range(8)]))}.items():
-    det = Detector(L, p, b)
-    for nf, cap in ((1, 1), (40, 40), (0, 4096)):
-        res["%s_%d" % (name, nf)] = det.checked_select(nf, cap)
-torch.save(res, sys.argv[1])
-"""
-
-
-def _run_variant(tmp_path, name, env_extra):
-    out = str(tmp_path / (name + ".pt"))
-    env = dict(os.environ)
-    for k in ("AG_BLUR_NO_TMA", "AG_DETECT_WARP_V1", "AG_DETECT_TILED", "AG_PYR_FUSED"):
-        env.pop(k, None)
-    env.update(env_extra)
-    r = subprocess.run([sys.executable, "-c", _SCRIPT, out, ROOT], env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-2000:]
-    return torch.load(out)
-
-
-def test_detector_variants_agree_with_the_default(L, tmp_path):
-    """The first register formulation (AG_DETECT_WARP_V1) gives the default's bits on the odd-shape and the level-drop batches.  The
-    shared-memory tiled detector (AG_DETECT_TILED) makes the same decisions and responses bit for bit, but sums the 27 soft-argmax taps
-    one by one where the register kernels add per-row sums: its LAFs must be the taps-order restatement's bits
-    (tests/detect_restated.py), the default's the rows-order one's."""
-    base = _run_variant(tmp_path, "default", {})
-    assert int(base["odd_0"][4].max()) > 20 and int(base["adv_0"][4].max()) > 0
-    v1 = _run_variant(tmp_path, "v1", {"AG_DETECT_WARP_V1": "1"})
-    tiled = _run_variant(tmp_path, "tiled", {"AG_DETECT_TILED": "1"})
-    plan, _, pyrs = gpu_pyramids(L, mixed_batch(97, 131, 5), 3)
-    cands = {"odd": [OracleCandidates(p, plan_sigmas(plan), MR) for p in pyrs],
-             "adv": [OracleCandidates(adversarial_pyramid(s), plan_sigmas(L.make_plan(1, 40, 40, 3, 1.6, 5)), MR) for s in range(8)]}
-    R = {(name, order): restate(cs, order) for name, cs in cands.items() for order in ("rows", "taps")}
-    differ = 0
-    for key in base:
-        name, nf = key.split("_")
-        for i, (x, y, z) in enumerate(zip(base[key], v1[key], tiled[key])):
-            assert torch.equal(x, y), ("AG_DETECT_WARP_V1", key, i)
-            if i != 1:
-                assert torch.equal(x, z), ("AG_DETECT_TILED", key, i)
-        for b, c in enumerate(cands[name]):
-            cap = base[key][0].size(1)
-            assert_image(base[key], b, cut(expected(c, R[(name, "rows")][b], int(nf)), cap), ("default", key))
-            assert_image(tiled[key], b, cut(expected(c, R[(name, "taps")][b], int(nf)), cap), ("AG_DETECT_TILED", key))
-        differ += int((bits(base[key][1]) != bits(tiled[key][1])).any(-1).any(-1).sum())
-    print("\ndetector variants: AG_DETECT_WARP_V1 bit-identical; AG_DETECT_TILED equal to the taps-order restatement, its LAFs differ "
-          "from the default's on %d rows" % differ)
-    assert differ > 0

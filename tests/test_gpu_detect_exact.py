@@ -1,17 +1,13 @@
 """GPU tests (-m gpu): every keypoint LAF the detector writes, bit for bit against the soft-argmax restatement
 (tests/detect_restated.py) in the order of the kernel that produced it, and within the float64 bound.
 
-The register kernels (detect_rows_kernel, the default at nlevels = 3, and detect_warp_kernel under AG_DETECT_WARP_V1) sum the
-window by rows; detect_level_kernel (other level counts, and the response-map entry point) and detect_fused_kernel
-(AG_DETECT_TILED) tap by tap.  The two orders differ in the last bits on most candidates, so only a bit-exact comparison tells
+The register kernel (detect_rows_kernel, at nlevels = 3) sums the window by rows; detect_level_kernel (other level counts, and
+the response-map entry point) tap by tap.  The two orders differ in the last bits on most candidates, so only a bit-exact comparison tells
 which ran.  Counts, responses, octave and level indices are the oracle's (tests/helpers.py::OracleCandidates) as in
 test_gpu_detect.py, and rows beyond the count keep their sentinel.  The cases put candidates on the strip and band seams, on the
 image edges at border 0 and 1, and at low contrast (pyramids scaled by 2^-k), where every positive pixel is a candidate, den is
 dominated by its 1e-8 and the responses are fp32 subnormals."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -26,7 +22,6 @@ from helpers import (SENTINEL, Detector, OracleCandidates, adversarial_pyramid, 
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda"
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 MR = 5.192
 ISENT = int(SENTINEL)
 WORST = {}
@@ -226,52 +221,3 @@ def test_low_contrast(L, low_base, k):
                 if b != big:
                     for x, y in zip(out, ref):
                         assert torch.equal(x[b], y[b]), (k, b)
-
-
-# ---- variants -----------------------------------------------------------------------------------------------------------------------
-_SCRIPT = r"""
-import sys, torch
-sys.path.insert(0, sys.argv[2]); sys.path.insert(0, sys.argv[2] + "/tests"); sys.path.insert(0, sys.argv[2] + "/oracle")
-import affnet_b200._lib as L
-import detect_cases as DC
-from helpers import Detector, adversarial_pyramid, flat_pyramid, gpu_pyramids, mixed_batch
-res = {}
-plan, buf, _ = gpu_pyramids(L, mixed_batch(97, 131, 5), 3)
-plan8 = L.make_plan(8, 40, 40, 3, 1.6, 5)
-planS = L.make_plan(1, *DC.SEAM_SHAPE, 3, 1.6, 5)
-low = DC.low_contrast_case()[2]
-planL = L.make_plan(1, 160, 200, 3, 1.6, 5)
-cases = {"odd": (plan, buf, 5.192), "adv": (plan8, flat_pyramid(plan8, [adversarial_pyramid(s) for s in range(8)]), 5.192),
-         "seam": (planS, flat_pyramid(planS, [DC.seam_case()[2]]), 0.0), "low66": (planL, flat_pyramid(planL, [DC.scaled(low, 66)]), 5.192)}
-for name, (p, b, mr) in cases.items():
-    det = Detector(L, p, b, mr=mr, cap=3 * sum(p.h[o] * p.w[o] for o in range(p.n_octaves)))
-    res[name] = det.checked_select(2000, None, 5.192)
-torch.save(res, sys.argv[1])
-"""
-
-
-def test_variants_match_their_order_exactly(L, tmp_path):
-    """AG_DETECT_TILED (detect_fused_kernel) equals the taps restatement and AG_DETECT_WARP_V1 (detect_warp_kernel) the rows
-    restatement, bit for bit, at a_scale 5.192, on odd shapes, level-drop pyramids, the seam pyramid at border 0 and the k = 66
-    low-contrast pyramid."""
-    plan, _, pyrs_odd = gpu_pyramids(L, mixed_batch(97, 131, 5), 3)
-    sig = plan_sigmas(plan)
-    cands = {"odd": [OracleCandidates(p, sig, MR) for p in pyrs_odd],
-             "adv": [OracleCandidates(adversarial_pyramid(s), plan_sigmas(L.make_plan(1, 40, 40, 3, 1.6, 5)), MR) for s in range(8)],
-             "seam": [OracleCandidates(DC.seam_case()[2], DC.seam_case()[1], 0.0)],
-             "low66": [OracleCandidates(DC.scaled(DC.low_contrast_case()[2], 66), DC.low_contrast_case()[1], MR)]}
-    for name, env, order in (("v1", {"AG_DETECT_WARP_V1": "1"}, "rows"), ("tiled", {"AG_DETECT_TILED": "1"}, "taps")):
-        out = str(tmp_path / (name + ".pt"))
-        e = dict(os.environ)
-        for k in ("AG_BLUR_NO_TMA", "AG_DETECT_WARP_V1", "AG_DETECT_TILED", "AG_PYR_FUSED"):
-            e.pop(k, None)
-        e.update(env)
-        r = subprocess.run([sys.executable, "-c", _SCRIPT, out, ROOT], env=e, capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, r.stderr[-2000:]
-        res = torch.load(out)
-        rows = 0
-        for key, cs in cands.items():
-            Rs = restated(cs, order, 5.192)
-            rows += sum(assert_exact(res[key], b, c, R, 2000, (name, key)) for b, (c, R) in enumerate(zip(cs, Rs)))
-        print("\n%s: %d LAF rows bit-exact to the %s restatement" % (name, rows, order))
-    print("worst error / bound by case: %s" % {k: round(v, 3) for k, v in WORST.items()})

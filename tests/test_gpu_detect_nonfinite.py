@@ -5,7 +5,7 @@ unmodified reference by tests/test_detect_nonfinite_cpu.py) under its one deviat
   and at B = 3 with a NaN tile on a 32-pixel tile seam.
 - ag_detect_level_from_responses on the golden NMS cases (a NaN beside a maximum, an inf centre, NaN survivors on a nonzero octave
   map, a level dropped by a NaN).
-- The detector (default rows kernel, AG_DETECT_WARP_V1, AG_DETECT_TILED; detect_level_kernel at other level counts) with NaN and
+- The detector (the rows kernel at nlevels = 3, detect_level_kernel at other level counts) with NaN and
   +-inf in the image and in single pyramid levels on the 30-column strip seams, the 48-row band seams and the edges, at border 0 and
   5, for nlevels 1, 3 and 6; on images scaled by 2^k across the Hessian's overflow; a batch of 16 holding one NaN image.  Per image:
   the count, responses, octave and level identical to the oracle, LAFs bit for bit the restatement of the kernel's order (NaN
@@ -13,9 +13,6 @@ unmodified reference by tests/test_detect_nonfinite_cpu.py) under its one deviat
 - Selection through ag_select_keypoints, ag_select_topk_keypoints above 16384 keys and ag_select_all_keypoints at th = 28.41.
 - DetectDescribePipeline (AffNet + OriNet, Baumberg + histogram) on a batch holding a NaN image, against the single-image API."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -29,7 +26,6 @@ from helpers import (SENTINEL, Detector, OracleCandidates, flat_pyramid, gold, g
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda"
-ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 MR = 5.192
 ISENT = int(SENTINEL)
 Z = gold("nonfinite.npz")
@@ -250,55 +246,6 @@ def test_select_topk_above_16384_and_threshold_keep_all(L):
     out = det_t.select_all(max(c.total for c in ct))
     rows_t = sum(assert_image(out, b, c, R, 0, "th 28.41 all") for b, (c, R) in enumerate(zip(ct, Rt)))
     print("\n1080x1920 with %d NaN / inf pixels: top-20000 %d rows, th 28.41 keep-all %d rows" % (len(spots), rows, rows_t))
-
-
-# ---- A/B kernel variants -----------------------------------------------------------------------------------------------------------
-_SCRIPT = r"""
-import sys, torch
-sys.path.insert(0, sys.argv[2]); sys.path.insert(0, sys.argv[2] + "/tests"); sys.path.insert(0, sys.argv[2] + "/oracle")
-import affnet_b200._lib as L
-from helpers import Detector, flat_pyramid, gpu_pyramids
-import test_gpu_detect_nonfinite as T
-res = {}
-plan, buf, pyrs = gpu_pyramids(L, T.seam_batch(), 3)
-for name, b in {"image": buf, "levels": flat_pyramid(plan, T.level_pokes(pyrs, 5))}.items():
-    for mr in (5, 0):
-        det = Detector(L, plan, b, mr=mr)
-        for nf, cap in ((1, 1), (40, 40), (0, 4096)):
-            res["%s_%d_%d" % (name, mr, nf)] = det.checked_select(nf, cap) if nf else det.select_all(cap)
-torch.save(res, sys.argv[1])
-"""
-
-
-def _run_variant(tmp_path, name, env_extra):
-    out = str(tmp_path / (name + ".pt"))
-    env = dict(os.environ)
-    for k in ("AG_BLUR_NO_TMA", "AG_DETECT_WARP_V1", "AG_DETECT_TILED", "AG_PYR_FUSED"):
-        env.pop(k, None)
-    env.update(env_extra)
-    r = subprocess.run([sys.executable, "-c", _SCRIPT, out, ROOT], env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-2000:]
-    return torch.load(out)
-
-
-def test_detector_variants_on_nonfinite_values(L, tmp_path):
-    """AG_DETECT_WARP_V1 gives the default's bits; AG_DETECT_TILED the oracle's decisions and the taps-order restatement's LAFs."""
-    base = _run_variant(tmp_path, "default", {})
-    v1 = _run_variant(tmp_path, "v1", {"AG_DETECT_WARP_V1": "1"})
-    tiled = _run_variant(tmp_path, "tiled", {"AG_DETECT_TILED": "1"})
-    plan, _, pyrs = gpu_pyramids(L, seam_batch(), 3)
-    src = {"image": pyrs, "levels": level_pokes(pyrs, 5)}
-    rows = 0
-    for key in base:
-        name, mr, nf = key.split("_")
-        for x, y in zip(base[key], v1[key]):
-            assert torch.equal(bits(x) if x.is_floating_point() else x, bits(y) if y.is_floating_point() else y), ("AG_DETECT_WARP_V1", key)
-        cands = [OracleCandidates(p, plan_sigmas(plan), float(mr)) for p in src[name]]
-        for order, out in (("rows", base[key]), ("taps", tiled[key])):
-            for b, c in enumerate(cands):
-                R = Restated(c.pyr, c.sigmas, c.seq, order)
-                rows += assert_image(out, b, c, R, int(nf), (order, key), out_cap=out[0].size(1))
-    print("\ndetector variants on non-finite values: %d rows identical to the oracle and restatement" % rows)
 
 
 # ---- the batched pipeline --------------------------------------------------------------------------------------------------------

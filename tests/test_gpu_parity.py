@@ -85,38 +85,6 @@ def test_gaussian_blur_and_pyramid_vs_oracle(L):
     assert torch.equal(p2[2][3][0], pyr[2][3][0])
 
 
-@pytest.mark.parametrize("shape", [(1, 768, 1024), (3, 480, 640), (2, 200, 328), (1, 97, 132), (2, 1080, 1920)])
-def test_fused_octave_pyramid_is_bit_identical_to_the_per_level_blurs(L, shape):
-    """The one-launch-per-octave pyramid (pyramid_fused.cuh: rows streamed through shared memory, bulk-copied input rows, column strips and
-    row bands with halos; selectable, not the default because it measured slower): every level must equal the chain of single-level
-    blurs (same fmaf order) bit for bit, including the replicate borders, the strip / band seams and the stride-2 seeds of the next octaves."""
-    from affnet_b200.Utils import GaussianBlur
-    from affnet_b200.HandCraftedModules import ScalePyramid
-    B, H, Wd = shape
-    g = torch.Generator().manual_seed(H + Wd)
-    x = (torch.rand(B, 1, H, Wd, generator=g) * 255).to(DEV)
-    sp = ScalePyramid(3, 1.6, 5)
-    old = L.lib().ag_debug_pyramid_mode(1)
-    try:
-        plan, buf = sp.build(x)
-    finally:
-        L.lib().ag_debug_pyramid_mode(old)
-    pyr, sig, pix = ScalePyramid.views(plan, buf)
-    cur = None
-    for o in range(plan.n_octaves):
-        for l in range(plan.n_levels):
-            bs = plan.blur_sigma[o][l]
-            if o == 0 and l == 0:
-                cur = GaussianBlur(bs)(x)
-            elif l == 0:
-                cur = seed[:, :, ::2, ::2].contiguous()
-            else:
-                cur = GaussianBlur(bs)(cur)
-            if l == plan.n_levels - 2:
-                seed = cur
-            assert torch.equal(pyr[o][l], cur), (shape, o, l, (pyr[o][l] - cur).abs().max().item())
-
-
 def test_hessian_bit_exact(L):
     from affnet_b200.HandCraftedModules import HessianResp
     g = torch.Generator().manual_seed(4)

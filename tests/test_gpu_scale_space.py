@@ -203,22 +203,6 @@ def test_pyramid_batch_equals_single_images(L):
                 assert bits_equal(level(plan, buf, o, l)[b], level(p1, b1, o, l)[0]), (b, o, l)
 
 
-@pytest.mark.parametrize("case", K.FUSED_CASES, ids=lambda c: "%s-B%d-%dx%d" % c[:4])
-def test_fused_octave_pyramid_bit_exact(L, case):
-    _, B, H, W, nl, s, border = case
-    plan = L.make_plan(B, H, W, nl, s, border)
-    x = case_input(case)
-    old = L.lib().ag_debug_pyramid_mode(1)
-    try:
-        names = [n for n, _ in L.profile(lambda: L.check(build(L, plan, x)[0]))]
-        rc, buf = build(L, plan, x)
-    finally:
-        L.lib().ag_debug_pyramid_mode(old)
-    L.check(rc)
-    assert "octave_kernel" in names, names
-    check_pyramid(plan, buf, x, ("fused",) + case)
-
-
 _NO_TMA = r"""
 import ctypes as C, sys, torch
 for p in ("", "/oracle", "/tests"):
@@ -246,8 +230,6 @@ def test_pyramid_without_tensor_maps_bit_exact(L, tmp_path):
     """AG_BLUR_NO_TMA=1 (a driver without the tensor-map encoder): interior tiles take per-row bulk copies."""
     path = str(tmp_path / "no_tma.pt")
     env = dict(os.environ)
-    for k in ("AG_BLUR_NO_TMA", "AG_PYR_FUSED"):
-        env.pop(k, None)
     env["AG_BLUR_NO_TMA"] = "1"
     r = subprocess.run([sys.executable, "-c", _NO_TMA, path, ROOT], env=env, capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-2000:]
