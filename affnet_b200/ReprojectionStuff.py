@@ -1,6 +1,6 @@
 """ReprojectionStuff.py counterpart for verifying matches on the device: the reference's ground-truth check
 (get_GT_correspondence_indexes, ReprojectionStuff.py:126-137), homography RANSAC (the notebook's ransac_validate) and
-fundamental-matrix RANSAC (its findFundamentalMatrix alternative), for one pair or for every pair of a batch in one call.  The batched calls take DetectDescribePipeline.run's LAFs and
+fundamental-matrix RANSAC (its findFundamentalMatrix alternative, also as DEGENSAC), for one pair or for every pair of a batch in one call.  The batched calls take DetectDescribePipeline.run's LAFs and
 Losses.match_snn_pairs' (tent, ntent) as they are, never synchronise with the host, and are capturable in the same CUDA graph."""
 import torch
 
@@ -76,14 +76,18 @@ def find_homography_pairs(lafs1, tent, ntent, lafs2=None, pairs=None, inl_th=2.0
     return H, inl, ninl, iters
 
 
-def find_fundamental_pairs(lafs1, tent, ntent, lafs2=None, pairs=None, inl_th=0.5, confidence=0.99, max_iters=50000, seed=0):
+def find_fundamental_pairs(lafs1, tent, ntent, lafs2=None, pairs=None, inl_th=0.5, confidence=0.99, max_iters=50000, seed=0,
+                           degensac=False):
     """Fundamental-matrix RANSAC for every pair, in one launch (ag_fundamental_ransac), with the inputs of find_homography_pairs.  For
     scenes with depth, where one homography explains one plane only.  A tentative is an inlier when its Sampson distance to F is at most
     inl_th px.  inl_th = 0.5 is the notebook's alternative findFundamentalMatrix(src, dst, 0.5); confidence and max_iters are those of
     its findHomography call.  Deterministic for a seed, and a pair's result does not depend on the other pairs.
     -> (F [P,3,3] float32 with unit Frobenius norm and its largest-magnitude entry positive, inl [P,tcap] uint8, ninl [P] int32, iters [P]
     int32 7-point samples evaluated).  ninl[p] is -1 for a pair that cannot be verified (ntent -1, an index out of range); 0 with F = 0
-    when it has fewer than 7 tentatives or no usable sample.  Rows at or beyond ntent[p] are unspecified."""
+    when it has fewer than 7 tentatives or no usable sample.  Rows at or beyond ntent[p] are unspecified.
+    degensac=True (ag_fundamental_degensac) adds DEGENSAC's degeneracy test, plane-and-parallax and local optimisation, for scenes where
+    one plane (a facade, a floor) carries most matches: pydegensac.findFundamentalMatrix's algorithm family, with the same inputs and
+    outputs."""
     fn = "find_fundamental_pairs"
     if not float(inl_th) > 0.0 or float(inl_th) == float("inf"):
         raise L.AffnetB200Error("%s: inl_th must be finite and > 0" % fn)
@@ -99,9 +103,10 @@ def find_fundamental_pairs(lafs1, tent, ntent, lafs2=None, pairs=None, inl_th=0.
     iters = torch.empty(P, dtype=torch.int32, device=dev)
     if P == 0:
         return F, inl, ninl, iters
-    L.check(L.lib().ag_fundamental_ransac(L.ptr(a), a.size(0), a.size(1), L.ptr(b), b.size(0), b.size(1), L.ptr(pairs), P, L.ptr(tent),
-                                          L.ptr(ntent), tcap, float(inl_th), float(confidence), int(max_iters), int(seed) & (2 ** 64 - 1),
-                                          L.ptr(F), L.ptr(inl), L.ptr(ninl), L.ptr(iters), L.stream_ptr()))
+    entry = L.lib().ag_fundamental_degensac if degensac else L.lib().ag_fundamental_ransac
+    L.check(entry(L.ptr(a), a.size(0), a.size(1), L.ptr(b), b.size(0), b.size(1), L.ptr(pairs), P, L.ptr(tent), L.ptr(ntent), tcap,
+                  float(inl_th), float(confidence), int(max_iters), int(seed) & (2 ** 64 - 1), L.ptr(F), L.ptr(inl), L.ptr(ninl),
+                  L.ptr(iters), L.stream_ptr()))
     return F, inl, ninl, iters
 
 

@@ -128,6 +128,7 @@ PROTOTYPES = {
     "ag_match_pairs": (i32, [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, i32, f32, vp, sz, vp, vp, vp, vp, vp, vp, vp]),
     "ag_homography_ransac": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp, vp]),
     "ag_fundamental_ransac": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp, vp]),
+    "ag_fundamental_degensac": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp, vp]),
     "ag_gt_correspondences_pairs": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, vp, f32, vp, vp, vp, vp, vp]),
     "ag_pipeline_create": (i32, [C.POINTER(PipelineConfig), vp, vp, vp, C.POINTER(vp)]),
     "ag_pipeline_create_ex": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), vp, vp, vp, C.POINTER(vp)]),

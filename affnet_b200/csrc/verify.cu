@@ -1,9 +1,11 @@
 // Geometric verification of the batched matcher's tentatives (after ag_match_pairs), one CTA per pair:
 //   ag_homography_ransac         homography RANSAC (the notebook's ransac_validate: findHomography(src, dst, 2.0, 0.99, 50000))
 //   ag_fundamental_ransac        fundamental-matrix RANSAC (the notebook's commented-out findFundamentalMatrix(src, dst, 0.5))
+//   ag_fundamental_degensac      the same with DEGENSAC's degeneracy test, plane-and-parallax and local optimisation (pydegensac's family)
 //   ag_gt_correspondences_pairs  ReprojectionStuff.get_GT_correspondence_indexes (the reference's "true matches" count), per pair
 //
-// Both RANSACs are deterministic and restated line by line in numpy by tests/oracle_ransac.py and tests/oracle_fransac.py, so their
+// The RANSACs are deterministic and restated line by line in numpy by tests/oracle_ransac.py, tests/oracle_fransac.py and
+// tests/oracle_degensac.py, so their
 // decisions (samples, degeneracy, inlier counts, the stopping point) are reproduced exactly.  For that reason all their arithmetic is
 // fp64, with + - * / sqrt only where a decision depends on it, and this file is compiled with
 // -fmad=false (build.sh): numpy rounds every product and sum separately, so fused multiply-adds here would move near-threshold decisions.
@@ -780,8 +782,199 @@ __device__ bool refit_f(const float* L1, const float* L2, const int* tent, int n
     return !s.bad;
 }
 
+// Up to REFIT_ROUNDS least-squares refits of the model M (shared; a homography, or a fundamental matrix when FUND) on its inliers at
+// th2, each kept only if the inlier count does not drop: the rounds that end both kernels, for DEGENSAC's plane H and its local
+// optimisation.  Block-wide; on return M is the last kept model and `inl` its mask (rows < n).
+// Returns its inlier count.
+template <bool FUND>
+__device__ __forceinline__ int refit_rounds(const float* L1, const float* L2, const int* tent, int n, double th2, unsigned char* inl,
+                                            double* M, RansacShared& s) {
+    int cnt = score_rows<FUND>(M, L1, L2, tent, n, th2, inl, s);
+    for (int r = 0; r < REFIT_ROUNDS && cnt >= (FUND ? F_REFIT_MIN : 4); r++) {
+        if (!(FUND ? refit_f(L1, L2, tent, n, inl, cnt, s) : refit(L1, L2, tent, n, inl, cnt, s))) break;
+        const int c2 = score_rows<FUND>(s.Hr, L1, L2, tent, n, th2, nullptr, s);
+        if (c2 < cnt) break;
+        cnt = c2;
+        if (threadIdx.x < 9) M[threadIdx.x] = s.Hr[threadIdx.x];
+        __syncthreads();
+        score_rows<FUND>(M, L1, L2, tent, n, th2, inl, s);
+    }
+    return cnt;
+}
+
 __device__ __forceinline__ bool finite4(float4 c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z) && isfinite(c.w); }
 
+// ---- DEGENSAC (Chum, Werner and Matas, CVPR 2005): degeneracy test, plane-and-parallax, local optimisation ------------------------
+constexpr double DEG_H_TH_FACTOR = 4.0;   // DEG_H_TH = DEG_H_TH_FACTOR * inl_th: a point agrees with a plane H within it (transfer, px)
+constexpr int DEG_MIN_AGREE = 5;          // a 7-point sample is H-degenerate when some triplet's H agrees with this many of its points
+constexpr uint64_t DEG_SEED_TAG = 0xD5A61266F0C9392Cull;   // the plane-and-parallax sampler's stream: seed ^ DEG_SEED_TAG
+constexpr uint32_t DEG_H_BASE = 0x80000000u;   // its hypotheses: DEG_H_BASE + k VT + thread (k: degeneracy tests so far), above any h
+__constant__ int deg_triplets[5][3] = {{0, 1, 2}, {3, 4, 5}, {0, 1, 6}, {3, 4, 6}, {2, 5, 6}};
+
+// (a x b) into o.
+__device__ __forceinline__ void cross_v(const double* a, const double* b, double* o) {
+    o[0] = a[1] * b[2] - a[2] * b[1];
+    o[1] = a[2] * b[0] - a[0] * b[2];
+    o[2] = a[0] * b[1] - a[1] * b[0];
+}
+// O = [e]x M: column c of O is e x (column c of M).
+__device__ __forceinline__ void skew_mul(const double* e, const double* M, double* O) {
+    for (int c = 0; c < 3; c++) {
+        const double m[3] = {M[c], M[3 + c], M[6 + c]};
+        double o[3];
+        cross_v(e, m, o);
+        O[c] = o[0]; O[3 + c] = o[1]; O[6 + c] = o[2];
+    }
+}
+
+// The homography of the plane through the three correspondences c[0..2] compatible with F (Hartley and Zisserman, result 13.6):
+// H = A - e' (M^-1 b)', A = [e']x F, M the image-1 points as rows, b_m = (x'_m x A x_m).(x'_m x e') / |x'_m x e'|^2, normalised by
+// normalise_h.  False when M is singular or H / H[2][2] is not finite.
+__device__ bool triplet_homography(const double* A, const double* e, const float4* c, double* H) {
+    double b[3], M[9];
+    for (int m = 0; m < 3; m++) {
+        const double x = c[m].x, y = c[m].y;
+        const double ax[3] = {A[0] * x + A[1] * y + A[2], A[3] * x + A[4] * y + A[5], A[6] * x + A[7] * y + A[8]};
+        const double xp[3] = {(double)c[m].z, (double)c[m].w, 1.0};
+        double pp[3], q[3];
+        cross_v(xp, ax, pp);
+        cross_v(xp, e, q);
+        b[m] = (pp[0] * q[0] + pp[1] * q[1] + pp[2] * q[2]) / (q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+        M[3 * m] = x; M[3 * m + 1] = y; M[3 * m + 2] = 1.0;
+    }
+    double Ad[9];
+    adj3(M, Ad);
+    const double det = M[0] * Ad[0] + M[1] * Ad[3] + M[2] * Ad[6];
+    if (det == 0.0) return false;
+    double v[3];
+    for (int k = 0; k < 9; k++) Ad[k] = Ad[k] / det;
+    for (int r = 0; r < 3; r++) v[r] = Ad[3 * r] * b[0] + Ad[3 * r + 1] * b[1] + Ad[3 * r + 2] * b[2];
+    for (int r = 0; r < 3; r++)
+        for (int k = 0; k < 3; k++) H[3 * r + k] = A[3 * r + k] - e[r] * v[k];
+    return normalise_h(H);
+}
+
+// Degeneracy test of the 7-point sample c with its model F: e' the left epipole (F' e' = 0, the smallest eigenvector of F F' by jacobi3),
+// and for each of the five triplets of Chum et al. the H of triplet_homography.  Returns the most sample points that one H agrees with
+// (is_inlier at thd2), that H (the lowest triplet on ties) in Hd.  One thread.
+__device__ int degeneracy_test(const double* F, const float4 (&c)[F_SAMPLE], double thd2, double* Hd) {
+    double G[9], V[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+    for (int r = 0; r < 3; r++)
+        for (int k = 0; k < 3; k++) G[3 * r + k] = F[3 * r] * F[3 * k] + F[3 * r + 1] * F[3 * k + 1] + F[3 * r + 2] * F[3 * k + 2];
+    jacobi3(G, V);
+    const int m = smallest_diag<3>(G);
+    const double e[3] = {V[m], V[3 + m], V[6 + m]};
+    double A[9];
+    skew_mul(e, F, A);
+    int best = 0;
+    for (int t = 0; t < 5; t++) {
+        const float4 ct[3] = {c[deg_triplets[t][0]], c[deg_triplets[t][1]], c[deg_triplets[t][2]]};
+        double H[9];
+        if (!triplet_homography(A, e, ct, H)) continue;
+        int k = 0;
+        for (int q = 0; q < F_SAMPLE; q++) k += is_inlier(H, c[q], thd2);
+        if (k > best) {
+            best = k;
+            for (int i = 0; i < 9; i++) Hd[i] = H[i];
+        }
+    }
+    return best;
+}
+
+// Shared state of the DEGENSAC steps (apart from RansacShared).
+struct DegenShared {
+    double Hd[9];
+    unsigned long long key[VT / 32];
+    int agree;
+};
+
+// The DEGENSAC steps after a chunk's winner (sample h, model s.H, `best` inliers) has raised the so-far-best count: the degeneracy test
+// of its sample; for an H-degenerate sample, H refitted on its inliers at DEG_H_TH (the homography RANSAC's rounds) and
+// plane-and-parallax, thread t drawing two rows that are not inliers of H from hypothesis DEG_H_BASE + k VT + t of the stream
+// seed ^ DEG_SEED_TAG, F = [e']x H with e' = (H x_a x x'_a) x (H x_b x x'_b), the best (most inliers, then lowest thread) replacing
+// s.H when it has more inliers; then the refit rounds on s.H.  `inl` is scratch.  Block-wide; returns the new so-far-best count.
+__device__ __noinline__ int degensac_step(const float* L1, const float* L2, const int* tent, int n, int ntiles, double th2, uint64_t seed,
+                                          int h, int k, unsigned char* inl, int best, RansacShared& s) {
+    __shared__ DegenShared d;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const double thd2 = (DEG_H_TH_FACTOR * DEG_H_TH_FACTOR) * th2;
+    if (tid == 0) {
+        int idx[F_SAMPLE], got = 0;
+        for (int dr = 0; dr < MAX_DRAWS && got < F_SAMPLE; dr++) {
+            const int v = draw_index(seed, h, dr, n);
+            bool dup = false;
+            for (int q = 0; q < got; q++) dup |= idx[q] == v;
+            if (!dup) idx[got++] = v;
+        }
+        float4 c[F_SAMPLE];
+        for (int q = 0; q < F_SAMPLE; q++) c[q] = tent_centres(L1, L2, tent, idx[q]);
+        d.agree = degeneracy_test(s.H, c, thd2, d.Hd);
+    }
+    __syncthreads();
+    if (d.agree >= DEG_MIN_AGREE) {
+        refit_rounds<false>(L1, L2, tent, n, thd2, inl, d.Hd, s);   // inl: the inliers of d.Hd
+        double F[9];
+        bool ok;
+        {
+            const uint32_t hh = DEG_H_BASE + (uint32_t)k * VT + (uint32_t)tid;
+            int idx[2], got = 0;
+            for (int dr = 0; dr < MAX_DRAWS && got < 2; dr++) {
+                const int v = draw_index(seed ^ DEG_SEED_TAG, (int)hh, dr, n);
+                if (!inl[v] && (got == 0 || v != idx[0])) idx[got++] = v;
+            }
+            ok = got == 2;
+            if (ok) {
+                double l[2][3];
+                for (int q = 0; q < 2; q++) {
+                    const float4 c = tent_centres(L1, L2, tent, idx[q]);
+                    const double x = c.x, y = c.y;
+                    const double hx[3] = {d.Hd[0] * x + d.Hd[1] * y + d.Hd[2], d.Hd[3] * x + d.Hd[4] * y + d.Hd[5],
+                                          d.Hd[6] * x + d.Hd[7] * y + d.Hd[8]};
+                    const double xp[3] = {(double)c.z, (double)c.w, 1.0};
+                    cross_v(hx, xp, l[q]);
+                }
+                double e[3];
+                cross_v(l[0], l[1], e);
+                skew_mul(e, d.Hd, F);
+                ok = normalise_f(F);
+            }
+        }
+        int cnt = 0;
+        for (int tb = 0; tb < ntiles; tb++) {
+            const int t0 = tb * VTILE, m = min(VTILE, n - t0);
+            if (ntiles > 1) {   // one tile stays loaded from the first chunk
+                __syncthreads();
+                for (int t = tid; t < m; t += VT) s.tile[t] = tent_centres(L1, L2, tent, t0 + t);
+                __syncthreads();
+            }
+            if (ok)
+                for (int t = 0; t < m; t++) cnt += is_inlier_f(F, s.tile[t], th2);
+        }
+        const unsigned long long mine = ok ? ((unsigned long long)cnt << 32) | (unsigned)~(unsigned)tid : 0ull;
+        unsigned long long key = mine;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
+            key = k2 > key ? k2 : key;
+        }
+        if (lane == 0) d.key[warp] = key;
+        __syncthreads();
+        unsigned long long bk = 0;
+#pragma unroll
+        for (int w = 0; w < VT / 32; w++) bk = d.key[w] > bk ? d.key[w] : bk;
+        const int bc = (int)(bk >> 32);
+        if (bk != 0 && bc > best) {
+            if (mine == bk)
+                for (int q = 0; q < 9; q++) s.H[q] = F[q];
+            best = bc;
+        }
+        __syncthreads();
+    }
+    return refit_rounds<true>(L1, L2, tent, n, th2, inl, s.H, s);
+}
+
+// DEGEN: ag_fundamental_degensac (degensac_step whenever a chunk's winner raises the so-far-best count); otherwise ag_fundamental_ransac.
+template <bool DEGEN>
 __global__ void __launch_bounds__(VT) fransac_kernel(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2, int S2,
                                                      int cap2, const int* __restrict__ pairs, const int* __restrict__ tent_all,
                                                      const int* __restrict__ ntent, int tcap, double th2, double log1mconf, int max_iters,
@@ -822,6 +1015,7 @@ __global__ void __launch_bounds__(VT) fransac_kernel(const float* __restrict__ l
         // fewer than 7 finite rows, or all of them on one point in an image: no hypothesis is drawn (iters = 0)
         const bool search = nd >= (double)F_SAMPLE && var1 > 0.0 && var2 > 0.0;
         const int ntiles = (n + VTILE - 1) / VTILE;
+        int ntests = 0;   // DEGEN: degeneracy tests so far
         for (int h0 = 0; search; h0 += VT) {
             const int h = h0 + tid;
             double Fm[3][9];
@@ -895,6 +1089,11 @@ __global__ void __launch_bounds__(VT) fransac_kernel(const float* __restrict__ l
                             for (int k = 0; k < 9; k++) s.H[k] = Fm[r][k];
                 }
                 best = bc;
+                if constexpr (DEGEN) {
+                    __syncthreads();
+                    best = degensac_step(L1, L2, tent, n, ntiles, th2, seed, 0x7fffffff - (int)((bk >> 2) & 0xffffffffull), ntests++, inl,
+                                         best, s);
+                }
             }
             h_done = min(h0 + VT, max_iters);
             double need;   // adaptive number of samples for `confidence`
@@ -972,9 +1171,27 @@ int ag_fundamental_ransac(const float* d_lafs1, int S1, int cap1, const float* d
     AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
     AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
     const double th = inl_th;
-    fransac_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
-                                                       log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_F, d_inl, d_ninl, d_iters);
+    fransac_kernel<false><<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
+                                                              log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_F, d_inl, d_ninl,
+                                                              d_iters);
     AG_CHECK_LAUNCH("fransac_kernel");
+    return AG_OK;
+}
+
+int ag_fundamental_degensac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                            const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
+                            float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
+    int rc = verify_args("ag_fundamental_degensac", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc) return rc;
+    AG_REQUIRE(d_F && d_inl && d_ninl, "NULL output");
+    AG_REQUIRE(inl_th > 0.f && isfinite(inl_th), "inl_th must be finite and > 0");
+    AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
+    AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
+    const double th = inl_th;
+    fransac_kernel<true><<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
+                                                             log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_F, d_inl, d_ninl,
+                                                             d_iters);
+    AG_CHECK_LAUNCH("fransac_kernel<DEGEN>");
     return AG_OK;
 }
 

@@ -408,6 +408,24 @@ int ag_match_pairs(const float* d_desc1, const int* d_count1, int S1, int cap1, 
  *   F; d_ninl [P], d_iters [P] (samples evaluated; may be NULL).  n < 7 tentatives, fewer than 7 finite ones, all of them on one point
  *   of an image (iters = 0), or no model with an inlier: ninl = 0, F = 0, mask rows < n = 0.
  *   AG_ERR_INVALID also for inl_th not finite and > 0, confidence outside (0, 1), max_iters < 1.
+ * ag_fundamental_degensac: ag_fundamental_ransac with DEGENSAC's steps (Chum, Werner and Matas, CVPR 2005; pydegensac's algorithm
+ * family, not its bits), for scenes where one plane carries most matches and a 7-point sample from it yields a wrong F that explains
+ * the plane.  The arguments, refusals, -1 rule, outputs, determinism and pair independence of ag_fundamental_ransac.  Whenever a
+ * chunk's winner raises the so-far-best count, before the stopping rule:
+ *   1. degeneracy test of its sample (re-drawn from (seed, h)): e' the left epipole (F' e' = 0, the smallest eigenvector of F F' by a
+ *      3x3 Jacobi), A = [e']x F, and for the triplets {0,1,2}, {3,4,5}, {0,1,6}, {3,4,6}, {2,5,6} the plane homography
+ *      H = A - e' (M^-1 b)' (M the triplet's image-1 points as rows, b_m = (x'_m x A x_m).(x'_m x e') / |x'_m x e'|^2, a singular M
+ *      skipped), normalised to H[2][2] = 1.  A sample point agrees with H when it is a homography inlier of H at
+ *      DEG_H_TH = 4 inl_th.  The sample is H-degenerate when one H agrees with >= 5 of its 7 points (the H with most, the lowest
+ *      triplet on ties).
+ *   2. for an H-degenerate sample, plane-and-parallax: H is refitted by the homography RANSAC's least-squares rounds on its inliers
+ *      at DEG_H_TH; each of the 256 threads draws two distinct rows that are not inliers of H (rejection, at most 64 draws, from
+ *      hypothesis 2^31 + k 256 + thread of the sampler with seed ^ 0xD5A61266F0C9392C, k the degeneracy tests so far), and
+ *      F = [e']x H with e' = (H x_a x x'_a) x (H x_b x x'_b).  The F with most inliers (then the lowest thread) replaces the
+ *      so-far-best model when it has more inliers.
+ *   3. local optimisation: the refit rounds of the end (below) on the so-far-best model; their count is the `best` of the stopping
+ *      rule.  d_inl is scratch in the meantime.
+ *   After the search, the refit rounds and outputs are ag_fundamental_ransac's; d_iters counts the 7-point samples.
  * ag_gt_correspondences_pairs: get_GT_correspondence_indexes (ReprojectionStuff.py:126-137) per pair with d_H1to2 [P,3,3]: the image-2
  * centres of all the pair's tentatives are mapped through H^-1 into image 1, and tentative t is true when ANY of them lies within
  * dist_threshold of its image-1 centre, by the fp32 distance sqrt(|(|p|^2 + |a|^2) - 2 a.p + 1e-12|) (nearest: the lowest index among the
@@ -419,6 +437,9 @@ int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_
 int ag_fundamental_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                           const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
                           float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
+int ag_fundamental_degensac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                            const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
+                            float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
 int ag_gt_correspondences_pairs(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                                 const int* d_tent, const int* d_ntent, int tcap, const float* d_H1to2, float dist_threshold,
                                 float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream);
