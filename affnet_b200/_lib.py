@@ -60,6 +60,11 @@ class PipelineEstimators(C.Structure):
 DESC_HARDNET, DESC_SIFT = 0, 1
 
 
+class FrobeniusParams(C.Structure):
+    _fields_ = [("dist_threshold", C.c_float), ("center_dist_th", C.c_float), ("scale_diff_coef", C.c_float), ("center_gate", C.c_int),
+                ("skip_center", C.c_int), ("do_up_is_up", C.c_int), ("inv_to_eye", C.c_int)]
+
+
 class PipelineDescriptor(C.Structure):
     _fields_ = [("kind", C.c_int), ("ps", C.c_int), ("clipval", C.c_float)]
 
@@ -130,6 +135,9 @@ PROTOTYPES = {
     "ag_fundamental_ransac": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp, vp]),
     "ag_fundamental_degensac": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp, vp]),
     "ag_gt_correspondences_pairs": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, vp, f32, vp, vp, vp, vp, vp]),
+    "ag_gt_frobenius_pairs": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, vp, C.POINTER(FrobeniusParams), vp, vp, vp, vp, vp]),
+    "ag_gt_frobenius_sets": (i32, [vp, i32, i32, vp, vp, i32, i32, vp, vp, i32, vp, C.POINTER(FrobeniusParams), vp, vp, vp, vp, vp]),
+    "ag_reproject_lafs": (i32, [vp, i32, i32, vp, i32, i32, vp, vp]),
     "ag_pipeline_create": (i32, [C.POINTER(PipelineConfig), vp, vp, vp, C.POINTER(vp)]),
     "ag_pipeline_create_ex": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), vp, vp, vp, C.POINTER(vp)]),
     "ag_pipeline_create_desc": (i32, [C.POINTER(PipelineConfig), C.POINTER(PipelineEstimators), C.POINTER(PipelineDescriptor), vp, vp, vp,

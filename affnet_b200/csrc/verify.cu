@@ -3,6 +3,8 @@
 //   ag_fundamental_ransac        fundamental-matrix RANSAC (the notebook's commented-out findFundamentalMatrix(src, dst, 0.5))
 //   ag_fundamental_degensac      the same with DEGENSAC's degeneracy test, plane-and-parallax and local optimisation (pydegensac's family)
 //   ag_gt_correspondences_pairs  ReprojectionStuff.get_GT_correspondence_indexes (the reference's "true matches" count), per pair
+//   ag_gt_frobenius_pairs / _sets  get_GT_correspondence_indexes_Fro(_and_center): affine-shape ground truth on tentatives or whole sets
+//   ag_reproject_lafs            ReprojectionStuff.reprojectLAFs
 //
 // The RANSACs are deterministic and restated line by line in numpy by tests/oracle_ransac.py, tests/oracle_fransac.py and
 // tests/oracle_degensac.py, so their
@@ -46,10 +48,11 @@ __device__ __forceinline__ int pair_tentatives(const int* __restrict__ pairs, in
     return n;
 }
 
-// Block-wide: true when every tentative row of the pair indexes a row inside its set's cap (nothing is read otherwise).
+// Block-wide over NT threads: true when every tentative row of the pair indexes a row inside its set's cap (nothing is read otherwise).
+template <int NT = VT>
 __device__ bool rows_in_range(const int* __restrict__ tent, int n, int cap1, int cap2) {
     bool bad = false;
-    for (int t = threadIdx.x; t < n; t += VT) {
+    for (int t = threadIdx.x; t < n; t += NT) {
         const int r1 = tent[2 * (size_t)t], r2 = tent[2 * (size_t)t + 1];
         bad |= r1 < 0 || r1 >= cap1 || r2 < 0 || r2 >= cap2;
     }
@@ -440,6 +443,22 @@ __global__ void __launch_bounds__(VT) ransac_kernel(const float* __restrict__ la
 // ---- ground-truth check (ReprojectionStuff.py:126-137) ----------------------------------------------------------------------------
 constexpr int GT_TILE = 2048;
 
+// H1to2^-1 = adj(H) / det(H) of the fp32 H, in fp64.
+__device__ __forceinline__ void inverse_h(const float* __restrict__ H1to2, double* Hi) {
+    double H[9], A[9];
+    for (int k = 0; k < 9; k++) H[k] = H1to2[k];
+    adj3(H, A);
+    const double det = H[0] * A[0] + H[1] * A[3] + H[2] * A[6];
+    for (int k = 0; k < 9; k++) Hi[k] = A[k] / det;
+}
+
+// Distance between the centre (ax, ay), na = |a|^2, and q = (x, y, |p|^2, -): sqrt(|(|p|^2 + |a|^2) - 2 a.p + 1e-12|), the rounding
+// steps of ReprojectionStuff.distance_matrix_vector.
+__device__ __forceinline__ float centre_dist(float ax, float ay, float na, float4 q) {
+    const float dot = __fmaf_rn(ay, q.y, __fmul_rn(ax, q.x));
+    return sqrtf(fabsf(__fadd_rn(__fsub_rn(__fadd_rn(q.z, na), __fmul_rn(2.f, dot)), 1e-12f)));
+}
+
 __global__ void __launch_bounds__(VT) gt_kernel(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2, int S2,
                                                 int cap2, const int* __restrict__ pairs, const int* __restrict__ tent_all,
                                                 const int* __restrict__ ntent, int tcap, const float* __restrict__ H1to2, float th,
@@ -458,13 +477,7 @@ __global__ void __launch_bounds__(VT) gt_kernel(const float* __restrict__ lafs1,
     }
     const float* L1 = lafs1 + (size_t)i * cap1 * 6;
     const float* L2 = lafs2 + (size_t)j * cap2 * 6;
-    if (tid == 0) {   // H1to2^-1 = adj(H) / det(H), in fp64
-        double H[9], A[9];
-        for (int k = 0; k < 9; k++) H[k] = H1to2[(size_t)p * 9 + k];
-        adj3(H, A);
-        const double det = H[0] * A[0] + H[1] * A[3] + H[2] * A[6];
-        for (int k = 0; k < 9; k++) Hi[k] = A[k] / det;
-    }
+    if (tid == 0) inverse_h(H1to2 + (size_t)p * 9, Hi);
     __syncthreads();
     const size_t base = (size_t)p * tcap;
     int run = 0;
@@ -489,10 +502,7 @@ __global__ void __launch_bounds__(VT) gt_kernel(const float* __restrict__ lafs1,
             __syncthreads();
             if (t < n)
                 for (int u = 0; u < m; u++) {
-                    const float4 q = tile[u];
-                    // sqrt(|(|p|^2 + |a|^2) - 2 a.p + 1e-12|), the rounding steps of ReprojectionStuff.distance_matrix_vector
-                    const float dot = __fmaf_rn(ay, q.y, __fmul_rn(ax, q.x));
-                    const float v = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fadd_rn(q.z, na), __fmul_rn(2.f, dot)), 1e-12f)));
+                    const float v = centre_dist(ax, ay, na, tile[u]);
                     if (v < best) { best = v; bi = u0 + u; }   // ascending u: the lowest index among the minima
                 }
         }
@@ -512,6 +522,251 @@ __global__ void __launch_bounds__(VT) gt_kernel(const float* __restrict__ lafs1,
         __syncthreads();   // wsum is rewritten by the next row block
     }
     if (tid == 0) ntrue[p] = run;
+}
+
+// ---- Frobenius ground truth (ReprojectionStuff.py:139-203): affine-shape consistency of every row of side 1 against side 2 ----------
+// Per-row and per-column operands are derived in fp64 from the fp32 LAFs and rounded once to fp32; the (row, column) loop is fp32 in
+// the order below, and tests/frobenius_restated.py restates all of it.  CUDA cores only: the loop ends in a min / argmin and a
+// threshold decision, so a reduced-precision product would move rows across the threshold and change which column wins.
+constexpr int FRO_NT = 64;       // side-1 rows per CTA, one per thread: many CTAs per pair, so one large pair still fills the GPU
+constexpr int FRO_TILE = 512;    // side-2 columns per shared-memory tile (18 KB): 12 CTAs per SM
+
+// s = sqrt|det A| in fp64, rounded once; with up_is_up the 2x2 part becomes rectify_up_is_up(A / s) * s in fp32 (LAF.py:285-291,
+// ReprojectionStuff.py:162-169).  s is that of A as given.
+__device__ __forceinline__ float frame_2x2(float (&a)[4], bool up_is_up) {
+    const float s = (float)sqrt(fabs((double)a[0] * a[3] - (double)a[1] * a[2]));
+    if (up_is_up) {
+        float r[4];
+        rectify_up_is_up(__fdiv_rn(a[0], s), __fdiv_rn(a[1], s), __fdiv_rn(a[2], s), __fdiv_rn(a[3], s), r);
+        for (int k = 0; k < 4; k++) a[k] = __fmul_rn(r[k], s);
+    }
+    return s;
+}
+
+// reprojectLAFs (ReprojectionStuff.py:9-40) of the LAF l = [[a00, a01, x], [a10, a11, y]] through G, in fp64: the centre
+// (u, v, w) = G (x, y, 1) / w and the 2x2 part linH(G, x, y) A; A' (row-major) and t' rounded once.
+__device__ __forceinline__ void reproject_laf(const double* G, const float* __restrict__ l, float (&A)[4], float (&t)[2]) {
+    const double x = l[2], y = l[5];
+    const double w = G[6] * x + G[7] * y + G[8], n1 = G[0] * x + G[1] * y + G[2], n2 = G[3] * x + G[4] * y + G[5];
+    const double q1 = n1 / (w * w), q2 = n2 / (w * w);
+    const double j00 = G[0] / w - q1 * G[6], j01 = G[1] / w - q1 * G[7], j10 = G[3] / w - q2 * G[6], j11 = G[4] / w - q2 * G[7];
+    const double a00 = l[0], a01 = l[1], a10 = l[3], a11 = l[4];
+    A[0] = (float)(j00 * a00 + j01 * a10); A[1] = (float)(j00 * a01 + j01 * a11);
+    A[2] = (float)(j10 * a00 + j11 * a10); A[3] = (float)(j10 * a01 + j11 * a11);
+    t[0] = (float)(n1 / w); t[1] = (float)(n2 / w);
+}
+
+// Row i of side 1.  inv_to_eye: m = (B, c) with B = A^-1 and c = -B t (fp64 from A's fp64 inverse), all NaN when the frame is
+// non-finite or singular (det == 0) or B, c do not fit fp32, so none of the row's distances is below anything.  Otherwise m is the
+// LHF's entries (a00, a01, tx, a10, a11, ty) and nl its squared norm (the LHF's 9 entries, or the 2x2 part's 4 with skip_center).
+struct FroRow {
+    float m[6], nl, x, y, na, s1e;
+};
+
+__device__ __forceinline__ void frob_row(const float* __restrict__ l, const ag_frobenius_params_t& prm, FroRow& r) {
+    float a[4] = {l[0], l[1], l[3], l[4]};
+    const float s = frame_2x2(a, prm.do_up_is_up != 0);
+    r.x = l[2]; r.y = l[5];
+    r.na = __fadd_rn(__fmul_rn(r.x, r.x), __fmul_rn(r.y, r.y));
+    r.s1e = __fadd_rn(s, 1e-12f);
+    r.nl = 0.f;
+    if (prm.inv_to_eye) {
+        const double det = (double)a[0] * a[3] - (double)a[1] * a[2];
+        const double b0 = a[3] / det, b1 = -(double)a[1] / det, b2 = -(double)a[2] / det, b3 = a[0] / det;
+        const double tx = r.x, ty = r.y;
+        r.m[0] = (float)b0; r.m[1] = (float)b1; r.m[2] = (float)b2; r.m[3] = (float)b3;
+        r.m[4] = (float)(-(b0 * tx + b1 * ty)); r.m[5] = (float)(-(b2 * tx + b3 * ty));
+        bool ok = det != 0.0;
+        for (int k = 0; k < 4; k++) ok &= isfinite(a[k]);
+        for (int k = 0; k < 6; k++) ok &= isfinite(r.m[k]);
+        if (!ok)
+            for (int k = 0; k < 6; k++) r.m[k] = __int_as_float(0x7fc00000);
+    } else {
+        r.m[0] = a[0]; r.m[1] = a[1]; r.m[2] = r.x; r.m[3] = a[2]; r.m[4] = a[3]; r.m[5] = r.y;
+        double q = (double)a[0] * a[0] + (double)a[1] * a[1] + (double)a[2] * a[2] + (double)a[3] * a[3];
+        if (!prm.skip_center) q = q + (double)r.x * r.x + (double)r.y * r.y + 1.0;
+        r.nl = (float)q;
+    }
+}
+
+// Column j of side 2 mapped into image 1 -> tile entries: ta = A' (rectified with up_is_up), tt = (x', y', |t'|^2, s'), tn = |LHF'|^2
+// (only read when inv_to_eye is 0).
+__device__ __forceinline__ void frob_col(const double* G, const float* __restrict__ l, const ag_frobenius_params_t& prm, float4& ta, float4& tt,
+                                         float& tn) {
+    float A[4], t[2];
+    reproject_laf(G, l, A, t);
+    const float s = frame_2x2(A, prm.do_up_is_up != 0);
+    ta = make_float4(A[0], A[1], A[2], A[3]);
+    tt = make_float4(t[0], t[1], __fadd_rn(__fmul_rn(t[0], t[0]), __fmul_rn(t[1], t[1])), s);
+    double q = (double)A[0] * A[0] + (double)A[1] * A[1] + (double)A[2] * A[2] + (double)A[3] * A[3];
+    if (!prm.skip_center) q = q + (double)t[0] * t[0] + (double)t[1] * t[1] + 1.0;
+    tn = (float)q;
+}
+
+__device__ __forceinline__ float dot2f(float a, float b, float c, float d) { return __fadd_rn(__fmul_rn(a, b), __fmul_rn(c, d)); }
+__device__ __forceinline__ float sqf(float a) { return __fmul_rn(a, a); }
+
+// One row against m columns of a tile.  The distance D, in this order of fp32 operations:
+//   INV:  M = B A' (each entry fl(fl(b a) + fl(b a))), D = ((fl(M00 - 1)^2 + M01^2) + M10^2) + fl(M11 - 1)^2, and without SKIP
+//         D = D + (r0^2 + r1^2), r = fl(fl(B t') + c) with (B t')_k = fl(fl(b_k0 x') + fl(b_k1 y'));
+//   !INV: dot = the products of the LHFs' entries summed left to right (a00, a01, [tx,] a10, a11[, ty, then + 1]),
+//         D = sqrt(|fl(fl(|LHF'|^2 + |LHF|^2) - fl(2 dot)) + 1e-12|).
+// GATE: D + 1000 (1 - scale_ok + centre_far) with centre_far = centre_dist >= cth and scale_ok = |1 - s' / fl(s + 1e-12)| <= coef
+// (always true when coef <= 0).  That sum is never below D, so it is only formed when D < best.
+template <bool INV, bool SKIP, bool GATE>
+__device__ __forceinline__ void frob_scan(const FroRow& r, const float4* __restrict__ ta, const float4* __restrict__ tt,
+                                          const float* __restrict__ tn, int m, int u0, const ag_frobenius_params_t& prm, float& best, int& bi) {
+    const bool sgate = prm.scale_diff_coef > 0.f;
+    for (int u = 0; u < m; u++) {
+        const float4 a = ta[u], t = tt[u];
+        float d;
+        if (INV) {
+            const float m00 = dot2f(r.m[0], a.x, r.m[1], a.z), m01 = dot2f(r.m[0], a.y, r.m[1], a.w);
+            const float m10 = dot2f(r.m[2], a.x, r.m[3], a.z), m11 = dot2f(r.m[2], a.y, r.m[3], a.w);
+            d = __fadd_rn(__fadd_rn(__fadd_rn(sqf(__fsub_rn(m00, 1.f)), sqf(m01)), sqf(m10)), sqf(__fsub_rn(m11, 1.f)));
+            if (!SKIP) {
+                const float r0 = __fadd_rn(dot2f(r.m[0], t.x, r.m[1], t.y), r.m[4]);
+                const float r1 = __fadd_rn(dot2f(r.m[2], t.x, r.m[3], t.y), r.m[5]);
+                d = __fadd_rn(d, __fadd_rn(sqf(r0), sqf(r1)));
+            }
+        } else {
+            float dot;
+            if (SKIP) {
+                dot = __fadd_rn(__fadd_rn(dot2f(r.m[0], a.x, r.m[1], a.y), __fmul_rn(r.m[3], a.z)), __fmul_rn(r.m[4], a.w));
+            } else {
+                dot = __fadd_rn(dot2f(r.m[0], a.x, r.m[1], a.y), __fmul_rn(r.m[2], t.x));
+                dot = __fadd_rn(__fadd_rn(__fadd_rn(dot, __fmul_rn(r.m[3], a.z)), __fmul_rn(r.m[4], a.w)), __fmul_rn(r.m[5], t.y));
+                dot = __fadd_rn(dot, 1.f);
+            }
+            d = sqrtf(fabsf(__fadd_rn(__fsub_rn(__fadd_rn(tn[u], r.nl), __fmul_rn(2.f, dot)), 1e-12f)));
+        }
+        if (!(d < best)) continue;
+        if (GATE) {
+            const bool far = centre_dist(r.x, r.y, r.na, t) >= prm.center_dist_th;
+            const bool ok = !sgate || fabsf(__fsub_rn(1.f, __fdiv_rn(t.w, r.s1e))) <= prm.scale_diff_coef;
+            d = __fadd_rn(__fmul_rn(__fadd_rn(__fsub_rn(1.f, ok ? 1.f : 0.f), far ? 1.f : 0.f), 1000.f), d);
+            if (!(d < best)) continue;
+        }
+        best = d; bi = u0 + u;   // ascending u: the lowest index among the minima; NaN never wins
+    }
+}
+
+// Pair p -> (i, j) and the row / column counts n1, n2 (tentative mode: n1 = n2 = ntent[p]), or false when the pair cannot be checked:
+// an image index out of range, a count outside 0..cap.  The tentative rows' range is checked by the caller (block-wide).
+template <bool TENT>
+__device__ __forceinline__ bool frob_pair(const int* __restrict__ pairs, int p, int S1, int cap1, int S2, int cap2, const int* __restrict__ cnt1,
+                                          const int* __restrict__ cnt2, int tcap, int& i, int& j, int& n1, int& n2) {
+    if (TENT) {
+        n1 = n2 = pair_tentatives(pairs, p, S1, S2, cnt1, tcap, i, j);
+        return n1 >= 0;
+    }
+    i = pairs ? pairs[2 * (size_t)p] : p;
+    j = pairs ? pairs[2 * (size_t)p + 1] : p;
+    if (i < 0 || i >= S1 || j < 0 || j >= S2) return false;
+    n1 = cnt1[i]; n2 = cnt2[j];
+    return n1 >= 0 && n1 <= cap1 && n2 >= 0 && n2 <= cap2;
+}
+
+// Grid (P, rcap / FRO_NT): thread t of CTA y owns row y FRO_NT + t of pair p; the CTA streams the pair's reprojected columns through
+// shared memory and writes the row's (min_dist, idx2).  TENT: rows and columns are the tentatives' rows of lafs1 / lafs2, cnt1 = ntent;
+// otherwise rows 0..cnt1[i]-1 of set i against rows 0..cnt2[j]-1 of set j.
+template <bool TENT>
+__global__ void __launch_bounds__(FRO_NT) frob_pass_kernel(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2,
+                                                           int S2, int cap2, const int* __restrict__ pairs, const int* __restrict__ tent_all,
+                                                           const int* __restrict__ cnt1, const int* __restrict__ cnt2, int rcap,
+                                                           const float* __restrict__ H1to2, const ag_frobenius_params_t prm,
+                                                           float* __restrict__ min_dist, int* __restrict__ idx2) {
+    __shared__ float4 ta[FRO_TILE], tt[FRO_TILE];
+    __shared__ float tn[FRO_TILE];
+    __shared__ double G[9];
+    const int p = blockIdx.x, tid = threadIdx.x, t = blockIdx.y * FRO_NT + tid;
+    int i, j, n1, n2;
+    if (!frob_pair<TENT>(pairs, p, S1, cap1, S2, cap2, cnt1, cnt2, rcap, i, j, n1, n2) || (int)blockIdx.y * FRO_NT >= n1) return;
+    const int* tent = TENT ? tent_all + (size_t)p * rcap * 2 : nullptr;
+    if (TENT && !rows_in_range<FRO_NT>(tent, n1, cap1, cap2)) return;
+    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
+    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
+    if (tid == 0) inverse_h(H1to2 + (size_t)p * 9, G);
+    FroRow r;
+    if (t < n1) frob_row(L1 + (size_t)(TENT ? tent[2 * (size_t)t] : t) * 6, prm, r);
+    float best = INFINITY;
+    int bi = 0;
+    const int variant = (prm.inv_to_eye ? 4 : 0) + (prm.skip_center ? 2 : 0) + (prm.center_gate ? 1 : 0);
+    for (int u0 = 0; u0 < n2; u0 += FRO_TILE) {
+        const int m = min(FRO_TILE, n2 - u0);
+        __syncthreads();
+        for (int u = tid; u < m; u += FRO_NT)
+            frob_col(G, L2 + (size_t)(TENT ? tent[2 * (size_t)(u0 + u) + 1] : u0 + u) * 6, prm, ta[u], tt[u], tn[u]);
+        __syncthreads();
+        if (t >= n1) continue;
+        switch (variant) {
+            case 0: frob_scan<false, false, false>(r, ta, tt, tn, m, u0, prm, best, bi); break;
+            case 1: frob_scan<false, false, true>(r, ta, tt, tn, m, u0, prm, best, bi); break;
+            case 2: frob_scan<false, true, false>(r, ta, tt, tn, m, u0, prm, best, bi); break;
+            case 3: frob_scan<false, true, true>(r, ta, tt, tn, m, u0, prm, best, bi); break;
+            case 4: frob_scan<true, false, false>(r, ta, tt, tn, m, u0, prm, best, bi); break;
+            case 5: frob_scan<true, false, true>(r, ta, tt, tn, m, u0, prm, best, bi); break;
+            case 6: frob_scan<true, true, false>(r, ta, tt, tn, m, u0, prm, best, bi); break;
+            default: frob_scan<true, true, true>(r, ta, tt, tn, m, u0, prm, best, bi); break;
+        }
+    }
+    if (t < n1) {
+        min_dist[(size_t)p * rcap + t] = best;
+        idx2[(size_t)p * rcap + t] = bi;
+    }
+}
+
+// One CTA per pair: the rows with min_dist <= dist_threshold in ascending order into true / ntrue (-1 for a pair that cannot be checked).
+template <bool TENT>
+__global__ void __launch_bounds__(VT) frob_compact_kernel(int S1, int cap1, int S2, int cap2, const int* __restrict__ pairs,
+                                                          const int* __restrict__ tent_all, const int* __restrict__ cnt1,
+                                                          const int* __restrict__ cnt2, int rcap, float th, const float* __restrict__ min_dist,
+                                                          int* __restrict__ true_all, int* __restrict__ ntrue) {
+    __shared__ int wsum[VT / 32];
+    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int i, j, n1, n2;
+    bool ok = frob_pair<TENT>(pairs, p, S1, cap1, S2, cap2, cnt1, cnt2, rcap, i, j, n1, n2);
+    if (TENT && ok) ok = rows_in_range(tent_all + (size_t)p * rcap * 2, n1, cap1, cap2);
+    if (!ok) {
+        if (tid == 0) ntrue[p] = -1;
+        return;
+    }
+    const size_t base = (size_t)p * rcap;
+    int run = 0;
+    for (int r0 = 0; r0 < n1; r0 += VT) {
+        const int t = r0 + tid;
+        const bool keep = t < n1 && min_dist[base + t] <= th;
+        const unsigned b = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) wsum[warp] = __popc(b);
+        __syncthreads();
+        int off = run, tot = 0;
+#pragma unroll
+        for (int w = 0; w < VT / 32; w++) {
+            off += w < warp ? wsum[w] : 0;
+            tot += wsum[w];
+        }
+        if (keep) true_all[base + off + __popc(b & ((1u << lane) - 1u))] = t;
+        run += tot;
+        __syncthreads();   // wsum is rewritten by the next row block
+    }
+    if (tid == 0) ntrue[p] = run;
+}
+
+// reprojectLAFs for S sets of cap rows, one H per set (G = H, or H^-1 with invert), the 2x2 part rectified with up_is_up.
+__global__ void reproject_lafs_kernel(const float* __restrict__ lafs, int cap, const float* __restrict__ H, int invert, int up_is_up,
+                                      float* __restrict__ out) {
+    const int s = blockIdx.y, r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= cap) return;
+    double G[9];
+    if (invert) inverse_h(H + (size_t)s * 9, G);
+    else
+        for (int k = 0; k < 9; k++) G[k] = H[(size_t)s * 9 + k];
+    const size_t o = ((size_t)s * cap + r) * 6;
+    float A[4], t[2];
+    reproject_laf(G, lafs + o, A, t);
+    frame_2x2(A, up_is_up != 0);
+    out[o] = A[0]; out[o + 1] = A[1]; out[o + 2] = t[0];
+    out[o + 3] = A[2]; out[o + 4] = A[3]; out[o + 5] = t[1];
 }
 
 // ---- fundamental-matrix RANSAC (the notebook's alternative line, findFundamentalMatrix(src, dst, 0.5)) ----------------------------
@@ -1205,6 +1460,59 @@ int ag_gt_correspondences_pairs(const float* d_lafs1, int S1, int cap1, const fl
     gt_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, d_H1to2, dist_threshold,
                                                   d_min_dist, d_idx2, d_true, d_ntrue);
     AG_CHECK_LAUNCH("gt_kernel");
+    return AG_OK;
+}
+
+static int frobenius_params(const ag_frobenius_params_t* prm) {
+    AG_REQUIRE(prm, "NULL parameters");
+    AG_REQUIRE(prm->dist_threshold >= 0.f, "dist_threshold must be >= 0 (and not NaN)");
+    AG_REQUIRE(prm->center_dist_th >= 0.f, "center_dist_th must be >= 0 (and not NaN)");
+    AG_REQUIRE(prm->scale_diff_coef == prm->scale_diff_coef, "scale_diff_coef must not be NaN");
+    return AG_OK;
+}
+
+int ag_gt_frobenius_pairs(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                          const int* d_tent, const int* d_ntent, int tcap, const float* d_H1to2, const ag_frobenius_params_t* prm,
+                          float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream) {
+    int rc = verify_args("ag_gt_frobenius_pairs", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc) return rc;
+    AG_REQUIRE(d_H1to2 && d_min_dist && d_idx2 && d_true && d_ntrue, "NULL homography or output");
+    if ((rc = frobenius_params(prm))) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    frob_pass_kernel<true><<<dim3(P, cdiv(tcap, FRO_NT)), FRO_NT, 0, st>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent,
+                                                                          nullptr, tcap, d_H1to2, *prm, d_min_dist, d_idx2);
+    AG_CHECK_LAUNCH("frob_pass_kernel");
+    frob_compact_kernel<true><<<P, VT, 0, st>>>(S1, cap1, S2, cap2, d_pairs, d_tent, d_ntent, nullptr, tcap, prm->dist_threshold, d_min_dist,
+                                                d_true, d_ntrue);
+    AG_CHECK_LAUNCH("frob_compact_kernel");
+    return AG_OK;
+}
+
+int ag_gt_frobenius_sets(const float* d_lafs1, int S1, int cap1, const int* d_count1, const float* d_lafs2, int S2, int cap2,
+                         const int* d_count2, const int* d_pairs, int P, const float* d_H1to2, const ag_frobenius_params_t* prm,
+                         float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream) {
+    AG_REQUIRE(d_lafs1 && d_lafs2 && d_count1 && d_count2, "NULL LAFs or counts");
+    AG_REQUIRE(S1 >= 1 && S2 >= 1 && cap1 >= 1 && cap2 >= 1 && P >= 1, "S1, S2, cap1, cap2 and P must be >= 1");
+    AG_REQUIRE(d_pairs || (S1 == S2 && P == S1), "d_pairs == NULL (pair p = (p, p)) needs S1 == S2 == P");
+    AG_REQUIRE(cap1 <= MAX_TCAP, "cap1 must be <= 4194240");
+    AG_REQUIRE(d_H1to2 && d_min_dist && d_idx2 && d_true && d_ntrue, "NULL homography or output");
+    int rc = frobenius_params(prm);
+    if (rc) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    frob_pass_kernel<false><<<dim3(P, cdiv(cap1, FRO_NT)), FRO_NT, 0, st>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, nullptr, d_count1,
+                                                                           d_count2, cap1, d_H1to2, *prm, d_min_dist, d_idx2);
+    AG_CHECK_LAUNCH("frob_pass_kernel");
+    frob_compact_kernel<false><<<P, VT, 0, st>>>(S1, cap1, S2, cap2, d_pairs, nullptr, d_count1, d_count2, cap1, prm->dist_threshold,
+                                                 d_min_dist, d_true, d_ntrue);
+    AG_CHECK_LAUNCH("frob_compact_kernel");
+    return AG_OK;
+}
+
+int ag_reproject_lafs(const float* d_lafs, int S, int cap, const float* d_H, int invert, int up_is_up, float* d_out, void* stream) {
+    AG_REQUIRE(d_lafs && d_H && d_out, "NULL LAFs, homography or output");
+    AG_REQUIRE(S >= 1 && S <= 65535 && cap >= 1, "S must be in 1..65535 and cap >= 1");
+    reproject_lafs_kernel<<<dim3(cdiv(cap, VT), S), VT, 0, (cudaStream_t)stream>>>(d_lafs, cap, d_H, invert, up_is_up, d_out);
+    AG_CHECK_LAUNCH("reproject_lafs_kernel");
     return AG_OK;
 }
 

@@ -430,7 +430,36 @@ int ag_match_pairs(const float* d_desc1, const int* d_count1, int S1, int cap1, 
  * centres of all the pair's tentatives are mapped through H^-1 into image 1, and tentative t is true when ANY of them lies within
  * dist_threshold of its image-1 centre, by the fp32 distance sqrt(|(|p|^2 + |a|^2) - 2 a.p + 1e-12|) (nearest: the lowest index among the
  * minima, NaN ignored).  d_min_dist, d_idx2 [P,tcap]; d_true [P,tcap] the true t in ascending order, d_ntrue [P] their number.
- *   AG_ERR_INVALID also for dist_threshold < 0 or NaN. */
+ *   AG_ERR_INVALID also for dist_threshold < 0 or NaN.
+ * ag_gt_frobenius_pairs: get_GT_correspondence_indexes_Fro / _Fro_and_center (ReprojectionStuff.py:139-203) per pair, with the
+ * arguments, the -1 rule and the outputs of ag_gt_correspondences_pairs: row t (lafs1[i, tent[p,t,0]]) against the frames
+ * lafs2[j, tent[p,u,1]] of all the pair's tentatives, mapped into image 1 through H^-1 (H^-1 in fp64, linearised at each centre as
+ * reprojectLAFs / linH do; each mapped frame rounded once to fp32).  With B = A1^-1, c = -B t1 (fp64, rounded once) the distance is
+ * D = |B A2' - I|_F^2 + |B t2' + c|^2 (the first term only with skip_center); inv_to_eye = 0 takes instead the reference's expanded
+ * sqrt(|(|L2'|^2 + |L1|^2) - 2 L1.L2' + 1e-12|) over the 3x3 frames' 9 entries (the 2x2 parts' 4 with skip_center).  center_gate adds
+ * 1000 when the centres are >= center_dist_th apart (gt_kernel's distance) and 1000 when |1 - s2 / (s1 + 1e-12)| > scale_diff_coef
+ * (s = sqrt|det A|, A as given; no scale gate when scale_diff_coef <= 0); do_up_is_up rectifies both 2x2 parts to
+ * rectifyAffineTransformationUpIsUp(A / s) s first.  Per row: the minimum with the lowest index, NaN ignored, (+inf, 0) when there is
+ * none; true when <= dist_threshold.  A side-1 frame that is not finite, singular (det 0) or whose inverse overflows fp32 has only NaN
+ * distances with inv_to_eye (min_dist +inf, idx2 0, never true); a non-finite side-2 frame never wins a row.  The fp32 operation order is
+ * that of tests/frobenius_restated.py.  Rows at or beyond ntent are neither read nor written.
+ *   AG_ERR_INVALID also for NULL prm, dist_threshold or center_dist_th < 0 or NaN, scale_diff_coef NaN.
+ * ag_gt_frobenius_sets: the same on whole detection sets (affine-region repeatability): pair p = (i, j) checks rows
+ * 0..d_count1[i]-1 of set i against rows 0..d_count2[j]-1 of set j (counts read on the device; d_count1 [S1], d_count2 [S2]).
+ * d_min_dist, d_idx2, d_true [P,cap1]; d_ntrue [P], -1 when i or j is out of range or a count lies outside 0..cap.  A row at or beyond
+ * count1 is neither read nor written, nor is a column at or beyond count2.  d_pairs may be NULL when S1 == S2 == P.
+ * ag_reproject_lafs: reprojectLAFs (ReprojectionStuff.py:23-40) of S sets of cap LAFs [S,cap,2,3], set s through d_H[s] (its fp64
+ * inverse with invert != 0), the 2x2 part rectified as above with up_is_up != 0 -> d_out [S,cap,2,3]; the frames of
+ * ag_gt_frobenius_*'s side 2. */
+typedef struct {
+    float dist_threshold;   /* a row is true when its minimum is <= this */
+    float center_dist_th;   /* center_gate: + 1000 when the centres are at least this far apart */
+    float scale_diff_coef;  /* center_gate: + 1000 when the scale ratio differs from 1 by more; <= 0: no scale gate */
+    int center_gate;        /* 0: get_GT_correspondence_indexes_Fro; 1: get_GT_correspondence_indexes_Fro_and_center */
+    int skip_center;        /* skip_center_in_Fro */
+    int do_up_is_up;
+    int inv_to_eye;
+} ag_frobenius_params_t;
 int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                          const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
                          float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
@@ -443,6 +472,13 @@ int ag_fundamental_degensac(const float* d_lafs1, int S1, int cap1, const float*
 int ag_gt_correspondences_pairs(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                                 const int* d_tent, const int* d_ntent, int tcap, const float* d_H1to2, float dist_threshold,
                                 float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream);
+int ag_gt_frobenius_pairs(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                          const int* d_tent, const int* d_ntent, int tcap, const float* d_H1to2, const ag_frobenius_params_t* prm,
+                          float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream);
+int ag_gt_frobenius_sets(const float* d_lafs1, int S1, int cap1, const int* d_count1, const float* d_lafs2, int S2, int cap2,
+                         const int* d_count2, const int* d_pairs, int P, const float* d_H1to2, const ag_frobenius_params_t* prm,
+                         float* d_min_dist, int* d_idx2, int* d_true, int* d_ntrue, void* stream);
+int ag_reproject_lafs(const float* d_lafs, int S, int cap, const float* d_H, int invert, int up_is_up, float* d_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Batched end-to-end pipeline (new; the reference processes one image at a time):
