@@ -8,6 +8,9 @@ import torch
 from . import _lib as L
 
 MAX_TCAP = 4194240   # ag_match_pairs' cap1 limit
+# find_homography_pairs(affine=True)'s frame threshold: the smallest of {0.5, 1, 2, 4} (4 is the reference's threshold for this distance)
+# that keeps >= 95 % of the GT-true tentatives of the warped pairs and graf 1->6 under the true H (DESIGN.md, profiles/affine_ransac_h100.json)
+AFFINE_LAF_TH = 0.5
 
 
 def _int_shape(t, shape, name, fn, label=None):
@@ -47,7 +50,8 @@ def _pair_args(fn, lafs1, tent, ntent, lafs2, pairs):
     return a, b, tent, ntent, pairs, P, tcap
 
 
-def find_homography_pairs(lafs1, tent, ntent, lafs2=None, pairs=None, inl_th=2.0, confidence=0.99, max_iters=50000, seed=0):
+def find_homography_pairs(lafs1, tent, ntent, lafs2=None, pairs=None, inl_th=2.0, confidence=0.99, max_iters=50000, seed=0, affine=False,
+                          laf_th=None):
     """Homography RANSAC for every pair, in one launch (ag_homography_ransac): lafs1 [S1,cap1,2,3] and lafs2 [S2,cap2,2,3] (default:
     lafs1) pixel LAFs, tent [P,tcap,2] / ntent [P] of match_snn_pairs, pairs [P,2] as given to match_snn_pairs (None: pair p = (p, p)).
     Tentative t joins the centres lafs1[i, tent[p,t,0], :, 2] and lafs2[j, tent[p,t,1], :, 2].  The defaults are those of the notebook's
@@ -55,10 +59,24 @@ def find_homography_pairs(lafs1, tent, ntent, lafs2=None, pairs=None, inl_th=2.0
     other pairs.
     -> (H [P,3,3] float32 with H[2,2] = 1, inl [P,tcap] uint8, ninl [P] int32, iters [P] int32 hypotheses evaluated).  ninl[p] is -1 for a
     pair that cannot be verified (ntent -1, an index out of range); 0 with H = 0 when it has fewer than 4 tentatives or no usable sample.
-    Rows at or beyond ntent[p] are unspecified."""
+    Rows at or beyond ntent[p] are unspecified.
+    affine=True (ag_homography_ransac_affine) uses the whole frames: each tentative is an affine correspondence (its centres and the local
+    affinity A2 A1^-1), two of them give a hypothesis where points need four, and an inlier must also have frames that agree with H:
+    D = |A1^-1 J A2 - I|_F^2 <= laf_th, J the Jacobian of H^-1 at the image-2 centre (the reference's skip-centre Frobenius distance).
+    laf_th defaults to AFFINE_LAF_TH (0.5); +inf tests the centres and the frames' finiteness only.  0.5 keeps >= 97 % of the true
+    matches of small synthetic warps but only 76 % on graf 1->6 (91 % at 4): for wide-baseline pairs, whose frames are noisier, a larger
+    laf_th keeps more true matches (graf 1->6: 36 inliers at 0.5, 43 at 1, 45 at 2).  The frames must be oriented (OriNet or
+    histogram orientation): without orientation (do_ori=False) and with an in-plane rotation between the views A2 A1^-1 is wrong, and
+    the 4-point call is the right one.  iters then counts 2-AC samples, and fewer than 2 tentatives give ninl 0."""
     fn = "find_homography_pairs"
     if not float(inl_th) > 0.0 or float(inl_th) == float("inf"):
         raise L.AffnetB200Error("%s: inl_th must be finite and > 0" % fn)
+    if laf_th is not None and not affine:
+        raise L.AffnetB200Error("%s: laf_th is the affine test's threshold and needs affine=True" % fn)
+    if affine:
+        laf_th = AFFINE_LAF_TH if laf_th is None else float(laf_th)
+        if not laf_th > 0.0:
+            raise L.AffnetB200Error("%s: laf_th must be > 0 (+inf: no frame threshold)" % fn)
     if not 0.0 < float(confidence) < 1.0:
         raise L.AffnetB200Error("%s: confidence must be in (0, 1)" % fn)
     if int(max_iters) < 1:
@@ -70,6 +88,12 @@ def find_homography_pairs(lafs1, tent, ntent, lafs2=None, pairs=None, inl_th=2.0
     ninl = torch.empty(P, dtype=torch.int32, device=dev)
     iters = torch.empty(P, dtype=torch.int32, device=dev)
     if P == 0:
+        return H, inl, ninl, iters
+    if affine:
+        L.check(L.lib().ag_homography_ransac_affine(L.ptr(a), a.size(0), a.size(1), L.ptr(b), b.size(0), b.size(1), L.ptr(pairs), P,
+                                                    L.ptr(tent), L.ptr(ntent), tcap, float(inl_th), laf_th, float(confidence), int(max_iters),
+                                                    int(seed) & (2 ** 64 - 1), L.ptr(H), L.ptr(inl), L.ptr(ninl), L.ptr(iters),
+                                                    L.stream_ptr()))
         return H, inl, ninl, iters
     L.check(L.lib().ag_homography_ransac(L.ptr(a), a.size(0), a.size(1), L.ptr(b), b.size(0), b.size(1), L.ptr(pairs), P, L.ptr(tent),
                                          L.ptr(ntent), tcap, float(inl_th), float(confidence), int(max_iters), int(seed) & (2 ** 64 - 1),

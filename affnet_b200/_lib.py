@@ -132,6 +132,8 @@ PROTOTYPES = {
     "ag_match_pairs_workspace_bytes": (sz, [i32, i32, i32, i32, i32]),
     "ag_match_pairs": (i32, [vp, vp, i32, i32, vp, vp, i32, i32, i32, vp, i32, f32, vp, sz, vp, vp, vp, vp, vp, vp, vp]),
     "ag_homography_ransac": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp, vp]),
+    "ag_homography_ransac_affine": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp,
+                                          vp]),
     "ag_fundamental_ransac": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp, vp]),
     "ag_fundamental_degensac": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, f32, f32, i32, C.c_uint64, vp, vp, vp, vp, vp]),
     "ag_gt_correspondences_pairs": (i32, [vp, i32, i32, vp, i32, i32, vp, i32, vp, vp, i32, vp, f32, vp, vp, vp, vp, vp]),

@@ -1,13 +1,14 @@
 // Geometric verification of the batched matcher's tentatives (after ag_match_pairs), one CTA per pair:
 //   ag_homography_ransac         homography RANSAC (the notebook's ransac_validate: findHomography(src, dst, 2.0, 0.99, 50000))
+//   ag_homography_ransac_affine  the same from 2 affine correspondences per sample, with frame-consistent inliers
 //   ag_fundamental_ransac        fundamental-matrix RANSAC (the notebook's commented-out findFundamentalMatrix(src, dst, 0.5))
 //   ag_fundamental_degensac      the same with DEGENSAC's degeneracy test, plane-and-parallax and local optimisation (pydegensac's family)
 //   ag_gt_correspondences_pairs  ReprojectionStuff.get_GT_correspondence_indexes (the reference's "true matches" count), per pair
 //   ag_gt_frobenius_pairs / _sets  get_GT_correspondence_indexes_Fro(_and_center): affine-shape ground truth on tentatives or whole sets
 //   ag_reproject_lafs            ReprojectionStuff.reprojectLAFs
 //
-// The RANSACs are deterministic and restated line by line in numpy by tests/oracle_ransac.py, tests/oracle_fransac.py and
-// tests/oracle_degensac.py, so their
+// The RANSACs are deterministic and restated line by line in numpy by tests/oracle_ransac.py, tests/oracle_ac_ransac.py,
+// tests/oracle_fransac.py and tests/oracle_degensac.py, so their
 // decisions (samples, degeneracy, inlier counts, the stopping point) are reproduced exactly.  For that reason all their arithmetic is
 // fp64, with + - * / sqrt only where a decision depends on it, and this file is compiled with
 // -fmad=false (build.sh): numpy rounds every product and sum separately, so fused multiply-adds here would move near-threshold decisions.
@@ -64,6 +65,16 @@ __device__ __forceinline__ float4 tent_centres(const float* __restrict__ L1, con
     const float* a = L1 + (size_t)tent[2 * (size_t)t] * 6;
     const float* b = L2 + (size_t)tent[2 * (size_t)t + 1] * 6;
     return make_float4(a[2], a[5], b[2], b[5]);
+}
+
+// Tentative t as an affine correspondence: its centres c (as tent_centres) and the 2x2 parts (a00, a01, a10, a11) of both frames.
+struct AcRow {
+    float4 c, a1, a2;
+};
+__device__ __forceinline__ AcRow tent_ac(const float* __restrict__ L1, const float* __restrict__ L2, const int* __restrict__ tent, int t) {
+    const float* a = L1 + (size_t)tent[2 * (size_t)t] * 6;
+    const float* b = L2 + (size_t)tent[2 * (size_t)t + 1] * 6;
+    return {make_float4(a[2], a[5], b[2], b[5]), make_float4(a[0], a[1], a[3], a[4]), make_float4(b[0], b[1], b[3], b[4])};
 }
 
 // ---- fp64 3x3 helpers (row-major), in the restatement's operation order ------------------------------------------------------------
@@ -260,16 +271,23 @@ __device__ void normal_matrix_eigen(RansacShared& s) {
 }
 
 __device__ __forceinline__ bool is_inlier_f(const double* F, float4 c, double th2);
+__device__ __forceinline__ bool is_inlier_ac(const double* H, const double* G, const AcRow& r, double th2, double laf_th);
 
-// Inliers of H (a homography, or a fundamental matrix when FUND) over all n tentatives (thread t handles rows t, t + VT, ...); writes
-// the mask when `inl` is not NULL.  Block total.
-template <bool FUND = false>
+// Inliers of H (a homography, or a fundamental matrix when FUND; with AFF a homography whose inliers must also pass the frame test at
+// laf_th) over all n tentatives (thread t handles rows t, t + VT, ...); writes the mask when `inl` is not NULL.  Block total.
+template <bool FUND = false, bool AFF = false>
 __device__ int score_rows(const double* H, const float* L1, const float* L2, const int* tent, int n, double th2, unsigned char* inl,
-                          RansacShared& s) {
+                          RansacShared& s, double laf_th = 0.0) {
+    double G[9];
+    if (AFF) adj3(H, G);
     int cnt = 0;
     for (int t = threadIdx.x; t < n; t += VT) {
-        const float4 c = tent_centres(L1, L2, tent, t);
-        const bool in = FUND ? is_inlier_f(H, c, th2) : is_inlier(H, c, th2);
+        bool in;
+        if (AFF) in = is_inlier_ac(H, G, tent_ac(L1, L2, tent, t), th2, laf_th);
+        else {
+            const float4 c = tent_centres(L1, L2, tent, t);
+            in = FUND ? is_inlier_f(H, c, th2) : is_inlier(H, c, th2);
+        }
         cnt += in;
         if (inl) inl[t] = in;
     }
@@ -545,11 +563,20 @@ __device__ __forceinline__ float frame_2x2(float (&a)[4], bool up_is_up) {
 
 // reprojectLAFs (ReprojectionStuff.py:9-40) of the LAF l = [[a00, a01, x], [a10, a11, y]] through G, in fp64: the centre
 // (u, v, w) = G (x, y, 1) / w and the 2x2 part linH(G, x, y) A; A' (row-major) and t' rounded once.
-__device__ __forceinline__ void reproject_laf(const double* G, const float* __restrict__ l, float (&A)[4], float (&t)[2]) {
-    const double x = l[2], y = l[5];
-    const double w = G[6] * x + G[7] * y + G[8], n1 = G[0] * x + G[1] * y + G[2], n2 = G[3] * x + G[4] * y + G[5];
+// linH (ReprojectionStuff.py:9-21): the Jacobian j (row-major) of x -> G x at (x, y), with (n1, n2, w) = G (x, y, 1).  It does not
+// depend on G's scale.
+__device__ __forceinline__ void lin_h(const double* G, double x, double y, double (&j)[4], double& n1, double& n2, double& w) {
+    w = G[6] * x + G[7] * y + G[8];
+    n1 = G[0] * x + G[1] * y + G[2];
+    n2 = G[3] * x + G[4] * y + G[5];
     const double q1 = n1 / (w * w), q2 = n2 / (w * w);
-    const double j00 = G[0] / w - q1 * G[6], j01 = G[1] / w - q1 * G[7], j10 = G[3] / w - q2 * G[6], j11 = G[4] / w - q2 * G[7];
+    j[0] = G[0] / w - q1 * G[6]; j[1] = G[1] / w - q1 * G[7]; j[2] = G[3] / w - q2 * G[6]; j[3] = G[4] / w - q2 * G[7];
+}
+
+__device__ __forceinline__ void reproject_laf(const double* G, const float* __restrict__ l, float (&A)[4], float (&t)[2]) {
+    double j[4], n1, n2, w;
+    lin_h(G, l[2], l[5], j, n1, n2, w);
+    const double j00 = j[0], j01 = j[1], j10 = j[2], j11 = j[3];
     const double a00 = l[0], a01 = l[1], a10 = l[3], a11 = l[4];
     A[0] = (float)(j00 * a00 + j01 * a10); A[1] = (float)(j00 * a01 + j01 * a11);
     A[2] = (float)(j10 * a00 + j11 * a10); A[3] = (float)(j10 * a01 + j11 * a11);
@@ -1039,20 +1066,21 @@ __device__ bool refit_f(const float* L1, const float* L2, const int* tent, int n
 
 // Up to REFIT_ROUNDS least-squares refits of the model M (shared; a homography, or a fundamental matrix when FUND) on its inliers at
 // th2, each kept only if the inlier count does not drop: the rounds that end both kernels, for DEGENSAC's plane H and its local
-// optimisation.  Block-wide; on return M is the last kept model and `inl` its mask (rows < n).
+// optimisation, and (AFF: the inliers also pass the frame test at laf_th; the refit is the same point DLT) for the affine homography
+// RANSAC's.  Block-wide; on return M is the last kept model and `inl` its mask (rows < n).
 // Returns its inlier count.
-template <bool FUND>
+template <bool FUND, bool AFF = false>
 __device__ __forceinline__ int refit_rounds(const float* L1, const float* L2, const int* tent, int n, double th2, unsigned char* inl,
-                                            double* M, RansacShared& s) {
-    int cnt = score_rows<FUND>(M, L1, L2, tent, n, th2, inl, s);
+                                            double* M, RansacShared& s, double laf_th = 0.0) {
+    int cnt = score_rows<FUND, AFF>(M, L1, L2, tent, n, th2, inl, s, laf_th);
     for (int r = 0; r < REFIT_ROUNDS && cnt >= (FUND ? F_REFIT_MIN : 4); r++) {
         if (!(FUND ? refit_f(L1, L2, tent, n, inl, cnt, s) : refit(L1, L2, tent, n, inl, cnt, s))) break;
-        const int c2 = score_rows<FUND>(s.Hr, L1, L2, tent, n, th2, nullptr, s);
+        const int c2 = score_rows<FUND, AFF>(s.Hr, L1, L2, tent, n, th2, nullptr, s, laf_th);
         if (c2 < cnt) break;
         cnt = c2;
         if (threadIdx.x < 9) M[threadIdx.x] = s.Hr[threadIdx.x];
         __syncthreads();
-        score_rows<FUND>(M, L1, L2, tent, n, th2, inl, s);
+        score_rows<FUND, AFF>(M, L1, L2, tent, n, th2, inl, s, laf_th);
     }
     return cnt;
 }
@@ -1382,6 +1410,256 @@ __global__ void __launch_bounds__(VT) fransac_kernel(const float* __restrict__ l
     }
 }
 
+// ---- homography RANSAC from two affine correspondences (ag_homography_ransac_affine) -------------------------------------------------
+// A tentative of two LAFs gives the centre pair and the local affinity A2 A1^-1, which is the Jacobian a homography has at that point:
+// two of them determine H, where points need four, and a row whose frames disagree with H is not an inlier.
+constexpr int ATILE = sizeof(RansacShared::tile) / sizeof(AcRow);   // 682 rows of 48 B in RansacShared's tile (32 KB)
+constexpr double CHOL_EPS = 1e-10;   // 2-AC normal equations: a Cholesky pivot <= CHOL_EPS times its diagonal entry is a degenerate sample
+// LO-RANSAC's iterative local optimisation (Chum, Matas and Kittler, 2003): point DLT on the inliers at LO_FACTOR times both thresholds
+// (centre and frame), then at half that, ... down to 1 times.  A 2-AC hypothesis from two true matches with noisy frames fits near its
+// sample only: it may have fewer than 4 inliers at the strict thresholds, where the refit rounds cannot start.
+constexpr double LO_FACTOR = 16.0;
+constexpr int LO_STEPS = 5;          // factors 16, 8, 4, 2, 1
+
+// The frame distance of row r under the homography whose adjugate is G (H^-1 up to scale): D = |A1^-1 J A2 - I|_F^2 with J = linH(G) at
+// the image-2 centre, the reference's skip-centre Frobenius distance (get_GT_correspondence_indexes_Fro with skip_center_in_Fro) of the
+// row's own pair, in fp64.  False when either frame is not finite or singular.
+__device__ __forceinline__ bool frame_distance(const double* G, const AcRow& r, double& D) {
+    if (!finite4(r.a1) || !finite4(r.a2)) return false;
+    const double a00 = r.a1.x, a01 = r.a1.y, a10 = r.a1.z, a11 = r.a1.w;
+    const double b00 = r.a2.x, b01 = r.a2.y, b10 = r.a2.z, b11 = r.a2.w;
+    const double det1 = a00 * a11 - a01 * a10, det2 = b00 * b11 - b01 * b10;
+    if (det1 == 0.0 || det2 == 0.0) return false;
+    double j[4], n1, n2, w;
+    lin_h(G, r.c.z, r.c.w, j, n1, n2, w);
+    const double e00 = j[0] * b00 + j[1] * b10, e01 = j[0] * b01 + j[1] * b11, e10 = j[2] * b00 + j[3] * b10, e11 = j[2] * b01 + j[3] * b11;
+    const double i00 = a11 / det1, i01 = -a01 / det1, i10 = -a10 / det1, i11 = a00 / det1;
+    const double d00 = (i00 * e00 + i01 * e10) - 1.0, m01 = i00 * e01 + i01 * e11, m10 = i10 * e00 + i11 * e10;
+    const double d11 = (i10 * e01 + i11 * e11) - 1.0;
+    D = ((d00 * d00 + m01 * m01) + m10 * m10) + d11 * d11;
+    return true;
+}
+
+// Affine inlier: is_inlier(H) at the centres, finite non-singular frames and D <= laf_th (G = adj(H)).
+__device__ __forceinline__ bool is_inlier_ac(const double* H, const double* G, const AcRow& r, double th2, double laf_th) {
+    if (!is_inlier(H, r.c, th2)) return false;
+    double D;
+    return frame_distance(G, r, D) && D <= laf_th;
+}
+
+// Hypothesis from 2 affine correspondences, fp64 in this order; false for a degenerate sample.
+//  - Degenerate: a non-finite centre or frame, coincident centres in either image, det A1 or det A2 = 0, det(A2 A1^-1) of different
+//    signs for the two ACs (the counterpart of the 4-point mixed-orientation rule), a Cholesky pivot <= CHOL_EPS times its diagonal entry,
+//    or a non-finite H.
+//  - Each image's two centres are Hartley-normalised: midpoint c and scale s = sqrt(2 / var), var = (d / 2)^2 (refit's, for two points).
+//  - In normalised coordinates AC k gives A_n = (s2 / s1) A2 A1^-1 and 6 equations linear in (h11 .. h32) with h33 = 1: the 2 point
+//    equations and the 4 of dx'/dx = A_n, e.g. h11 - (u' + a11 u) h31 - a11 v h32 = a11.  Fixing h33 = 1 is safe: Hn[2][2] is the w of H
+//    at the image-1 midpoint, and w > 0 at both sample points (both visible under H) makes it positive at their midpoint.
+//  - The 12 x 8 system is solved by least squares: normal equations (upper triangle, accumulated row by row), Cholesky, forward and back
+//    substitution; then H = T2^-1 Hn T1 and normalise_h.
+__device__ bool ac_homography(const AcRow (&a)[2], double* H) {
+    double d1[2], d2[2];
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+        if (!finite4(a[k].c) || !finite4(a[k].a1) || !finite4(a[k].a2)) return false;
+        d1[k] = (double)a[k].a1.x * a[k].a1.w - (double)a[k].a1.y * a[k].a1.z;
+        d2[k] = (double)a[k].a2.x * a[k].a2.w - (double)a[k].a2.y * a[k].a2.z;
+        if (d1[k] == 0.0 || d2[k] == 0.0) return false;
+    }
+    if (((d1[0] > 0.0) == (d2[0] > 0.0)) != ((d1[1] > 0.0) == (d2[1] > 0.0))) return false;
+    const double c1x = ((double)a[0].c.x + a[1].c.x) * 0.5, c1y = ((double)a[0].c.y + a[1].c.y) * 0.5;
+    const double c2x = ((double)a[0].c.z + a[1].c.z) * 0.5, c2y = ((double)a[0].c.w + a[1].c.w) * 0.5;
+    const double h1x = ((double)a[1].c.x - a[0].c.x) * 0.5, h1y = ((double)a[1].c.y - a[0].c.y) * 0.5;
+    const double h2x = ((double)a[1].c.z - a[0].c.z) * 0.5, h2y = ((double)a[1].c.w - a[0].c.w) * 0.5;
+    const double var1 = h1x * h1x + h1y * h1y, var2 = h2x * h2x + h2y * h2y;
+    if (!(var1 > 0.0) || !(var2 > 0.0)) return false;
+    const double s1 = sqrt(2.0 / var1), s2 = sqrt(2.0 / var2), rs = s2 / s1;
+    double N[8][8], b[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        b[k] = 0.0;
+#pragma unroll
+        for (int l = 0; l < 8; l++) N[k][l] = 0.0;
+    }
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+        const double u = (a[k].c.x - c1x) * s1, v = (a[k].c.y - c1y) * s1, up = (a[k].c.z - c2x) * s2, vp = (a[k].c.w - c2y) * s2;
+        const double p00 = a[k].a1.x, p01 = a[k].a1.y, p10 = a[k].a1.z, p11 = a[k].a1.w;
+        const double q00 = a[k].a2.x, q01 = a[k].a2.y, q10 = a[k].a2.z, q11 = a[k].a2.w;
+        const double i00 = p11 / d1[k], i01 = -p01 / d1[k], i10 = -p10 / d1[k], i11 = p00 / d1[k];
+        const double n00 = (q00 * i00 + q01 * i10) * rs, n01 = (q00 * i01 + q01 * i11) * rs;
+        const double n10 = (q10 * i00 + q11 * i10) * rs, n11 = (q10 * i01 + q11 * i11) * rs;
+        const double rows[6][9] = {{u, v, 1.0, 0.0, 0.0, 0.0, -(up * u), -(up * v), up},
+                                   {0.0, 0.0, 0.0, u, v, 1.0, -(vp * u), -(vp * v), vp},
+                                   {1.0, 0.0, 0.0, 0.0, 0.0, 0.0, -(up + n00 * u), -(n00 * v), n00},
+                                   {0.0, 1.0, 0.0, 0.0, 0.0, 0.0, -(n01 * u), -(up + n01 * v), n01},
+                                   {0.0, 0.0, 0.0, 1.0, 0.0, 0.0, -(vp + n10 * u), -(n10 * v), n10},
+                                   {0.0, 0.0, 0.0, 0.0, 1.0, 0.0, -(n11 * u), -(vp + n11 * v), n11}};
+#pragma unroll
+        for (int e = 0; e < 6; e++)
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                b[i] = b[i] + rows[e][i] * rows[e][8];
+#pragma unroll
+                for (int l = i; l < 8; l++) N[i][l] = N[i][l] + rows[e][i] * rows[e][l];
+            }
+    }
+    // Cholesky N = L L' (L in the lower triangle of N; N's upper triangle stays), then L z = b and L' h = z
+    double dg[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        double d = N[j][j];
+#pragma unroll
+        for (int k = 0; k < j; k++) d = d - N[j][k] * N[j][k];
+        if (!(d > CHOL_EPS * N[j][j])) return false;
+        dg[j] = sqrt(d);
+#pragma unroll
+        for (int i = j + 1; i < 8; i++) {
+            double t = N[j][i];
+#pragma unroll
+            for (int k = 0; k < j; k++) t = t - N[i][k] * N[j][k];
+            N[i][j] = t / dg[j];
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        double t = b[i];
+#pragma unroll
+        for (int k = 0; k < i; k++) t = t - N[i][k] * b[k];
+        b[i] = t / dg[i];
+    }
+#pragma unroll
+    for (int i = 7; i >= 0; i--) {
+        double t = b[i];
+#pragma unroll
+        for (int k = i + 1; k < 8; k++) t = t - N[k][i] * b[k];
+        b[i] = t / dg[i];
+    }
+    const double Hn[9] = {b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7], 1.0};
+    const double T1[9] = {s1, 0.0, -(s1 * c1x), 0.0, s1, -(s1 * c1y), 0.0, 0.0, 1.0};
+    const double T2i[9] = {1.0 / s2, 0.0, c2x, 0.0, 1.0 / s2, c2y, 0.0, 0.0, 1.0};
+    double tmp[9];
+    mul3(T2i, Hn, tmp);
+    mul3(tmp, T1, H);
+    return normalise_h(H);
+}
+
+// The local optimisation of a chunk's winner (in s.H and Hl, shared) that raised the so-far-best count: the refit rounds on s.H, and
+// from Hl the shrinking-threshold refits (LO_FACTOR, LO_STEPS; stopping at fewer than 4 inliers or a failed refit) followed by the refit
+// rounds.  s.H ends as the second result when its count is higher, else the first.  `inl` is scratch.  Block-wide; returns the count.
+__device__ int ac_local_opt(const float* L1, const float* L2, const int* tent, int n, double th2, double laf_th, unsigned char* inl,
+                            double* Hl, RansacShared& s) {
+    const int c0 = refit_rounds<false, true>(L1, L2, tent, n, th2, inl, s.H, s, laf_th);
+    double f = LO_FACTOR;
+    for (int k = 0; k < LO_STEPS; k++) {
+        const int c = score_rows<false, true>(Hl, L1, L2, tent, n, th2 * (f * f), inl, s, laf_th * f);
+        if (c < 4 || !refit(L1, L2, tent, n, inl, c, s)) break;   // c is the block total: uniform
+        if (threadIdx.x < 9) Hl[threadIdx.x] = s.Hr[threadIdx.x];
+        __syncthreads();
+        f = f * 0.5;
+    }
+    const int c1 = refit_rounds<false, true>(L1, L2, tent, n, th2, inl, Hl, s, laf_th);
+    if (c1 <= c0) return c0;
+    if (threadIdx.x < 9) s.H[threadIdx.x] = Hl[threadIdx.x];
+    __syncthreads();
+    return c1;
+}
+
+// ransac_kernel's search with 2-AC samples and the affine inlier test, and ac_local_opt each time a chunk's winner raises the
+// so-far-best count.  Rows go through RansacShared's tile as AcRow, ATILE at a time.
+__global__ void __launch_bounds__(VT) ac_ransac_kernel(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2,
+                                                       int S2, int cap2, const int* __restrict__ pairs, const int* __restrict__ tent_all,
+                                                       const int* __restrict__ ntent, int tcap, double th2, double laf_th, double log1mconf,
+                                                       int max_iters, uint64_t seed, float* __restrict__ Hout, unsigned char* __restrict__ inl_all,
+                                                       int* __restrict__ ninl, int* __restrict__ iters) {
+    __shared__ RansacShared s;
+    __shared__ double Hl[9];   // ac_local_opt's second model
+    AcRow* tile = reinterpret_cast<AcRow*>(s.tile);
+    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int i, j;
+    const int n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
+    const int* tent = tent_all + (size_t)p * tcap * 2;
+    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
+        if (tid == 0) ninl[p] = -1;
+        return;
+    }
+    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
+    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
+    unsigned char* inl = inl_all + (size_t)p * tcap;
+    int best = 0, h_done = 0;
+    if (n >= 2) {
+        const int ntiles = (n + ATILE - 1) / ATILE;
+        for (int h0 = 0;; h0 += VT) {
+            const int h = h0 + tid;
+            double H[9], G[9];
+            bool ok = h < max_iters;
+            if (ok) {
+                int idx[2], got = 0;
+                for (int d = 0; d < MAX_DRAWS && got < 2; d++) {
+                    const int v = draw_index(seed, h, d, n);
+                    if (got == 0 || v != idx[0]) idx[got++] = v;
+                }
+                ok = got == 2;
+                if (ok) {
+                    const AcRow a[2] = {tent_ac(L1, L2, tent, idx[0]), tent_ac(L1, L2, tent, idx[1])};
+                    ok = ac_homography(a, H);
+                }
+                if (ok) adj3(H, G);
+            }
+            int cnt = 0;
+            for (int tb = 0; tb < ntiles; tb++) {
+                const int t0 = tb * ATILE, m = min(ATILE, n - t0);
+                if (ntiles > 1 || h0 == 0) {
+                    __syncthreads();
+                    for (int t = tid; t < m; t += VT) tile[t] = tent_ac(L1, L2, tent, t0 + t);
+                    __syncthreads();
+                }
+                if (ok)
+                    for (int t = 0; t < m; t++) cnt += is_inlier_ac(H, G, tile[t], th2, laf_th);
+            }
+            // best of the chunk: highest count, then lowest h
+            const unsigned long long mine = ok ? ((unsigned long long)cnt << 32) | (unsigned)~(unsigned)h : 0ull;
+            unsigned long long key = mine;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
+                key = k2 > key ? k2 : key;
+            }
+            if (lane == 0) s.key[warp] = key;
+            __syncthreads();
+            unsigned long long bk = 0;
+#pragma unroll
+            for (int w = 0; w < VT / 32; w++) bk = s.key[w] > bk ? s.key[w] : bk;
+            const int bc = (int)(bk >> 32);
+            if (bk != 0 && bc > best) {
+                if (mine == bk) {
+#pragma unroll
+                    for (int k = 0; k < 9; k++) s.H[k] = Hl[k] = H[k];
+                }
+                __syncthreads();
+                // local optimisation: a 2-AC hypothesis is noisier than a 4-point one; the point-DLT refits bring it to their accuracy
+                best = ac_local_opt(L1, L2, tent, n, th2, laf_th, inl, Hl, s);
+            }
+            h_done = min(h0 + VT, max_iters);
+            double need;   // adaptive number of samples for `confidence`
+            const double pr = (double)best / (double)n, p2 = pr * pr;
+            if (p2 >= 1.0) need = 0.0;
+            else if (p2 <= 0.0) need = INFINITY;
+            else need = ceil(log1mconf / log(1.0 - p2));
+            __syncthreads();
+            if ((double)h_done >= fmin(need, (double)max_iters)) break;
+        }
+    }
+    if (best > 0) best = refit_rounds<false, true>(L1, L2, tent, n, th2, inl, s.H, s, laf_th);
+    else
+        for (int t = tid; t < n; t += VT) inl[t] = 0;
+    if (tid < 9) Hout[(size_t)p * 9 + tid] = best > 0 ? (float)s.H[tid] : 0.f;
+    if (tid == 0) {
+        ninl[p] = best;
+        if (iters) iters[p] = h_done;
+    }
+}
+
 int verify_args(const char* fn, const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                 const int* d_tent, const int* d_ntent, int tcap) {
     const char* msg = nullptr;
@@ -1413,6 +1691,24 @@ int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_
     ransac_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
                                                       log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_H, d_inl, d_ninl, d_iters);
     AG_CHECK_LAUNCH("ransac_kernel");
+    return AG_OK;
+}
+
+int ag_homography_ransac_affine(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                                const int* d_tent, const int* d_ntent, int tcap, float inl_th, float laf_th, float confidence, int max_iters,
+                                unsigned long long seed, float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
+    int rc = verify_args("ag_homography_ransac_affine", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc) return rc;
+    AG_REQUIRE(d_H && d_inl && d_ninl, "NULL output");
+    AG_REQUIRE(inl_th > 0.f && isfinite(inl_th), "inl_th must be finite and > 0");
+    AG_REQUIRE(laf_th > 0.f, "laf_th must be > 0 (and not NaN)");
+    AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
+    AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
+    const double th = inl_th;
+    ac_ransac_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
+                                                         (double)laf_th, log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_H, d_inl,
+                                                         d_ninl, d_iters);
+    AG_CHECK_LAUNCH("ac_ransac_kernel");
     return AG_OK;
 }
 

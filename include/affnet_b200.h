@@ -389,6 +389,25 @@ int ag_match_pairs(const float* d_desc1, const int* d_count1, int S1, int cap1, 
  *   d_H [P,3,3] (H[2][2] = 1), d_inl [P,tcap] u8, d_ninl [P], d_iters [P] (hypotheses evaluated; may be NULL).  n < 4 tentatives or no
  *   hypothesis with an inlier: ninl = 0, H = 0, mask rows < n = 0.
  *   AG_ERR_INVALID also for inl_th not finite and > 0, confidence outside (0, 1), max_iters < 1.
+ * ag_homography_ransac_affine: ag_homography_ransac on affine correspondences (a tentative of two LAFs: its centres and the local affinity
+ * A2 A1^-1, A the LAF's 2x2 part), with the arguments, refusals, -1 rule, outputs, determinism and pair independence of
+ * ag_homography_ransac and one more argument, laf_th.  The frames must be oriented (OriNet or histogram orientation).
+ *   Sample: hypothesis h takes the first 2 distinct draws of the same sampler (at most 64 draws).
+ *   Solver, fp64 in a fixed order: each image's two centres are normalised by a similarity (midpoint, scale sqrt(2 / var), var = (d/2)^2);
+ *   each AC gives 2 point equations and 4 of dx'/dx = (s2 / s1) A2 A1^-1, linear in h11..h32 with h33 = 1; the 12 x 8 least-squares
+ *   system is solved through its normal equations by Cholesky, then denormalised and scaled to H[2][2] = 1.
+ *   Degenerate sample (evaluated, never a winner): a non-finite centre or frame, coincident centres in either image, det A1 or det A2 = 0,
+ *   det(A2 A1^-1) of different signs for the two ACs, a Cholesky pivot <= 1e-10 times its diagonal entry, or a non-finite H.
+ *   Inlier: ag_homography_ransac's test at the centres and D <= laf_th, D = |A1^-1 J A2 - I|_F^2 with J the Jacobian of H^-1 at the
+ *   image-2 centre (the reference's skip-centre Frobenius distance of the row's own pair, fp64); a row with a non-finite or singular
+ *   frame is never an inlier.  laf_th = +inf tests the centres and the frames' finiteness only.
+ *   Each time a chunk's winner raises the so-far-best count, before the stopping rule, it is refined twice and the better result kept
+ *   (the second only when its count is higher): (1) the refit rounds (point DLT on the inliers, each kept while the count under this test
+ *   does not drop); (2) point DLT on the inliers at 16, 8, 4, 2 and 1 times both thresholds (stopping at fewer than 4 inliers or a failed
+ *   refit; LO-RANSAC's iterative step), then the refit rounds.  Its count is the `best` of N = ceil(log(1 - confidence) /
+ *   log(1 - (best/n)^2)).  After the search, the refit rounds and outputs are ag_homography_ransac's; d_iters counts the 2-AC samples.
+ *   n < 2 tentatives or no hypothesis with an inlier: ninl = 0, H = 0, mask rows < n = 0.  d_inl is scratch during the search.
+ *   AG_ERR_INVALID also for laf_th NaN or <= 0.
  * ag_fundamental_ransac: fundamental-matrix RANSAC per pair (the notebook's alternative, findFundamentalMatrix(src, dst, 0.5)), for
  * scenes with depth, which one homography does not explain; the arguments, refusals and -1 rule of ag_homography_ransac.  Everything is
  * fp64 in a fixed operation order.  The centres of the rows whose four coordinates are finite are Hartley-normalised (centroid, scale
@@ -463,6 +482,9 @@ typedef struct {
 int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                          const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
                          float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
+int ag_homography_ransac_affine(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                                const int* d_tent, const int* d_ntent, int tcap, float inl_th, float laf_th, float confidence, int max_iters,
+                                unsigned long long seed, float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
 int ag_fundamental_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                           const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
                           float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream);
