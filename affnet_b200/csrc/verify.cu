@@ -14,6 +14,11 @@
 // -fmad=false (build.sh): numpy rounds every product and sum separately, so fused multiply-adds here would move near-threshold decisions.
 // The block reductions of the refit run in a fixed order (strided per-thread sums, an xor butterfly per warp, warps in ascending order)
 // that the restatement repeats.
+//
+// Each RANSAC kernel (ransac_kernel, fransac_kernel<DEGEN>, ac_ransac_kernel) keeps its own search loop: sample, solver, scoring over
+// the tile, chunk key and stopping rule.  The steps they share are one device function each: verify_pair (the pair's rows, or -1),
+// draw_sample (the first K distinct draws), block_max_key (the chunk's winner), hartley (normalisation statistics), denormalise_h /
+// denormalise_f, refit_rounds and finish_ransac (the refits and the result).
 #include "common.cuh"
 
 namespace ag {
@@ -24,6 +29,7 @@ constexpr int MAX_DRAWS = 64;        // draws per hypothesis before it is counte
 constexpr double COLLINEAR_EPS = 1e-6;   // |cross(b - a, c - a)| <= eps * (|dx1| + |dy1|) * (|dx2| + |dy2|): collinear
 constexpr int JACOBI_SWEEPS = 10;
 constexpr int REFIT_ROUNDS = 3;
+constexpr int F_REFIT_MIN = 8;       // inliers needed by the fundamental matrix's 8-point refit
 constexpr int MAX_TCAP = 4194240;    // ag_match_pairs' cap1 limit
 
 __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
@@ -37,6 +43,19 @@ __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
 __device__ __forceinline__ int draw_index(uint64_t seed, int h, int d, int n) {
     const uint64_t r = splitmix64(splitmix64(((uint64_t)(uint32_t)h << 32) | (uint32_t)d) ^ seed);
     return (int)(((r >> 32) * (uint64_t)(uint32_t)n) >> 32);
+}
+
+// The sample of hypothesis h: its first K distinct draws, in draw order.  False when MAX_DRAWS draws give fewer (a degenerate sample).
+template <int K>
+__device__ __forceinline__ bool draw_sample(uint64_t seed, int h, int n, int (&idx)[K]) {
+    int got = 0;
+    for (int d = 0; d < MAX_DRAWS && got < K; d++) {
+        const int v = draw_index(seed, h, d, n);
+        bool dup = false;
+        for (int q = 0; q < got; q++) dup |= idx[q] == v;
+        if (!dup) idx[got++] = v;
+    }
+    return got == K;
 }
 
 // Pair p = (i, j) -> n tentatives, or -1 when the pair cannot be verified (an image index out of range, ntent outside 0..tcap).
@@ -60,6 +79,43 @@ __device__ bool rows_in_range(const int* __restrict__ tent, int n, int cap1, int
     return !__syncthreads_or(bad);
 }
 
+// Pair blockIdx.x of a one-CTA-per-pair kernel: its n tentatives `tent` and the LAF sets L1, L2 they index.  False, after thread 0
+// has written -1 to flag[pair], when the pair cannot be verified (pair_tentatives, rows_in_range).  Block-wide.
+__device__ __forceinline__ bool verify_pair(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2, int S2,
+                                           int cap2, const int* __restrict__ pairs, const int* __restrict__ tent_all,
+                                           const int* __restrict__ ntent, int tcap, int* __restrict__ flag, int& n, const int*& tent,
+                                           const float*& L1, const float*& L2) {
+    const int p = blockIdx.x;
+    int i, j;
+    n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
+    tent = tent_all + (size_t)p * tcap * 2;
+    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
+        if (threadIdx.x == 0) flag[p] = -1;
+        return false;
+    }
+    L1 = lafs1 + (size_t)i * cap1 * 6;
+    L2 = lafs2 + (size_t)j * cap2 * 6;
+    return true;
+}
+
+// Ordered compaction of one block of VT rows: every thread whose row t is kept writes t to out[base + run + its rank among the kept
+// rows]; returns run plus the block's count.  Block-wide; wsum is VT / 32 shared ints, free again on return.
+__device__ __forceinline__ int compact_rows(bool keep, int t, int* __restrict__ out, size_t base, int run, int* wsum) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned b = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) wsum[warp] = __popc(b);
+    __syncthreads();
+    int off = run, tot = 0;
+#pragma unroll
+    for (int w = 0; w < VT / 32; w++) {
+        off += w < warp ? wsum[w] : 0;
+        tot += wsum[w];
+    }
+    if (keep) out[base + off + __popc(b & ((1u << lane) - 1u))] = t;
+    __syncthreads();   // wsum is rewritten by the next row block
+    return run + tot;
+}
+
 // Centres of tentative t: (x1, y1) in image 1, (x2, y2) in image 2 (the LAF's third column).
 __device__ __forceinline__ float4 tent_centres(const float* __restrict__ L1, const float* __restrict__ L2, const int* __restrict__ tent, int t) {
     const float* a = L1 + (size_t)tent[2 * (size_t)t] * 6;
@@ -76,6 +132,8 @@ __device__ __forceinline__ AcRow tent_ac(const float* __restrict__ L1, const flo
     const float* b = L2 + (size_t)tent[2 * (size_t)t + 1] * 6;
     return {make_float4(a[2], a[5], b[2], b[5]), make_float4(a[0], a[1], a[3], a[4]), make_float4(b[0], b[1], b[3], b[4])};
 }
+
+__device__ __forceinline__ bool finite4(float4 c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z) && isfinite(c.w); }
 
 // ---- fp64 3x3 helpers (row-major), in the restatement's operation order ------------------------------------------------------------
 __device__ __forceinline__ void adj3(const double* m, double* o) {
@@ -99,6 +157,21 @@ __device__ __forceinline__ bool normalise_h(double* H) {
         ok &= isfinite(H[k]);
     }
     return ok;
+}
+
+// Hartley normalisation x -> T x, T = [s 0 -s cx; 0 s -s cy; 0 0 1], of both images.
+struct Hartley {
+    double c1x, c1y, s1, c2x, c2y, s2;
+};
+
+// H = T2^-1 Hn T1, normalised by normalise_h.
+__device__ __forceinline__ bool denormalise_h(const Hartley& T, const double* Hn, double* H) {
+    const double T1[9] = {T.s1, 0.0, -(T.s1 * T.c1x), 0.0, T.s1, -(T.s1 * T.c1y), 0.0, 0.0, 1.0};
+    const double T2i[9] = {1.0 / T.s2, 0.0, T.c2x, 0.0, 1.0 / T.s2, T.c2y, 0.0, 0.0, 1.0};
+    double tmp[9];
+    mul3(T2i, Hn, tmp);
+    mul3(tmp, T1, H);
+    return normalise_h(H);
 }
 
 // Inlier test: positive denominator and squared forward error <= th2.
@@ -176,6 +249,23 @@ __device__ __forceinline__ void block_sum(double (&v)[K], double (*red)[K], doub
         out[threadIdx.x] = s;
     }
     __syncthreads();
+}
+
+// The largest of the threads' keys (0: none), valid for every thread: an xor butterfly per warp, one key per warp in red (VT / 32
+// shared entries), a barrier, then the maximum over the warps.  red may be written again only after the caller's next barrier.
+__device__ __forceinline__ unsigned long long block_max_key(unsigned long long key, unsigned long long* red) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
+        key = k2 > key ? k2 : key;
+    }
+    if (lane == 0) red[warp] = key;
+    __syncthreads();
+    unsigned long long bk = 0;
+#pragma unroll
+    for (int w = 0; w < VT / 32; w++) bk = red[w] > bk ? red[w] : bk;
+    return bk;
 }
 
 struct RansacShared {
@@ -259,6 +349,14 @@ __device__ __forceinline__ int smallest_diag(const double* A) {
     return m;
 }
 
+// v = the eigenvector of the smallest eigenvalue of the symmetric 3x3 G (jacobi3, which overwrites G).
+__device__ __forceinline__ void smallest_eigvec3(double* G, double (&v)[3]) {
+    double V[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+    jacobi3(G, V);
+    const int m = smallest_diag<3>(G);
+    v[0] = V[m]; v[1] = V[3 + m]; v[2] = V[6 + m];
+}
+
 // s.A = the symmetric 9x9 whose upper triangle is s.sums (row by row), s.V = I, then jacobi9_warp.  Block-wide.
 __device__ void normal_matrix_eigen(RansacShared& s) {
     if (threadIdx.x < 81) {
@@ -303,25 +401,37 @@ __device__ int score_rows(const double* H, const float* L1, const float* L2, con
     return tot;
 }
 
-// Normalised-DLT least squares on the rows of the mask `inl` (Hartley normalisation, 9x9 normal matrix, smallest eigenvector by
-// cyclic Jacobi on warp 0).  Writes s.Hr; false when the inliers do not determine a finite homography.
-__device__ bool refit(const float* L1, const float* L2, const int* tent, int n, const unsigned char* inl, int cnt, RansacShared& s) {
-    // centroids and mean squared radii of both point sets
-    double st[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+// Hartley normalisation of the rows in the mask `inl`, or, without a mask, of the rows whose four coordinates are finite: per image
+// the centroid c and s = sqrt(2 / var), var the mean squared distance to c.  The sums of x, y, x^2, y^2 per image and the row count
+// (exact: at most MAX_TCAP) go through one block_sum, which reduces each of them on its own; the count into *nrows when given.
+// Block-wide; false, on every thread, unless var > 0 in both images.
+__device__ __forceinline__ bool hartley(const float* L1, const float* L2, const int* tent, int n, const unsigned char* inl, RansacShared& s,
+                                        Hartley& T, double* nrows = nullptr) {
+    double st[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int t = threadIdx.x; t < n; t += VT) {
         const float4 c = tent_centres(L1, L2, tent, t);
-        const bool in = inl[t];
+        const bool in = inl ? inl[t] != 0 : finite4(c);
         const double x1 = in ? (double)c.x : 0.0, y1 = in ? (double)c.y : 0.0, x2 = in ? (double)c.z : 0.0, y2 = in ? (double)c.w : 0.0;
         st[0] = st[0] + x1; st[1] = st[1] + y1; st[2] = st[2] + x1 * x1; st[3] = st[3] + y1 * y1;
         st[4] = st[4] + x2; st[5] = st[5] + y2; st[6] = st[6] + x2 * x2; st[7] = st[7] + y2 * y2;
+        st[8] = st[8] + (in ? 1.0 : 0.0);
     }
-    block_sum<8>(st, reinterpret_cast<double(*)[8]>(&s.red[0][0]), s.sums);
-    const double nd = (double)cnt;
-    const double c1x = s.sums[0] / nd, c1y = s.sums[1] / nd, c2x = s.sums[4] / nd, c2y = s.sums[5] / nd;
-    const double var1 = (s.sums[2] + s.sums[3]) / nd - (c1x * c1x + c1y * c1y);
-    const double var2 = (s.sums[6] + s.sums[7]) / nd - (c2x * c2x + c2y * c2y);
-    if (!(var1 > 0.0) || !(var2 > 0.0)) return false;   // uniform across the block: every thread returns
-    const double s1 = sqrt(2.0 / var1), s2 = sqrt(2.0 / var2);
+    block_sum<9>(st, reinterpret_cast<double(*)[9]>(&s.red[0][0]), s.sums);
+    const double nd = s.sums[8];
+    if (nrows) *nrows = nd;
+    T.c1x = s.sums[0] / nd; T.c1y = s.sums[1] / nd; T.c2x = s.sums[4] / nd; T.c2y = s.sums[5] / nd;
+    const double var1 = (s.sums[2] + s.sums[3]) / nd - (T.c1x * T.c1x + T.c1y * T.c1y);
+    const double var2 = (s.sums[6] + s.sums[7]) / nd - (T.c2x * T.c2x + T.c2y * T.c2y);
+    T.s1 = sqrt(2.0 / var1);
+    T.s2 = sqrt(2.0 / var2);
+    return var1 > 0.0 && var2 > 0.0;
+}
+
+// Normalised-DLT least squares on the rows of the mask `inl` (Hartley normalisation, 9x9 normal matrix, smallest eigenvector by
+// cyclic Jacobi on warp 0).  Writes s.Hr; false when the inliers do not determine a finite homography.
+__device__ bool refit(const float* L1, const float* L2, const int* tent, int n, const unsigned char* inl, RansacShared& s) {
+    Hartley T;
+    if (!hartley(L1, L2, tent, n, inl, s, T)) return false;   // uniform across the block: every thread returns
     // normal matrix: upper triangle, row by row
     double nm[45];
 #pragma unroll
@@ -329,7 +439,7 @@ __device__ bool refit(const float* L1, const float* L2, const int* tent, int n, 
     for (int t = threadIdx.x; t < n; t += VT) {
         const float4 c = tent_centres(L1, L2, tent, t);
         const bool in = inl[t];
-        const double u = (c.x - c1x) * s1, v = (c.y - c1y) * s1, up = (c.z - c2x) * s2, vp = (c.w - c2y) * s2;
+        const double u = (c.x - T.c1x) * T.s1, v = (c.y - T.c1y) * T.s1, up = (c.z - T.c2x) * T.s2, vp = (c.w - T.c2y) * T.s2;
         const double a1[9] = {-u, -v, -1.0, 0.0, 0.0, 0.0, up * u, up * v, up};
         const double a2[9] = {0.0, 0.0, 0.0, -u, -v, -1.0, vp * u, vp * v, vp};
         int e = 0;
@@ -342,16 +452,52 @@ __device__ bool refit(const float* L1, const float* L2, const int* tent, int n, 
     normal_matrix_eigen(s);
     if (threadIdx.x == 0) {
         const int m = smallest_diag<9>(s.A);
-        double Hn[9], tmp[9];
+        double Hn[9];
         for (int e = 0; e < 9; e++) Hn[e] = s.V[9 * e + m];
-        const double T1[9] = {s1, 0.0, -(s1 * c1x), 0.0, s1, -(s1 * c1y), 0.0, 0.0, 1.0};
-        const double T2i[9] = {1.0 / s2, 0.0, c2x, 0.0, 1.0 / s2, c2y, 0.0, 0.0, 1.0};
-        mul3(T2i, Hn, tmp);
-        mul3(tmp, T1, s.Hr);
-        s.bad = !normalise_h(s.Hr);
+        s.bad = !denormalise_h(T, Hn, s.Hr);
     }
     __syncthreads();
     return !s.bad;
+}
+
+__device__ bool refit_f(const float* L1, const float* L2, const int* tent, int n, const unsigned char* inl, RansacShared& s);
+
+// Up to REFIT_ROUNDS least-squares refits of the model M (shared; a homography, or a fundamental matrix when FUND) on its inliers at
+// th2, each kept only if the inlier count does not drop: the rounds that end every RANSAC kernel, for DEGENSAC's plane H and its local
+// optimisation, and (AFF: the inliers also pass the frame test at laf_th; the refit is the same point DLT) for the affine homography
+// RANSAC's.  Block-wide; on return M is the last kept model and `inl` its mask (rows < n).
+// Returns its inlier count.
+template <bool FUND, bool AFF = false>
+__device__ __forceinline__ int refit_rounds(const float* L1, const float* L2, const int* tent, int n, double th2, unsigned char* inl,
+                                            double* M, RansacShared& s, double laf_th = 0.0) {
+    int cnt = score_rows<FUND, AFF>(M, L1, L2, tent, n, th2, inl, s, laf_th);
+    for (int r = 0; r < REFIT_ROUNDS && cnt >= (FUND ? F_REFIT_MIN : 4); r++) {
+        if (!(FUND ? refit_f(L1, L2, tent, n, inl, s) : refit(L1, L2, tent, n, inl, s))) break;
+        const int c2 = score_rows<FUND, AFF>(s.Hr, L1, L2, tent, n, th2, nullptr, s, laf_th);
+        if (c2 < cnt) break;
+        cnt = c2;
+        if (threadIdx.x < 9) M[threadIdx.x] = s.Hr[threadIdx.x];
+        __syncthreads();
+        score_rows<FUND, AFF>(M, L1, L2, tent, n, th2, inl, s, laf_th);
+    }
+    return cnt;
+}
+
+// The end of a RANSAC kernel for pair blockIdx.x: the refit rounds on the search's winner s.H when it has `best` > 0 inliers (else an
+// all-zero mask), then the model (zero when nothing was found), its inlier count and the number of hypotheses evaluated.  Block-wide.
+template <bool FUND, bool AFF = false>
+__device__ __forceinline__ void finish_ransac(const float* L1, const float* L2, const int* tent, int n, double th2, int best, int h_done,
+                                              unsigned char* inl, RansacShared& s, float* __restrict__ Mout, int* __restrict__ ninl,
+                                              int* __restrict__ iters, double laf_th = 0.0) {
+    const int p = blockIdx.x, tid = threadIdx.x;
+    if (best > 0) best = refit_rounds<FUND, AFF>(L1, L2, tent, n, th2, inl, s.H, s, laf_th);
+    else
+        for (int t = tid; t < n; t += VT) inl[t] = 0;
+    if (tid < 9) Mout[(size_t)p * 9 + tid] = best > 0 ? (float)s.H[tid] : 0.f;
+    if (tid == 0) {
+        ninl[p] = best;
+        if (iters) iters[p] = h_done;
+    }
 }
 
 __global__ void __launch_bounds__(VT) ransac_kernel(const float* __restrict__ lafs1, int S1, int cap1, const float* __restrict__ lafs2, int S2,
@@ -360,39 +506,25 @@ __global__ void __launch_bounds__(VT) ransac_kernel(const float* __restrict__ la
                                                     uint64_t seed, float* __restrict__ Hout, unsigned char* __restrict__ inl_all,
                                                     int* __restrict__ ninl, int* __restrict__ iters) {
     __shared__ RansacShared s;
-    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    int i, j;
-    const int n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
-    const int* tent = tent_all + (size_t)p * tcap * 2;
-    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
-        if (tid == 0) ninl[p] = -1;
-        return;
-    }
-    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
-    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
-    unsigned char* inl = inl_all + (size_t)p * tcap;
+    const int tid = threadIdx.x;
+    const int* tent;
+    const float *L1, *L2;
+    int n;
+    if (!verify_pair(lafs1, S1, cap1, lafs2, S2, cap2, pairs, tent_all, ntent, tcap, ninl, n, tent, L1, L2)) return;
+    unsigned char* inl = inl_all + (size_t)blockIdx.x * tcap;
     int best = 0, h_done = 0;
     if (n >= 4) {
         const int ntiles = (n + VTILE - 1) / VTILE;
         for (int h0 = 0;; h0 += VT) {
             const int h = h0 + tid;
             double H[9];
-            bool ok = h < max_iters;
+            int idx[4];
+            bool ok = h < max_iters && draw_sample(seed, h, n, idx);
             if (ok) {
-                int idx[4], got = 0;
-                for (int d = 0; d < MAX_DRAWS && got < 4; d++) {
-                    const int v = draw_index(seed, h, d, n);
-                    bool dup = false;
-                    for (int q = 0; q < got; q++) dup |= idx[q] == v;
-                    if (!dup) idx[got++] = v;
-                }
-                ok = got == 4;
-                if (ok) {
-                    float4 c[4];
+                float4 c[4];
 #pragma unroll
-                    for (int q = 0; q < 4; q++) c[q] = tent_centres(L1, L2, tent, idx[q]);
-                    ok = minimal_homography(c, H);
-                }
+                for (int q = 0; q < 4; q++) c[q] = tent_centres(L1, L2, tent, idx[q]);
+                ok = minimal_homography(c, H);
             }
             int cnt = 0;
             for (int tb = 0; tb < ntiles; tb++) {
@@ -407,17 +539,7 @@ __global__ void __launch_bounds__(VT) ransac_kernel(const float* __restrict__ la
             }
             // best of the chunk: highest count, then lowest h
             const unsigned long long mine = ok ? ((unsigned long long)cnt << 32) | (unsigned)~(unsigned)h : 0ull;
-            unsigned long long key = mine;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const unsigned long long ok2 = __shfl_xor_sync(0xffffffffu, key, o);
-                key = ok2 > key ? ok2 : key;
-            }
-            if (lane == 0) s.key[warp] = key;
-            __syncthreads();
-            unsigned long long bk = 0;
-#pragma unroll
-            for (int w = 0; w < VT / 32; w++) bk = s.key[w] > bk ? s.key[w] : bk;
+            const unsigned long long bk = block_max_key(mine, s.key);
             const int bc = (int)(bk >> 32);
             if (bk != 0 && bc > best) {
                 if (mine == bk) {
@@ -436,26 +558,7 @@ __global__ void __launch_bounds__(VT) ransac_kernel(const float* __restrict__ la
             if ((double)h_done >= fmin(need, (double)max_iters)) break;
         }
     }
-    if (best > 0) {
-        int cnt = score_rows(s.H, L1, L2, tent, n, th2, inl, s);   // = best
-        for (int r = 0; r < REFIT_ROUNDS && cnt >= 4; r++) {
-            if (!refit(L1, L2, tent, n, inl, cnt, s)) break;
-            const int c2 = score_rows(s.Hr, L1, L2, tent, n, th2, nullptr, s);
-            if (c2 < cnt) break;
-            cnt = c2;
-            if (tid < 9) s.H[tid] = s.Hr[tid];
-            __syncthreads();
-            score_rows(s.H, L1, L2, tent, n, th2, inl, s);
-        }
-        best = cnt;
-    } else {
-        for (int t = tid; t < n; t += VT) inl[t] = 0;
-    }
-    if (tid < 9) Hout[(size_t)p * 9 + tid] = best > 0 ? (float)s.H[tid] : 0.f;
-    if (tid == 0) {
-        ninl[p] = best;
-        if (iters) iters[p] = h_done;
-    }
+    finish_ransac<false>(L1, L2, tent, n, th2, best, h_done, inl, s, Hout, ninl, iters);
 }
 
 // ---- ground-truth check (ReprojectionStuff.py:126-137) ----------------------------------------------------------------------------
@@ -485,16 +588,11 @@ __global__ void __launch_bounds__(VT) gt_kernel(const float* __restrict__ lafs1,
     __shared__ float4 tile[GT_TILE];   // (x, y, |x|^2, -) of the image-2 centres mapped into image 1
     __shared__ double Hi[9];
     __shared__ int wsum[VT / 32];
-    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    int i, j;
-    const int n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
-    const int* tent = tent_all + (size_t)p * tcap * 2;
-    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
-        if (tid == 0) ntrue[p] = -1;
-        return;
-    }
-    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
-    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
+    const int p = blockIdx.x, tid = threadIdx.x;
+    const int* tent;
+    const float *L1, *L2;
+    int n;
+    if (!verify_pair(lafs1, S1, cap1, lafs2, S2, cap2, pairs, tent_all, ntent, tcap, ntrue, n, tent, L1, L2)) return;
     if (tid == 0) inverse_h(H1to2 + (size_t)p * 9, Hi);
     __syncthreads();
     const size_t base = (size_t)p * tcap;
@@ -526,18 +624,7 @@ __global__ void __launch_bounds__(VT) gt_kernel(const float* __restrict__ lafs1,
         }
         const bool keep = t < n && best <= th;
         if (t < n) { min_dist[base + t] = best; idx2[base + t] = bi; }
-        const unsigned b = __ballot_sync(0xffffffffu, keep);
-        if (lane == 0) wsum[warp] = __popc(b);
-        __syncthreads();
-        int off = run, tot = 0;
-#pragma unroll
-        for (int w = 0; w < VT / 32; w++) {
-            off += w < warp ? wsum[w] : 0;
-            tot += wsum[w];
-        }
-        if (keep) true_all[base + off + __popc(b & ((1u << lane) - 1u))] = t;
-        run += tot;
-        __syncthreads();   // wsum is rewritten by the next row block
+        run = compact_rows(keep, t, true_all, base, run, wsum);
     }
     if (tid == 0) ntrue[p] = run;
 }
@@ -750,7 +837,7 @@ __global__ void __launch_bounds__(VT) frob_compact_kernel(int S1, int cap1, int 
                                                           const int* __restrict__ cnt2, int rcap, float th, const float* __restrict__ min_dist,
                                                           int* __restrict__ true_all, int* __restrict__ ntrue) {
     __shared__ int wsum[VT / 32];
-    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int p = blockIdx.x, tid = threadIdx.x;
     int i, j, n1, n2;
     bool ok = frob_pair<TENT>(pairs, p, S1, cap1, S2, cap2, cnt1, cnt2, rcap, i, j, n1, n2);
     if (TENT && ok) ok = rows_in_range(tent_all + (size_t)p * rcap * 2, n1, cap1, cap2);
@@ -763,18 +850,7 @@ __global__ void __launch_bounds__(VT) frob_compact_kernel(int S1, int cap1, int 
     for (int r0 = 0; r0 < n1; r0 += VT) {
         const int t = r0 + tid;
         const bool keep = t < n1 && min_dist[base + t] <= th;
-        const unsigned b = __ballot_sync(0xffffffffu, keep);
-        if (lane == 0) wsum[warp] = __popc(b);
-        __syncthreads();
-        int off = run, tot = 0;
-#pragma unroll
-        for (int w = 0; w < VT / 32; w++) {
-            off += w < warp ? wsum[w] : 0;
-            tot += wsum[w];
-        }
-        if (keep) true_all[base + off + __popc(b & ((1u << lane) - 1u))] = t;
-        run += tot;
-        __syncthreads();   // wsum is rewritten by the next row block
+        run = compact_rows(keep, t, true_all, base, run, wsum);
     }
     if (tid == 0) ntrue[p] = run;
 }
@@ -798,7 +874,6 @@ __global__ void reproject_lafs_kernel(const float* __restrict__ lafs, int cap, c
 
 // ---- fundamental-matrix RANSAC (the notebook's alternative line, findFundamentalMatrix(src, dst, 0.5)) ----------------------------
 constexpr int F_SAMPLE = 7;            // correspondences per hypothesis
-constexpr int F_REFIT_MIN = 8;         // inliers needed by the 8-point refit
 constexpr double PIVOT_EPS = 1e-9;     // 7-point elimination: a column whose largest candidate |pivot| <= PIVOT_EPS * max|A| is free
 constexpr int BISECT_STEPS = 1100;     // bisection cap per bracketed cubic root: enough to close any bracket in the double range
 
@@ -826,11 +901,6 @@ __device__ __forceinline__ bool normalise_f(double* F) {
     for (int k = 0; k < 9; k++) F[k] = F[k] / nr;
     return true;
 }
-
-// Hartley normalisation x -> T x, T = [s 0 -s cx; 0 s -s cy; 0 0 1], of both images.
-struct Hartley {
-    double c1x, c1y, s1, c2x, c2y, s2;
-};
 
 // F = T2' Fn T1, normalised by normalise_f.
 __device__ __forceinline__ bool denormalise_f(const Hartley& T, const double* Fn, double* F) {
@@ -1009,13 +1079,11 @@ __device__ __forceinline__ int seven_point(const double (&u)[F_SAMPLE][4], doubl
 // denormalised.  Thread 0.
 __device__ bool rank2_refit_f(const RansacShared& s, const Hartley& T, double* F) {
     const int m = smallest_diag<9>(s.A);
-    double Fn[9], G[9], V[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0}, P[9], Fr[9];
+    double Fn[9], G[9], v[3], P[9], Fr[9];
     for (int e = 0; e < 9; e++) Fn[e] = s.V[9 * e + m];
     for (int r = 0; r < 3; r++)
         for (int c = 0; c < 3; c++) G[3 * r + c] = Fn[r] * Fn[c] + Fn[3 + r] * Fn[3 + c] + Fn[6 + r] * Fn[6 + c];
-    jacobi3(G, V);
-    const int m3 = smallest_diag<3>(G);
-    const double v[3] = {V[m3], V[3 + m3], V[6 + m3]};
+    smallest_eigvec3(G, v);
     for (int r = 0; r < 3; r++)
         for (int c = 0; c < 3; c++) P[3 * r + c] = (r == c ? 1.0 : 0.0) - v[r] * v[c];
     mul3(Fn, P, Fr);
@@ -1025,24 +1093,9 @@ __device__ bool rank2_refit_f(const RansacShared& s, const Hartley& T, double* F
 // Normalised 8-point least squares on the rows of the mask `inl` (Hartley normalisation of those rows, the 9x9 normal matrix of the
 // constraint rows reduced in the fixed order, its smallest eigenvector, rank 2).  Writes s.Hr; false when the inliers do not give a
 // finite non-zero F.
-__device__ bool refit_f(const float* L1, const float* L2, const int* tent, int n, const unsigned char* inl, int cnt, RansacShared& s) {
-    double st[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int t = threadIdx.x; t < n; t += VT) {
-        const float4 c = tent_centres(L1, L2, tent, t);
-        const bool in = inl[t];
-        const double x1 = in ? (double)c.x : 0.0, y1 = in ? (double)c.y : 0.0, x2 = in ? (double)c.z : 0.0, y2 = in ? (double)c.w : 0.0;
-        st[0] = st[0] + x1; st[1] = st[1] + y1; st[2] = st[2] + x1 * x1; st[3] = st[3] + y1 * y1;
-        st[4] = st[4] + x2; st[5] = st[5] + y2; st[6] = st[6] + x2 * x2; st[7] = st[7] + y2 * y2;
-    }
-    block_sum<8>(st, reinterpret_cast<double(*)[8]>(&s.red[0][0]), s.sums);
-    const double nd = (double)cnt;
+__device__ bool refit_f(const float* L1, const float* L2, const int* tent, int n, const unsigned char* inl, RansacShared& s) {
     Hartley T;
-    T.c1x = s.sums[0] / nd; T.c1y = s.sums[1] / nd; T.c2x = s.sums[4] / nd; T.c2y = s.sums[5] / nd;
-    const double var1 = (s.sums[2] + s.sums[3]) / nd - (T.c1x * T.c1x + T.c1y * T.c1y);
-    const double var2 = (s.sums[6] + s.sums[7]) / nd - (T.c2x * T.c2x + T.c2y * T.c2y);
-    if (!(var1 > 0.0) || !(var2 > 0.0)) return false;   // uniform across the block: every thread returns
-    T.s1 = sqrt(2.0 / var1);
-    T.s2 = sqrt(2.0 / var2);
+    if (!hartley(L1, L2, tent, n, inl, s, T)) return false;   // uniform across the block: every thread returns
     double nm[45];
 #pragma unroll
     for (int k = 0; k < 45; k++) nm[k] = 0.0;
@@ -1063,29 +1116,6 @@ __device__ bool refit_f(const float* L1, const float* L2, const int* tent, int n
     __syncthreads();
     return !s.bad;
 }
-
-// Up to REFIT_ROUNDS least-squares refits of the model M (shared; a homography, or a fundamental matrix when FUND) on its inliers at
-// th2, each kept only if the inlier count does not drop: the rounds that end both kernels, for DEGENSAC's plane H and its local
-// optimisation, and (AFF: the inliers also pass the frame test at laf_th; the refit is the same point DLT) for the affine homography
-// RANSAC's.  Block-wide; on return M is the last kept model and `inl` its mask (rows < n).
-// Returns its inlier count.
-template <bool FUND, bool AFF = false>
-__device__ __forceinline__ int refit_rounds(const float* L1, const float* L2, const int* tent, int n, double th2, unsigned char* inl,
-                                            double* M, RansacShared& s, double laf_th = 0.0) {
-    int cnt = score_rows<FUND, AFF>(M, L1, L2, tent, n, th2, inl, s, laf_th);
-    for (int r = 0; r < REFIT_ROUNDS && cnt >= (FUND ? F_REFIT_MIN : 4); r++) {
-        if (!(FUND ? refit_f(L1, L2, tent, n, inl, cnt, s) : refit(L1, L2, tent, n, inl, cnt, s))) break;
-        const int c2 = score_rows<FUND, AFF>(s.Hr, L1, L2, tent, n, th2, nullptr, s, laf_th);
-        if (c2 < cnt) break;
-        cnt = c2;
-        if (threadIdx.x < 9) M[threadIdx.x] = s.Hr[threadIdx.x];
-        __syncthreads();
-        score_rows<FUND, AFF>(M, L1, L2, tent, n, th2, inl, s, laf_th);
-    }
-    return cnt;
-}
-
-__device__ __forceinline__ bool finite4(float4 c) { return isfinite(c.x) && isfinite(c.y) && isfinite(c.z) && isfinite(c.w); }
 
 // ---- DEGENSAC (Chum, Werner and Matas, CVPR 2005): degeneracy test, plane-and-parallax, local optimisation ------------------------
 constexpr double DEG_H_TH_FACTOR = 4.0;   // DEG_H_TH = DEG_H_TH_FACTOR * inl_th: a point agrees with a plane H within it (transfer, px)
@@ -1141,12 +1171,10 @@ __device__ bool triplet_homography(const double* A, const double* e, const float
 // and for each of the five triplets of Chum et al. the H of triplet_homography.  Returns the most sample points that one H agrees with
 // (is_inlier at thd2), that H (the lowest triplet on ties) in Hd.  One thread.
 __device__ int degeneracy_test(const double* F, const float4 (&c)[F_SAMPLE], double thd2, double* Hd) {
-    double G[9], V[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+    double G[9], e[3];
     for (int r = 0; r < 3; r++)
         for (int k = 0; k < 3; k++) G[3 * r + k] = F[3 * r] * F[3 * k] + F[3 * r + 1] * F[3 * k + 1] + F[3 * r + 2] * F[3 * k + 2];
-    jacobi3(G, V);
-    const int m = smallest_diag<3>(G);
-    const double e[3] = {V[m], V[3 + m], V[6 + m]};
+    smallest_eigvec3(G, e);
     double A[9];
     skew_mul(e, F, A);
     int best = 0;
@@ -1179,16 +1207,11 @@ struct DegenShared {
 __device__ __noinline__ int degensac_step(const float* L1, const float* L2, const int* tent, int n, int ntiles, double th2, uint64_t seed,
                                           int h, int k, unsigned char* inl, int best, RansacShared& s) {
     __shared__ DegenShared d;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const double thd2 = (DEG_H_TH_FACTOR * DEG_H_TH_FACTOR) * th2;
     if (tid == 0) {
-        int idx[F_SAMPLE], got = 0;
-        for (int dr = 0; dr < MAX_DRAWS && got < F_SAMPLE; dr++) {
-            const int v = draw_index(seed, h, dr, n);
-            bool dup = false;
-            for (int q = 0; q < got; q++) dup |= idx[q] == v;
-            if (!dup) idx[got++] = v;
-        }
+        int idx[F_SAMPLE];
+        draw_sample(seed, h, n, idx);   // the winner's sample: complete, since it gave a model
         float4 c[F_SAMPLE];
         for (int q = 0; q < F_SAMPLE; q++) c[q] = tent_centres(L1, L2, tent, idx[q]);
         d.agree = degeneracy_test(s.H, c, thd2, d.Hd);
@@ -1234,17 +1257,7 @@ __device__ __noinline__ int degensac_step(const float* L1, const float* L2, cons
                 for (int t = 0; t < m; t++) cnt += is_inlier_f(F, s.tile[t], th2);
         }
         const unsigned long long mine = ok ? ((unsigned long long)cnt << 32) | (unsigned)~(unsigned)tid : 0ull;
-        unsigned long long key = mine;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
-            key = k2 > key ? k2 : key;
-        }
-        if (lane == 0) d.key[warp] = key;
-        __syncthreads();
-        unsigned long long bk = 0;
-#pragma unroll
-        for (int w = 0; w < VT / 32; w++) bk = d.key[w] > bk ? d.key[w] : bk;
+        const unsigned long long bk = block_max_key(mine, d.key);
         const int bc = (int)(bk >> 32);
         if (bk != 0 && bc > best) {
             if (mine == bk)
@@ -1264,68 +1277,41 @@ __global__ void __launch_bounds__(VT) fransac_kernel(const float* __restrict__ l
                                                      uint64_t seed, float* __restrict__ Fout, unsigned char* __restrict__ inl_all,
                                                      int* __restrict__ ninl, int* __restrict__ iters) {
     __shared__ RansacShared s;
-    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    int i, j;
-    const int n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
-    const int* tent = tent_all + (size_t)p * tcap * 2;
-    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
-        if (tid == 0) ninl[p] = -1;
-        return;
-    }
-    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
-    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
-    unsigned char* inl = inl_all + (size_t)p * tcap;
+    const int tid = threadIdx.x;
+    const int* tent;
+    const float *L1, *L2;
+    int n;
+    if (!verify_pair(lafs1, S1, cap1, lafs2, S2, cap2, pairs, tent_all, ntent, tcap, ninl, n, tent, L1, L2)) return;
+    unsigned char* inl = inl_all + (size_t)blockIdx.x * tcap;
     int best = 0, h_done = 0;
     if (n >= F_SAMPLE) {
-        // Hartley normalisation of the rows whose four coordinates are finite (their number in st[8])
-        double st[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-        for (int t = tid; t < n; t += VT) {
-            const float4 c = tent_centres(L1, L2, tent, t);
-            const bool in = finite4(c);
-            const double x1 = in ? (double)c.x : 0.0, y1 = in ? (double)c.y : 0.0, x2 = in ? (double)c.z : 0.0, y2 = in ? (double)c.w : 0.0;
-            st[0] = st[0] + x1; st[1] = st[1] + y1; st[2] = st[2] + x1 * x1; st[3] = st[3] + y1 * y1;
-            st[4] = st[4] + x2; st[5] = st[5] + y2; st[6] = st[6] + x2 * x2; st[7] = st[7] + y2 * y2;
-            st[8] = st[8] + (in ? 1.0 : 0.0);
-        }
-        block_sum<9>(st, reinterpret_cast<double(*)[9]>(&s.red[0][0]), s.sums);
-        const double nd = s.sums[8];
+        // Hartley normalisation of the rows whose four coordinates are finite
         Hartley T;
-        T.c1x = s.sums[0] / nd; T.c1y = s.sums[1] / nd; T.c2x = s.sums[4] / nd; T.c2y = s.sums[5] / nd;
-        const double var1 = (s.sums[2] + s.sums[3]) / nd - (T.c1x * T.c1x + T.c1y * T.c1y);
-        const double var2 = (s.sums[6] + s.sums[7]) / nd - (T.c2x * T.c2x + T.c2y * T.c2y);
-        T.s1 = sqrt(2.0 / var1);
-        T.s2 = sqrt(2.0 / var2);
+        double nd;
+        const bool spread = hartley(L1, L2, tent, n, nullptr, s, T, &nd);
         // fewer than 7 finite rows, or all of them on one point in an image: no hypothesis is drawn (iters = 0)
-        const bool search = nd >= (double)F_SAMPLE && var1 > 0.0 && var2 > 0.0;
+        const bool search = nd >= (double)F_SAMPLE && spread;
         const int ntiles = (n + VTILE - 1) / VTILE;
         int ntests = 0;   // DEGEN: degeneracy tests so far
         for (int h0 = 0; search; h0 += VT) {
             const int h = h0 + tid;
             double Fm[3][9];
             bool okm[3] = {false, false, false};   // model r (root r in ascending order) exists
-            if (h < max_iters) {
-                int idx[F_SAMPLE], got = 0;
-                for (int d = 0; d < MAX_DRAWS && got < F_SAMPLE; d++) {
-                    const int v = draw_index(seed, h, d, n);
-                    bool dup = false;
-                    for (int q = 0; q < got; q++) dup |= idx[q] == v;
-                    if (!dup) idx[got++] = v;
+            int idx[F_SAMPLE];
+            if (h < max_iters && draw_sample(seed, h, n, idx)) {
+                double u[F_SAMPLE][4];
+                bool fin = true;
+                for (int q = 0; q < F_SAMPLE; q++) {
+                    const float4 c = tent_centres(L1, L2, tent, idx[q]);
+                    fin &= finite4(c);
+                    u[q][0] = (c.x - T.c1x) * T.s1; u[q][1] = (c.y - T.c1y) * T.s1;
+                    u[q][2] = (c.z - T.c2x) * T.s2; u[q][3] = (c.w - T.c2y) * T.s2;
                 }
-                if (got == F_SAMPLE) {
-                    double u[F_SAMPLE][4];
-                    bool fin = true;
-                    for (int q = 0; q < F_SAMPLE; q++) {
-                        const float4 c = tent_centres(L1, L2, tent, idx[q]);
-                        fin &= finite4(c);
-                        u[q][0] = (c.x - T.c1x) * T.s1; u[q][1] = (c.y - T.c1y) * T.s1;
-                        u[q][2] = (c.z - T.c2x) * T.s2; u[q][3] = (c.w - T.c2y) * T.s2;
-                    }
-                    double Fn[3][9];
-                    const int nl = fin ? seven_point(u, Fn) : 0;
+                double Fn[3][9];
+                const int nl = fin ? seven_point(u, Fn) : 0;
 #pragma unroll
-                    for (int r = 0; r < 3; r++)
-                        if (r < nl) okm[r] = denormalise_f(T, Fn[r], Fm[r]);
-                }
+                for (int r = 0; r < 3; r++)
+                    if (r < nl) okm[r] = denormalise_f(T, Fn[r], Fm[r]);
             }
             const bool any = okm[0] || okm[1] || okm[2];
             int cnt[3] = {0, 0, 0};
@@ -1351,17 +1337,7 @@ __global__ void __launch_bounds__(VT) fransac_kernel(const float* __restrict__ l
                 if (okm[r] && cnt[r] > cb) { cb = cnt[r]; rb = r; }
             const unsigned long long mine =
                 any ? ((unsigned long long)cb << 34) | ((unsigned long long)(0x7fffffff - h) << 2) | (unsigned long long)(3 - rb) : 0ull;
-            unsigned long long key = mine;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
-                key = k2 > key ? k2 : key;
-            }
-            if (lane == 0) s.key[warp] = key;
-            __syncthreads();
-            unsigned long long bk = 0;
-#pragma unroll
-            for (int w = 0; w < VT / 32; w++) bk = s.key[w] > bk ? s.key[w] : bk;
+            const unsigned long long bk = block_max_key(mine, s.key);
             const int bc = (int)(bk >> 34);
             if (bk != 0 && bc > best) {
                 if (mine == bk) {
@@ -1388,26 +1364,7 @@ __global__ void __launch_bounds__(VT) fransac_kernel(const float* __restrict__ l
             if ((double)h_done >= fmin(need, (double)max_iters)) break;
         }
     }
-    if (best > 0) {
-        int cnt = score_rows<true>(s.H, L1, L2, tent, n, th2, inl, s);   // = best
-        for (int r = 0; r < REFIT_ROUNDS && cnt >= F_REFIT_MIN; r++) {
-            if (!refit_f(L1, L2, tent, n, inl, cnt, s)) break;
-            const int c2 = score_rows<true>(s.Hr, L1, L2, tent, n, th2, nullptr, s);
-            if (c2 < cnt) break;
-            cnt = c2;
-            if (tid < 9) s.H[tid] = s.Hr[tid];
-            __syncthreads();
-            score_rows<true>(s.H, L1, L2, tent, n, th2, inl, s);
-        }
-        best = cnt;
-    } else {
-        for (int t = tid; t < n; t += VT) inl[t] = 0;
-    }
-    if (tid < 9) Fout[(size_t)p * 9 + tid] = best > 0 ? (float)s.H[tid] : 0.f;
-    if (tid == 0) {
-        ninl[p] = best;
-        if (iters) iters[p] = h_done;
-    }
+    finish_ransac<true>(L1, L2, tent, n, th2, best, h_done, inl, s, Fout, ninl, iters);
 }
 
 // ---- homography RANSAC from two affine correspondences (ag_homography_ransac_affine) -------------------------------------------------
@@ -1536,12 +1493,7 @@ __device__ bool ac_homography(const AcRow (&a)[2], double* H) {
         b[i] = t / dg[i];
     }
     const double Hn[9] = {b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7], 1.0};
-    const double T1[9] = {s1, 0.0, -(s1 * c1x), 0.0, s1, -(s1 * c1y), 0.0, 0.0, 1.0};
-    const double T2i[9] = {1.0 / s2, 0.0, c2x, 0.0, 1.0 / s2, c2y, 0.0, 0.0, 1.0};
-    double tmp[9];
-    mul3(T2i, Hn, tmp);
-    mul3(tmp, T1, H);
-    return normalise_h(H);
+    return denormalise_h({c1x, c1y, s1, c2x, c2y, s2}, Hn, H);
 }
 
 // The local optimisation of a chunk's winner (in s.H and Hl, shared) that raised the so-far-best count: the refit rounds on s.H, and
@@ -1553,7 +1505,7 @@ __device__ int ac_local_opt(const float* L1, const float* L2, const int* tent, i
     double f = LO_FACTOR;
     for (int k = 0; k < LO_STEPS; k++) {
         const int c = score_rows<false, true>(Hl, L1, L2, tent, n, th2 * (f * f), inl, s, laf_th * f);
-        if (c < 4 || !refit(L1, L2, tent, n, inl, c, s)) break;   // c is the block total: uniform
+        if (c < 4 || !refit(L1, L2, tent, n, inl, s)) break;   // c is the block total: uniform
         if (threadIdx.x < 9) Hl[threadIdx.x] = s.Hr[threadIdx.x];
         __syncthreads();
         f = f * 0.5;
@@ -1575,37 +1527,25 @@ __global__ void __launch_bounds__(VT) ac_ransac_kernel(const float* __restrict__
     __shared__ RansacShared s;
     __shared__ double Hl[9];   // ac_local_opt's second model
     AcRow* tile = reinterpret_cast<AcRow*>(s.tile);
-    const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    int i, j;
-    const int n = pair_tentatives(pairs, p, S1, S2, ntent, tcap, i, j);
-    const int* tent = tent_all + (size_t)p * tcap * 2;
-    if (n < 0 || !rows_in_range(tent, n, cap1, cap2)) {
-        if (tid == 0) ninl[p] = -1;
-        return;
-    }
-    const float* L1 = lafs1 + (size_t)i * cap1 * 6;
-    const float* L2 = lafs2 + (size_t)j * cap2 * 6;
-    unsigned char* inl = inl_all + (size_t)p * tcap;
+    const int tid = threadIdx.x;
+    const int* tent;
+    const float *L1, *L2;
+    int n;
+    if (!verify_pair(lafs1, S1, cap1, lafs2, S2, cap2, pairs, tent_all, ntent, tcap, ninl, n, tent, L1, L2)) return;
+    unsigned char* inl = inl_all + (size_t)blockIdx.x * tcap;
     int best = 0, h_done = 0;
     if (n >= 2) {
         const int ntiles = (n + ATILE - 1) / ATILE;
         for (int h0 = 0;; h0 += VT) {
             const int h = h0 + tid;
             double H[9], G[9];
-            bool ok = h < max_iters;
+            int idx[2];
+            bool ok = h < max_iters && draw_sample(seed, h, n, idx);
             if (ok) {
-                int idx[2], got = 0;
-                for (int d = 0; d < MAX_DRAWS && got < 2; d++) {
-                    const int v = draw_index(seed, h, d, n);
-                    if (got == 0 || v != idx[0]) idx[got++] = v;
-                }
-                ok = got == 2;
-                if (ok) {
-                    const AcRow a[2] = {tent_ac(L1, L2, tent, idx[0]), tent_ac(L1, L2, tent, idx[1])};
-                    ok = ac_homography(a, H);
-                }
-                if (ok) adj3(H, G);
+                const AcRow a[2] = {tent_ac(L1, L2, tent, idx[0]), tent_ac(L1, L2, tent, idx[1])};
+                ok = ac_homography(a, H);
             }
+            if (ok) adj3(H, G);
             int cnt = 0;
             for (int tb = 0; tb < ntiles; tb++) {
                 const int t0 = tb * ATILE, m = min(ATILE, n - t0);
@@ -1619,17 +1559,7 @@ __global__ void __launch_bounds__(VT) ac_ransac_kernel(const float* __restrict__
             }
             // best of the chunk: highest count, then lowest h
             const unsigned long long mine = ok ? ((unsigned long long)cnt << 32) | (unsigned)~(unsigned)h : 0ull;
-            unsigned long long key = mine;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const unsigned long long k2 = __shfl_xor_sync(0xffffffffu, key, o);
-                key = k2 > key ? k2 : key;
-            }
-            if (lane == 0) s.key[warp] = key;
-            __syncthreads();
-            unsigned long long bk = 0;
-#pragma unroll
-            for (int w = 0; w < VT / 32; w++) bk = s.key[w] > bk ? s.key[w] : bk;
+            const unsigned long long bk = block_max_key(mine, s.key);
             const int bc = (int)(bk >> 32);
             if (bk != 0 && bc > best) {
                 if (mine == bk) {
@@ -1650,14 +1580,7 @@ __global__ void __launch_bounds__(VT) ac_ransac_kernel(const float* __restrict__
             if ((double)h_done >= fmin(need, (double)max_iters)) break;
         }
     }
-    if (best > 0) best = refit_rounds<false, true>(L1, L2, tent, n, th2, inl, s.H, s, laf_th);
-    else
-        for (int t = tid; t < n; t += VT) inl[t] = 0;
-    if (tid < 9) Hout[(size_t)p * 9 + tid] = best > 0 ? (float)s.H[tid] : 0.f;
-    if (tid == 0) {
-        ninl[p] = best;
-        if (iters) iters[p] = h_done;
-    }
+    finish_ransac<false, true>(L1, L2, tent, n, th2, best, h_done, inl, s, Hout, ninl, iters, laf_th);
 }
 
 int verify_args(const char* fn, const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
@@ -1672,6 +1595,34 @@ int verify_args(const char* fn, const float* d_lafs1, int S1, int cap1, const fl
     return AG_ERR_INVALID;
 }
 
+// The RANSAC entry points' outputs and search parameters (M: the model output, H or F).
+int ransac_args(const char* fn, const float* d_M, const unsigned char* d_inl, const int* d_ninl, float inl_th, float confidence,
+                int max_iters) {
+    const char* msg = nullptr;
+    if (!d_M || !d_inl || !d_ninl) msg = "NULL output";
+    else if (!(inl_th > 0.f && isfinite(inl_th))) msg = "inl_th must be finite and > 0";
+    else if (!(confidence > 0.f && confidence < 1.f)) msg = "confidence must be in (0, 1)";
+    else if (!(max_iters >= 1 && max_iters <= 0x7fffffff - VT)) msg = "max_iters must be >= 1";
+    if (!msg) return AG_OK;
+    set_error("%s: %s", fn, msg);
+    return AG_ERR_INVALID;
+}
+
+// ag_fundamental_ransac (DEGEN false) and ag_fundamental_degensac, named fn.
+template <bool DEGEN>
+int fundamental_ransac(const char* fn, const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
+                       const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
+                       float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
+    int rc = verify_args(fn, d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc || (rc = ransac_args(fn, d_F, d_inl, d_ninl, inl_th, confidence, max_iters))) return rc;
+    const double th = inl_th;
+    fransac_kernel<DEGEN><<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
+                                                              log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_F, d_inl, d_ninl,
+                                                              d_iters);
+    AG_CHECK_LAUNCH(DEGEN ? "fransac_kernel<DEGEN>" : "fransac_kernel");
+    return AG_OK;
+}
+
 }  // namespace ag
 
 using namespace ag;
@@ -1681,12 +1632,9 @@ extern "C" {
 int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                          const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
                          float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
-    int rc = verify_args("ag_homography_ransac", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
-    if (rc) return rc;
-    AG_REQUIRE(d_H && d_inl && d_ninl, "NULL output");
-    AG_REQUIRE(inl_th > 0.f && isfinite(inl_th), "inl_th must be finite and > 0");
-    AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
-    AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
+    const char* fn = "ag_homography_ransac";
+    int rc = verify_args(fn, d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc || (rc = ransac_args(fn, d_H, d_inl, d_ninl, inl_th, confidence, max_iters))) return rc;
     const double th = inl_th;
     ransac_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
                                                       log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_H, d_inl, d_ninl, d_iters);
@@ -1697,13 +1645,10 @@ int ag_homography_ransac(const float* d_lafs1, int S1, int cap1, const float* d_
 int ag_homography_ransac_affine(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                                 const int* d_tent, const int* d_ntent, int tcap, float inl_th, float laf_th, float confidence, int max_iters,
                                 unsigned long long seed, float* d_H, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
-    int rc = verify_args("ag_homography_ransac_affine", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
-    if (rc) return rc;
-    AG_REQUIRE(d_H && d_inl && d_ninl, "NULL output");
-    AG_REQUIRE(inl_th > 0.f && isfinite(inl_th), "inl_th must be finite and > 0");
+    const char* fn = "ag_homography_ransac_affine";
+    int rc = verify_args(fn, d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
+    if (rc || (rc = ransac_args(fn, d_H, d_inl, d_ninl, inl_th, confidence, max_iters))) return rc;
     AG_REQUIRE(laf_th > 0.f, "laf_th must be > 0 (and not NaN)");
-    AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
-    AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
     const double th = inl_th;
     ac_ransac_kernel<<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
                                                          (double)laf_th, log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_H, d_inl,
@@ -1715,35 +1660,15 @@ int ag_homography_ransac_affine(const float* d_lafs1, int S1, int cap1, const fl
 int ag_fundamental_ransac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                           const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
                           float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
-    int rc = verify_args("ag_fundamental_ransac", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
-    if (rc) return rc;
-    AG_REQUIRE(d_F && d_inl && d_ninl, "NULL output");
-    AG_REQUIRE(inl_th > 0.f && isfinite(inl_th), "inl_th must be finite and > 0");
-    AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
-    AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
-    const double th = inl_th;
-    fransac_kernel<false><<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
-                                                              log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_F, d_inl, d_ninl,
-                                                              d_iters);
-    AG_CHECK_LAUNCH("fransac_kernel");
-    return AG_OK;
+    return fundamental_ransac<false>("ag_fundamental_ransac", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap, inl_th,
+                                     confidence, max_iters, seed, d_F, d_inl, d_ninl, d_iters, stream);
 }
 
 int ag_fundamental_degensac(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,
                             const int* d_tent, const int* d_ntent, int tcap, float inl_th, float confidence, int max_iters, unsigned long long seed,
                             float* d_F, unsigned char* d_inl, int* d_ninl, int* d_iters, void* stream) {
-    int rc = verify_args("ag_fundamental_degensac", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap);
-    if (rc) return rc;
-    AG_REQUIRE(d_F && d_inl && d_ninl, "NULL output");
-    AG_REQUIRE(inl_th > 0.f && isfinite(inl_th), "inl_th must be finite and > 0");
-    AG_REQUIRE(confidence > 0.f && confidence < 1.f, "confidence must be in (0, 1)");
-    AG_REQUIRE(max_iters >= 1 && max_iters <= 0x7fffffff - VT, "max_iters must be >= 1");
-    const double th = inl_th;
-    fransac_kernel<true><<<P, VT, 0, (cudaStream_t)stream>>>(d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, d_tent, d_ntent, tcap, th * th,
-                                                             log(1.0 - (double)confidence), max_iters, (uint64_t)seed, d_F, d_inl, d_ninl,
-                                                             d_iters);
-    AG_CHECK_LAUNCH("fransac_kernel<DEGEN>");
-    return AG_OK;
+    return fundamental_ransac<true>("ag_fundamental_degensac", d_lafs1, S1, cap1, d_lafs2, S2, cap2, d_pairs, P, d_tent, d_ntent, tcap, inl_th,
+                                    confidence, max_iters, seed, d_F, d_inl, d_ninl, d_iters, stream);
 }
 
 int ag_gt_correspondences_pairs(const float* d_lafs1, int S1, int cap1, const float* d_lafs2, int S2, int cap2, const int* d_pairs, int P,

@@ -11,7 +11,7 @@ import math
 
 import numpy as np
 
-from oracle_ransac import REFIT_ROUNDS, VT, adj3, draw_indices, inliers, mul3, normalise_h, refit
+from oracle_ransac import REFIT_ROUNDS, VT, adj3, inliers, mul3, normalise_h, refit, samples
 
 CHOL_EPS = 1e-10      # a Cholesky pivot <= CHOL_EPS times its diagonal entry is a degenerate sample
 LO_FACTOR = 16.0           # shrinking_lo's first threshold factor (halved at each refit)
@@ -23,15 +23,6 @@ def ac_rows(lafs1, lafs2):
     l1 = np.asarray(lafs1, np.float32).reshape(-1, 6)
     l2 = np.asarray(lafs2, np.float32).reshape(-1, 6)
     return np.concatenate([l1[:, [2, 5]], l2[:, [2, 5]], l1[:, [0, 1, 3, 4]], l2[:, [0, 1, 3, 4]]], 1)
-
-
-def samples2(seed, h, n):
-    """-> (idx [len(h),2] int64, ok [len(h)]): the first 2 distinct draws of each hypothesis (ok False when 64 draws give fewer)."""
-    dr = draw_indices(seed, h, n).astype(np.int64)
-    other = dr != dr[:, :1]
-    pos = np.argmax(other, axis=1)
-    r = np.arange(len(dr))
-    return np.stack([dr[:, 0], dr[r, pos]], 1), other.any(axis=1)
 
 
 def ac_homographies(s):
@@ -190,7 +181,7 @@ def ransac_ac(ac, inl_th=2.0, laf_th=2.0, confidence=0.99, max_iters=50000, seed
         h0 = 0
         while True:
             h = np.arange(h0, h0 + VT)
-            idx, ok = samples2(seed, h, n)
+            idx, ok = samples(seed, h, n, 2)
             ok &= h < max_iters
             Hs, okh = ac_homographies(ac[idx])
             ok &= okh

@@ -172,7 +172,7 @@ def degensac_f(pts, inl_th=0.5, confidence=0.99, max_iters=50000, seed=0, trace=
         h0 = 0
         while search:
             h = np.arange(h0, h0 + VT)
-            idx, ok = samples(seed, h, n)
+            idx, ok = samples(seed, h, n, F_SAMPLE)
             ok &= h < max_iters
             c = pts[idx]                                                    # [VT,7,4]
             ok &= np.isfinite(c).all(axis=(1, 2))

@@ -8,26 +8,12 @@ import math
 
 import numpy as np
 
-from oracle_ransac import JACOBI_SWEEPS, MAX_DRAWS, REFIT_ROUNDS, VT, adj3, block_sum, draw_indices, mul3, splitmix64  # noqa: F401
+from oracle_ransac import JACOBI_SWEEPS, MAX_DRAWS, REFIT_ROUNDS, VT, adj3, block_sum, draw_indices, mul3, samples, splitmix64  # noqa: F401
 
 F_SAMPLE = 7
 F_REFIT_MIN = 8
 PIVOT_EPS = 1e-9
 BISECT_STEPS = 1100   # enough to close any bracket in the double range; the bisection stops once the midpoint is an end
-
-
-def samples(seed, h, n, k=F_SAMPLE):
-    """-> (idx [len(h),k] int64, ok [len(h)]): the first k distinct draws of each hypothesis (ok False when 64 draws give fewer)."""
-    dr = draw_indices(seed, h, n).astype(np.int64)
-    eq = dr[:, :, None] == dr[:, None, :]
-    first = ~np.tril(eq, -1).any(axis=2)
-    rank = np.cumsum(first, axis=1)
-    ok = rank[:, -1] >= k
-    idx = np.zeros((len(dr), k), dtype=np.int64)
-    for q in range(k):
-        pos = np.argmax(first & (rank == q + 1), axis=1)
-        idx[:, q] = dr[np.arange(len(dr)), pos]
-    return idx, ok
 
 
 def cubic_roots(a3, a2, a1, a0):
@@ -312,7 +298,7 @@ def ransac_f(pts, inl_th=0.5, confidence=0.99, max_iters=50000, seed=0):
         h0 = 0
         while search:
             h = np.arange(h0, h0 + VT)
-            idx, ok = samples(seed, h, n)
+            idx, ok = samples(seed, h, n, F_SAMPLE)
             ok &= h < max_iters
             c = pts[idx]                                                    # [VT,7,4]
             ok &= np.isfinite(c).all(axis=(1, 2))

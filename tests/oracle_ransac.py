@@ -35,17 +35,18 @@ def draw_indices(seed, h, n):
     return ((r >> np.uint64(32)) * np.uint64(n)) >> np.uint64(32)
 
 
-def samples(seed, h, n):
-    """-> (idx [len(h),4] int64, ok [len(h)]): the first 4 distinct draws of each hypothesis (ok False when 64 draws give fewer)."""
+def samples(seed, h, n, k=4):
+    """-> (idx [len(h),k] int64, ok [len(h)]): the first k distinct draws of each hypothesis (ok False when 64 draws give fewer),
+    verify.cu's draw_sample<k>."""
     dr = draw_indices(seed, h, n).astype(np.int64)
     eq = dr[:, :, None] == dr[:, None, :]                                   # [H, d, e]
     first = ~np.tril(eq, -1).any(axis=2)                                    # draw d differs from every earlier draw
     rank = np.cumsum(first, axis=1)
-    ok = rank[:, -1] >= 4
-    idx = np.zeros((len(dr), 4), dtype=np.int64)
-    for k in range(4):
-        pos = np.argmax(first & (rank == k + 1), axis=1)
-        idx[:, k] = dr[np.arange(len(dr)), pos]
+    ok = rank[:, -1] >= k
+    idx = np.zeros((len(dr), k), dtype=np.int64)
+    for q in range(k):
+        pos = np.argmax(first & (rank == q + 1), axis=1)
+        idx[:, q] = dr[np.arange(len(dr)), pos]
     return idx, ok
 
 

@@ -219,7 +219,7 @@ def test_pivot_scene_is_rejected_by_the_pivot_rule_only():
     Cholesky applies, and with the relative pivot threshold at 0 a large share of them solves (the rest have a pivot <= 0)."""
     l1, l2 = AC.pivot_scene(11, 64)
     ac = A.ac_rows(l1, l2).astype(np.float64)
-    idx, ok = A.samples2(0, np.arange(1024), len(ac))
+    idx, ok = R.samples(0, np.arange(1024), len(ac), 2)
     assert ok.all() and np.isfinite(ac).all()
     s = ac[idx]
     d1 = s[..., 4] * s[..., 7] - s[..., 5] * s[..., 6]
@@ -240,7 +240,7 @@ def test_local_optimisation_lifts_a_noisy_winner():
     """On a constructed scene the shrinking-threshold refits start from the chunk's winner and never end below the refit rounds."""
     l1, l2, Hm, kind = AC.scene(40, 600, outliers=0.6, eps=0.15)
     ac = A.ac_rows(l1, l2).astype(np.float64)
-    idx, ok = A.samples2(0, np.arange(256), len(ac))
+    idx, ok = R.samples(0, np.arange(256), len(ac), 2)
     Hs, okh = A.ac_homographies(ac[idx])
     th2 = 4.0
     for k in np.nonzero(ok & okh)[0][:40]:
